@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the RAVE waveform hot path on B200.
+"""bench.py -- headline benchmark of the RAVE waveform hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W          # our arm (N>1 under torchrun)
     python bench.py --impl reference ...                   # the reference's CPU arithmetic (oracle port)
@@ -11,7 +11,7 @@ One "step" = one `RAVE.training_step` in phase 2, following the reference's sche
 whole 4-step cycles' worth of alternation starting at batch_idx 0.
 
 Prints ONE JSON line (rank 0).  Keys: see the task contract; `roofline` is for the kernel instance with the
-largest share of the step's tcgen05 time on its most expensive layer (timed alone, CUDA events, rotating
+largest share of the step's tensor-core time on its most expensive layer (timed alone, CUDA events, rotating
 buffers > L2), `step_roofline` = Sigma of per-launch rooflines / measured step, `forward_pqmf_enc_gen` the
 north-star forward (CUDA-graph replay; bf16 and the accurate bf16x3 mode), `stock_cudnn_tf32` the same step
 through stock torch/cuDNN TF32 on this GPU (the reference's own GPU path), `cpu_baseline` the oracle port on
@@ -50,7 +50,25 @@ def parse():
     ap.add_argument("--cpu-seconds", type=float, default=20.0)
     ap.add_argument("--quick", action="store_true", help="timed region only (parameter sweeps): no roofline / forward / "
                                                          "baseline sections")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed (its logged losses, a fixed sample of the updated "
+                         "parameters) as DIR/<name>.npy")
     return ap.parse_args()
+
+
+def dump_outputs(out_dir, logs, model, n_sample=1 << 16):
+    """What the last timed step computed: every logged value it returned (one float64 .npy each) and a fixed, seeded
+    sample of n_sample elements of the parameters it updated (param_sample.npy, float32, named-parameter order)."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, v in sorted(logs.items()):
+        a = v.detach().double().cpu().numpy() if hasattr(v, "detach") else np.asarray(v, dtype=np.float64)
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+    flat = torch.cat([p.detach().reshape(-1).float() for _, p in model.named_parameters()])
+    g = torch.Generator().manual_seed(0)
+    idx = torch.randperm(flat.numel(), generator=g)[:n_sample].sort().values
+    np.save(os.path.join(out_dir, "param_sample.npy"), flat[idx.to(flat.device)].cpu().numpy())
 
 
 def peaks():
@@ -59,11 +77,12 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"],
                     bf16_tflops_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16 -- bounds, not reached rates
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler(threading.Thread):
-    """SM clock + throttle reasons during the timed region (B200_PROFILING.md): NVML, else nvidia-smi."""
+    """SM clock + throttle reasons during the timed region: NVML, else nvidia-smi."""
 
     def __init__(self, index=0):
         super().__init__(daemon=True)
@@ -298,7 +317,7 @@ def run_reference(args):
 
 def profile_step(torch, model, x, pk):
     """One eager G-step and one eager D-step with every library call timed ALONE (sync + CUDA events: _lib.PROFILE).
-    Returns per kind: the launches, Sigma of their rooflines, and the tcgen05 launch shape with the largest total time."""
+    Returns per kind: the launches, Sigma of their rooflines, and the tensor-core launch shape with the largest total time."""
     from rave_b200 import _lib, roofline
     peak_f, peak_b = pk["bf16_tflops"] * 1e12, pk["hbm_gbs"] * 1e9
     out = {}
@@ -328,7 +347,7 @@ def profile_step(torch, model, x, pk):
 
 
 def _disc_on_engine(disc, x_dev):
-    """True when every sub-discriminator runs as tcgen05 chains: the v2 nets through the fused feature-matching path, the
+    """True when every sub-discriminator runs as tensor-core chains: the v2 nets through the fused feature-matching path, the
     Descript MPDs as one chain each and the MRD convs as one-layer chains (rave_b200/descript_discriminator.py)."""
     if hasattr(disc, "supports_fused_fm"):
         return bool(disc.supports_fused_fm(x_dev))
@@ -347,7 +366,7 @@ def _disc_on_engine(disc, x_dev):
 
 
 def dominant_launch_roofline(torch, prof, pk):
-    """`roofline`: the tcgen05 launch shape with the largest share of the step (3 G-steps + 1 D-step per cycle),
+    """`roofline`: the tensor-core launch shape with the largest share of the step (3 G-steps + 1 D-step per cycle),
     re-timed alone over rotating buffers (> L2), against max(bytes / HBM, flops / tensor) of THAT launch."""
     from rave_b200 import _lib, ops
     tot = {}
@@ -362,7 +381,7 @@ def dominant_launch_roofline(torch, prof, pk):
         if name != "rave_conv1d_tc_fwd":
             return name
         v = _lib.load().rave_conv1d_tc_plan(ints[0], ints[1], ints[4], ints[5], ints[6])
-        return f"conv_tc{'2' if v >> 24 else ''}_kernel<{v & 0xfff},{(v >> 12) & 0xfff}>"
+        return f"conv_tc_kernel<{v & 0xfff},{(v >> 12) & 0xfff}>"
     by_inst = {}
     for key, v in tot.items():
         by_inst.setdefault(instance(key), []).append((v[0], key))
@@ -371,7 +390,7 @@ def dominant_launch_roofline(torch, prof, pk):
     ms_layer, key = max(members)
     name, ints, ptrs = key
     fl, by = tot[key][2]
-    res = dict(kernel=inst, kernel_share_of_tcgen05_time=share, layer=dict(entry=name, ints=list(ints), ptrs=ptrs),
+    res = dict(kernel=inst, kernel_share_of_tc_time=share, layer=dict(entry=name, ints=list(ints), ptrs=ptrs),
                algorithmic_bytes=by, algorithmic_flops=fl)
     if name != "rave_conv1d_tc_fwd":
         res.update(bound=None, note="dominant launch is not a conv_tc forward-form launch; timed in situ only")
@@ -423,20 +442,6 @@ def dominant_launch_roofline(torch, prof, pk):
         ach, peak, unit = fl / (ms * 1e-3) / 1e12, pk["bf16_tflops"], "TFLOP/s"
     res.update(bound=bound, achieved=ach, peak=peak, unit=unit, frac=ach / peak, traffic=None,
                ms_per_launch=ms, peak_source=pk["source"] + " burst", timing=f"{n} launches over {nb} rotating buffer sets")
-    # DRAM bytes of the same launch from the committed `ncu --set full` capture (scripts/ncu_dominant.py -> ncu_traffic.py)
-    try:
-        import json as _json
-        tf = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r2_ncu_traffic.json")
-        if os.path.exists(tf):
-            for k, v in _json.load(open(tf)).items():
-                kk = k.replace(" ", "")
-                kk = kk[:kk.rfind(",")] + ">" if kk.count(",") == 2 else kk          # drop the X3 template flag
-                if kk == inst and (Bc, Cin, Lin, Cout, Lout, K, stride) == (64, 192, 4096, 384, 1024, 15, 4):
-                    res["traffic"] = v["traffic_bytes"]
-                    res["traffic_source"] = ("profiles/r2_ncu_traffic.json: dram__bytes_read.sum + dram__bytes_write.sum per "
-                                             f"launch, ncu --set full of this launch shape ({v['launches']} launches)")
-    except Exception:
-        pass
     return res
 
 
@@ -447,7 +452,7 @@ def forward_roofline(torch, model, x_dev, pk, modes=("bf16", "bf16x3")):
 
     Forward-only means inference / validation: the parameters do not move between replays, so the weight-normalised,
     tap-major bf16 layouts are prepared ONCE into persistent buffers (engine.enable_static_prep) instead of by every replay
-    (mt_rownorm + mt_prep were 273 us of a 1165 us replay: profiles/r2_trace_forward_bf16.txt).  `ms` is that graph;
+    `ms` is that graph;
     `ms_with_weight_prep` the same graph with the per-replay preparation left in (what a training step's forward pays)."""
     import rave_b200
     from rave_b200 import engine
@@ -579,7 +584,7 @@ def run_ours(args):
         model.on_train_batch_end()
     barrier()
 
-    # which parts actually ran on the tcgen05 engine
+    # which parts actually ran on the tensor-core engine
     on_engine = None
     try:
         if prec == "bf16" and model is not None:
@@ -598,12 +603,15 @@ def run_ours(args):
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     barrier()
     e0.record()
+    logs = None
     for i in range(args.steps):
-        step(i, x_dev if i % 2 == 0 else x_dev2)
+        logs = step(i, x_dev if i % 2 == 0 else x_dev2)
         model.on_train_batch_end()
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0 and logs is not None:
+        dump_outputs(args.dump_outputs, logs, model)
     launches = _lib.launch_count() - n0
     if trainer is not None:      # replayed launches do not pass through the library's counter
         launches += sum(trainer.launches[model.is_discriminator_step(i)] for i in range(args.steps))
@@ -664,7 +672,7 @@ def run_ours(args):
                 step_roof = dict(t_min_ms=cyc_roof, ms_per_step=ms / args.steps, frac=cyc_roof / (ms / args.steps),
                                  launches_timed_alone_ms=cyc_alone, frac_alone=cyc_roof / max(cyc_alone, 1e-9),
                                  other_launches_alone_ms=cyc_other,
-                                 note="t_min = Sigma over the tcgen05 conv / wgrad and PQMF launches of one step (3 G : 1 D) of "
+                                 note="t_min = Sigma over the tensor-core conv / wgrad and PQMF launches of one step (3 G : 1 D) of "
                                       "max(bytes / HBM peak, flops / bf16 peak); `frac` divides by the measured step (which also "
                                       "holds the loss / optimiser / layout kernels listed under other_launches_alone_ms), "
                                       "`frac_alone` by the same launches each timed alone")
@@ -693,10 +701,10 @@ def run_ours(args):
             "config": {"workload": f"{args.config} phase-2 training step (PQMF+enc+gen+discriminator, fwd+bwd+Adam; "
                                    f"1 D-step per 4), per-GPU batch {B}x{T} @48kHz",
                        "global_batch": world * B, "samples": T, "parallelism": f"dp{world}",
-                       "precision": ("bf16 operands / fp32 accumulate (tcgen05 engine); PQMF + losses fp32"
+                       "precision": ("bf16 operands / fp32 accumulate (wgmma engine); PQMF + losses fp32"
                                      if prec == "bf16" else "fp32 parity kernels (CUDA-core FMA)"),
-                       "tcgen05_engine": on_engine, "launch": graph_note,
-                       "l2_policy": "working set per step (>10 GB of activations) exceeds the 126 MB L2; "
+                       "tc_engine": on_engine, "launch": graph_note,
+                       "l2_policy": "working set per step (>10 GB of activations) exceeds the 50 MB L2; "
                                     "two alternating input batches"},
             "roofline": roof, "step_roofline": step_roof, "forward_pqmf_enc_gen": fwd, "stock_cudnn_tf32": stock,
             "cpu_baseline": cpu,
@@ -718,6 +726,8 @@ def run_ours(args):
 
 def main():
     args = parse()
+    if args.impl == "reference" and args.dump_outputs:
+        sys.exit("bench.py: --dump-outputs writes the outputs of the GPU path (--impl ours)")
     if args.impl == "reference":
         run_reference(args)
     else:

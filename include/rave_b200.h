@@ -1,5 +1,5 @@
 /*
- * rave_b200 -- C ABI of the B200-native (sm_100a) waveform hot path of acids-ircam/RAVE.
+ * rave_b200 -- C ABI of the H100-native (sm_90a) waveform hot path of acids-ircam/RAVE.
  *
  * The reference has no FFI: its hot path is issued through ATen library calls
  * (F.pad + F.conv1d / F.conv_transpose1d / nn.Conv2d -> cuDNN).  Each entry point below
@@ -33,8 +33,8 @@ extern "C" {
 
 /* precision modes of the tensor-core conv engine */
 #define RAVE_PREC_FP32 0 /* CUDA-core fp32 FMA: parity mode (<=1e-5 rel-L2 vs the fp32 CPU oracle) */
-#define RAVE_PREC_BF16 1 /* tcgen05 kind::f16, bf16 operands, fp32 accumulate in TMEM */
-#define RAVE_PREC_TF32 2 /* tcgen05 kind::tf32, fp32 operands read as tf32 */
+#define RAVE_PREC_BF16 1 /* wgmma, bf16 operands, fp32 accumulate in registers */
+#define RAVE_PREC_TF32 2 /* fp32 operands read as tf32 (no kernel on this path) */
 
 int rave_b200_version(void);
 const char *rave_b200_last_error(void);
@@ -137,9 +137,9 @@ int rave_am_tanh_bwd(const float *dy, const float *x, float *dx, int B, int C, i
 int rave_reparam_fwd(const float *z, const float *eps, float *zs, float *kl_sum, int B, int C, int L, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
- * tensor-core conv engine (tcgen05 + TMEM + TMA), implicit GEMM, time on the MMA M axis:
+ * tensor-core conv engine (wgmma + TMA, register accumulators), implicit GEMM, time on the MMA M axis:
  *   D[(b,l)][co] = sum_k sum_ci A_k[(b,l)][ci] * W_k[co][ci],   A_k = row-shifted view of the input.
- * See DESIGN.md section "tcgen05 conv engine".  Tensors on this path are CHANNEL-LAST:
+ * See DESIGN.md section "wgmma conv engine".  Tensors on this path are CHANNEL-LAST:
  *   xa      [B][Lin][Cin]  bf16 : the ALREADY ACTIVATED operand (written by the previous kernel's epilogue)
  *   wt      [K][Cout][Cin] bf16 : tap-major effective weights (rave_weight_to_tapmajor_bf16)
  *   res     [B][out_rows][Cout] fp32 or NULL (res_bf16: the same in bf16), bias [Cout] or NULL
@@ -162,7 +162,7 @@ int rave_reparam_fwd(const float *z, const float *eps, float *zs, float *kl_sum,
  * ------------------------------------------------------------------------------------------- */
 int rave_conv1d_tc_supported(int Cin, int Cout, int K, int stride, int dil);
 /* Fused Residual(DilatedUnit) forward (rave/blocks.py:31-45, 83-112):  out = x + Conv1x1(LeakyReLU(Conv3_dil(LeakyReLU(x))))
- * in one tcgen05 kernel; the intermediate operand stays in shared memory as the A operand of the second GEMM.
+ * in one wgmma kernel; the intermediate operand stays in shared memory as the A operand of the second GEMM.
  *   xa      [B][pitch][C] bf16 : a = LeakyReLU_{slope_in}(x), the unit's input operand (the skip x is recovered from it)
  *   w3t     [3][C][C] bf16, w1t [1][C][C] bf16 : tap-major effective weights (rave_weight_prep_tc_multi)
  *   a1_out  [B][pitch][C] bf16 or NULL : LeakyReLU_{slope_mid}(conv3) kept for the backward (training)
@@ -173,7 +173,7 @@ int rave_dilated_unit_tc_supported(int C, int L);
 int rave_dilated_unit_tc_fwd(const void *xa_bf16, const void *w3t_bf16, const void *w1t_bf16, void *a1_out,
                              float *out_f32, void *out_act, int B, int C, int L, int pitch, int dil, int pad_l,
                              float slope_in, float slope_mid, int act_out, float slope_out, void *stream);
-/* kernel instance rave_conv1d_tc_fwd selects for a shape: BLOCK_N | BLOCK_K << 12 | (CTA pair ? 1 << 24 : 0), 0 = none
+/* kernel instance rave_conv1d_tc_fwd selects for a shape: BLOCK_N | BLOCK_K << 12, 0 = none
  * (bench.py names the dominant kernel with it) */
 int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K);
 int rave_conv1d_tc_fwd(const void *xa_bf16, const void *wt_bf16, const float *bias, const float *res,
@@ -234,7 +234,7 @@ int rave_leaky_fm_stack_fwd(const float *x, float *a, float *stats, void *xs_bf1
  * feature-matching terms d (nullable)) * LeakyReLU'(a) */
 int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx, long Rh, int T,
                             int F, int C, int Fp, float slope, void *stream);
-/* Snake (rave/blocks.py:852-860) on the engine's channel-last bf16 streams [rows][C] (v3 chains on the tcgen05 kernels):
+/* Snake (rave/blocks.py:852-860) on the engine's channel-last bf16 streams [rows][C] (v3 chains on the wgmma kernels):
  * a = h + sin^2(alpha h) / (alpha + 1e-9);  backward: gh = ga * da/dh + add (add may be null), dalpha[c] += sum_rows
  * ga * da/dalpha (dalpha zeroed by the caller). */
 int rave_snake_cl_fwd(const void *h_bf16, const float *alpha, void *a_bf16, long rows, int C, void *stream);

@@ -1,4 +1,4 @@
-"""rave_b200 -- B200-native (sm_100a) waveform hot path of acids-ircam/RAVE.
+"""rave_b200 -- H100-native (sm_90a) waveform hot path of acids-ircam/RAVE.
 
 The package mirrors the reference's module surface for the path BASELINE.json names
 (`pqmf`, `blocks`, `discriminator`, `descript_discriminator`, `core` losses, `model.RAVE`)

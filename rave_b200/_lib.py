@@ -139,7 +139,7 @@ def launch_count() -> int:
 
 
 PROFILE = None      # set to a list: every call is timed alone (sync + CUDA events) and logged as
-                    # (entry point, integer arguments, milliseconds) -- scripts/profile_layers.py
+                    # (entry point, integer arguments, milliseconds)
 
 
 def call(name: str, *args):

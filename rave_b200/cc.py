@@ -4,7 +4,7 @@ third-party package `cached-conv>=2.5.0` (requirements.txt:14; semantics: SURVEY
 Same names / constructor arguments / attributes as `cached_conv` so the block definitions read
 like the reference's (`cc.Conv1d`, `cc.ConvTranspose1d`, `cc.get_padding`, `cc.CachedSequential`,
 `cc.AlignBranches`, `cc.CachedPadding1d`, `cc.MAX_BATCH_SIZE`, `cc.USE_BUFFER_CONV`,
-`cc.use_cached_conv`), but `forward` launches the sm_100a kernels of librave_b200.so.
+`cc.use_cached_conv`), but `forward` launches the sm_90a kernels of librave_b200.so.
 
 gin is not available: the two gin-configurable knobs the reference's configs bind
 (`cc.Conv1d.bias = False`, configs/v1.gin:33-34; `cc.get_padding.mode = 'causal'`,

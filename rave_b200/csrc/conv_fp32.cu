@@ -297,7 +297,7 @@ __global__ void wgrad_reduce_kernel(const float *__restrict__ part, float *__res
 static int wgrad_splits(int B, int Ca, int Cc, int Lp, int K) {
   const long tiles = (long)ceil_div(Ca, WM) * ceil_div(Cc, WN) * K;
   const long chunks = (long)B * ceil_div(Lp, WK);
-  long want = (148 * 4 + tiles - 1) / tiles;  // ~4 CTAs per SM in flight
+  long want = (132 * 4 + tiles - 1) / tiles;  // ~4 CTAs per SM in flight
   long max_by_work = chunks / 8 > 0 ? chunks / 8 : 1;
   if (want > max_by_work) want = max_by_work;
   if (want < 1) want = 1;
@@ -375,7 +375,7 @@ extern "C" int rave_conv1d_wgrad_f32(const float *P, const float *Q, float *dw, 
   RAVE_CHECK_LAUNCH("conv1d_wgrad_f32");
   const long total = (long)Ca * Cc * K;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   wgrad_reduce_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(a.part, dw, Ca, Cc, K, a.splits, os_a,
                                                                os_c);
   RAVE_CHECK_LAUNCH("wgrad_reduce");

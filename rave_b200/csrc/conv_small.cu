@@ -87,7 +87,7 @@ constexpr int C1_MAXK = 16;
 __global__ void __launch_bounds__(256)
 conv_c1_wgrad_kernel(const __nv_bfloat16 *__restrict__ g, const float *__restrict__ x, float *__restrict__ dwt,
                      int R, int x_pitch, int Lin, int Cout, int Cg, int Lout, int g_pitch, int K, int stride,
-                     int pad_l, int NL) {
+                     int pad_l, int NL, const BlockSum bs) {
   extern __shared__ float red[];   // [NL][K][Cout]
   const int half = Cout >> 1;
   const int c2 = (threadIdx.x % half) * 2;
@@ -137,8 +137,9 @@ conv_c1_wgrad_kernel(const __nv_bfloat16 *__restrict__ g, const float *__restric
   for (int i = threadIdx.x; i < K * Cout; i += blockDim.x) {
     float s = 0.f;
     for (int ln = 0; ln < NL; ++ln) s += red[(size_t)ln * K * Cout + i];
-    atomicAdd(dwt + i, s);                  // [k][co]  (== [1][K][C0p=Cout][C1p=1]), pre-zeroed
+    block_sum_put(bs, i, s);
   }
+  block_sum_finish(bs, dwt);               // [k][co]  (== [1][K][C0p=Cout][C1p=1]), pre-zeroed
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -209,7 +210,8 @@ conv_c1_dgrad_kernel(const __nv_bfloat16 *__restrict__ g, const float *__restric
 
 // column sums of a bf16 channel-last tensor: out[c] = sum_{r, l < L} g[r][l][c]   (conv bias gradient)
 __global__ void __launch_bounds__(256)
-colsum_bf16_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out, int L, int pitch, int Cg, int C) {
+colsum_bf16_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out, int L, int pitch, int Cg, int C,
+                   const BlockSum bs) {
   // grid (slices, R); block 256 = 32 position lanes x 8 channel groups; each thread strides channels
   __shared__ float red[8][33];
   const int r = blockIdx.y;
@@ -228,10 +230,11 @@ colsum_bf16_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out,
       float t = 0.f;
 #pragma unroll
       for (int i = 0; i < 8; ++i) t += red[i][lane_c];
-      atomicAdd(out + c, t);
+      block_sum_put(bs, c, t);
     }
     __syncthreads();
   }
+  block_sum_finish(bs, out);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -241,16 +244,17 @@ colsum_bf16_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ out,
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ float unleaky(float a, float inv_slope) { return a > 0.f ? a : a * inv_slope; }
 __device__ __forceinline__ void ldg256_nc(const void *p, uint32_t *r) {     // 32-byte aligned, read-only
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
+               : "l"(reinterpret_cast<const uint8_t *>(p) + 16));
 }
 
 // grid (blocks per batch entry, Bh): a batch entry's valid rows [L][C] are one contiguous range, so the index is linear
-// (no 64-bit divisions per element); two 256-bit loads per half in flight per thread; packed f32x2 arithmetic.
+// (no 64-bit divisions per element); two 32-byte row pieces per half in flight per thread.
 __global__ void __launch_bounds__(256)
 fm_stats_kernel(const __nv_bfloat16 *__restrict__ a, float *__restrict__ stats, int Bh, int L, int pitch, int C,
-                float inv_slope) {
+                float inv_slope, const BlockSum bs) {
   __shared__ float red0[8], red1[8];
   const long n_vec = (long)L * (C >> 4);                    // 16-channel vectors of one batch entry
   const size_t half = (size_t)Bh * pitch * C;
@@ -275,13 +279,13 @@ fm_stats_kernel(const __nv_bfloat16 *__restrict__ a, float *__restrict__ stats, 
       for (int j = 0; j < 8; ++j) {
         const float2 r = make_float2(bf16_lo(rw[u][j]), bf16_hi(rw[u][j]));
         const float2 f = make_float2(bf16_lo(fw[u][j]), bf16_hi(fw[u][j]));
-        const float2 rs = __fmul2_rn(r, inv2), fs = __fmul2_rn(f, inv2);
+        const float2 rs = make_float2(r.x * inv2.x, r.y * inv2.y), fs = make_float2(f.x * inv2.x, f.y * inv2.y);
         // inverse LeakyReLU (1 / slope >= 1): h = min(a, a / slope)
         const float2 hr = make_float2(fminf(r.x, rs.x), fminf(r.y, rs.y));
         const float2 hf = make_float2(fminf(f.x, fs.x), fminf(f.y, fs.y));
-        const float2 d = __fadd2_rn(hr, make_float2(-hf.x, -hf.y));
-        s0 = __fadd2_rn(s0, make_float2(fabsf(d.x), fabsf(d.y)));
-        s1 = __fadd2_rn(s1, make_float2(fabsf(hr.x), fabsf(hr.y)));
+        const float2 d = make_float2(hr.x - hf.x, hr.y - hf.y);
+        s0 = make_float2(s0.x + fabsf(d.x), s0.y + fabsf(d.y));
+        s1 = make_float2(s1.x + fabsf(hr.x), s1.y + fabsf(hr.y));
       }
     }
   }
@@ -297,9 +301,10 @@ fm_stats_kernel(const __nv_bfloat16 *__restrict__ a, float *__restrict__ stats, 
   if (threadIdx.x == 0) {
     float u0 = 0.f, u1 = 0.f;
     for (int i = 0; i < 8; ++i) { u0 += red0[i]; u1 += red1[i]; }
-    atomicAdd(stats, u0);
-    atomicAdd(stats + 1, u1);
+    block_sum_put(bs, 0, u0);
+    block_sum_put(bs, 1, u1);
   }
+  block_sum_finish(bs, stats);
 }
 
 // gradient of (d0 * S_diff + d1 * S_abs) with respect to h, written as the bf16 gradient stream:
@@ -357,7 +362,7 @@ extern "C" int rave_conv1d_c1_fwd(const float *x, const float *w, const float *b
   RAVE_CHECK_ARG(R <= 65535, "conv1d_c1_fwd: too many rows");
   const int per_row = Lout * (Cout / 8);
   int bx = (per_row + 255) / 256;
-  const int want = (148 * 16 + R - 1) / R;       // ~16 CTAs per SM in total
+  const int want = (132 * 16 + R - 1) / R;       // ~16 CTAs per SM in total
   if (bx > want) bx = want;
   if (bx < 1) bx = 1;
   const size_t smem = (size_t)(K + 1) * Cout * sizeof(float);
@@ -369,7 +374,7 @@ extern "C" int rave_conv1d_c1_fwd(const float *x, const float *w, const float *b
 }
 
 static int c1_wgrad_slices(int R, int Lout) {
-  int sl = (148 * 8 + R - 1) / R;                 // ~8 CTAs per SM in total
+  int sl = (132 * 8 + R - 1) / R;                 // ~8 CTAs per SM in total
   const int max_sl = (Lout + 63) / 64;            // at least 64 positions per slice
   if (sl > max_sl) sl = max_sl;
   if (sl < 1) sl = 1;
@@ -394,8 +399,11 @@ extern "C" int rave_conv1d_c1_wgrad(const void *g_bf16, const float *x, float *d
   const size_t smem = (size_t)NL * K * Cout * sizeof(float);
   RAVE_CHECK_ARG(smem <= 48 * 1024, "conv1d_c1_wgrad: reduction buffer too large");
   cudaMemsetAsync(dwt, 0, sizeof(float) * K * Cout, (cudaStream_t)stream);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, (long)slices * R, K * Cout, (cudaStream_t)stream)) return rc;
   conv_c1_wgrad_kernel<<<dim3(slices, R), threads, smem, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16 *)g_bf16, x, dwt, R, x_pitch, Lin, Cout, Cg, Lout, g_pitch, K, stride, pad_l, NL);
+      (const __nv_bfloat16 *)g_bf16, x, dwt, R, x_pitch, Lin, Cout, Cg, Lout, g_pitch, K, stride, pad_l, NL, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("conv1d_c1_wgrad");
   return 0;
 }
@@ -423,11 +431,14 @@ extern "C" int rave_colsum_bf16(const void *g_bf16, float *out, int R, int L, in
   RAVE_CHECK_ARG(g_bf16 && out && R > 0 && R <= 65535 && L > 0 && pitch >= L && C > 0 && Cg >= C,
                  "colsum_bf16: bad argument");
   cudaMemsetAsync(out, 0, sizeof(float) * C, (cudaStream_t)stream);
-  int sl = (148 * 8 + R - 1) / R;
+  int sl = (132 * 8 + R - 1) / R;
   const int max_sl = (L + 63) / 64;
   if (sl > max_sl) sl = max_sl;
   if (sl < 1) sl = 1;
-  colsum_bf16_kernel<<<dim3(sl, R), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)g_bf16, out, L, pitch, Cg, C);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, (long)sl * R, C, (cudaStream_t)stream)) return rc;
+  colsum_bf16_kernel<<<dim3(sl, R), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)g_bf16, out, L, pitch, Cg, C, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("colsum_bf16");
   return 0;
 }
@@ -441,11 +452,14 @@ extern "C" int rave_fm_stats(const void *a_bf16, float *stats, int Bh, int L, in
   RAVE_CHECK_ARG(Bh <= 65535, "fm_stats: %d batch entries per half > 65535", Bh);
   const long per_b = (long)L * (C / 16);
   long bx = (per_b + 511) / 512;                     // two vectors per thread and pass
-  const long cap = (148L * 8 + Bh - 1) / Bh;         // ~8 blocks per SM over the whole grid
+  const long cap = (132L * 8 + Bh - 1) / Bh;         // ~8 blocks per SM over the whole grid
   if (bx > cap) bx = cap;
   if (bx < 1) bx = 1;
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, bx * Bh, 2, (cudaStream_t)stream)) return rc;
   fm_stats_kernel<<<dim3((unsigned)bx, (unsigned)Bh), 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)a_bf16, stats,
-                                                                                    Bh, L, pitch, C, 1.f / slope);
+                                                                                    Bh, L, pitch, C, 1.f / slope, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("fm_stats");
   return 0;
 }
@@ -458,7 +472,7 @@ extern "C" int rave_fm_grad(const void *a_bf16, const float *dstats, void *gout_
                  "fm_grad: bad argument");
   const long total = (long)Bh * pitch * (C / 8);
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   fm_grad_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)a_bf16, dstats,
                                                                 (__nv_bfloat16 *)gout_bf16, Bh, L, pitch, C,
                                                                 1.f / slope);
@@ -480,7 +494,8 @@ extern "C" int rave_fm_grad(const void *a_bf16, const float *dstats, void *gout_
 namespace rave {
 
 __global__ void __launch_bounds__(256)
-score_stats_kernel(const float *__restrict__ s, float *__restrict__ stats, int Bh, int L, int pitch, int C) {
+score_stats_kernel(const float *__restrict__ s, float *__restrict__ stats, int Bh, int L, int pitch, int C,
+                   const BlockSum bs) {
   __shared__ float red[6][8];
   const long total = (long)Bh * L;
   const size_t half = (size_t)Bh * pitch * C;
@@ -508,8 +523,9 @@ score_stats_kernel(const float *__restrict__ s, float *__restrict__ stats, int B
   if (threadIdx.x < 6) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[threadIdx.x][i];
-    atomicAdd(stats + threadIdx.x, t);
+    block_sum_put(bs, threadIdx.x, t);
   }
+  block_sum_finish(bs, stats);
 }
 
 __global__ void __launch_bounds__(256)
@@ -547,8 +563,11 @@ extern "C" int rave_score_stats(const float *score, float *stats, int Bh, int L,
   using namespace rave;
   RAVE_CHECK_ARG(score && stats && Bh > 0 && L > 0 && pitch >= L && C > 0, "score_stats: bad argument");
   long blocks = ((long)Bh * L + 255) / 256;
-  if (blocks > 148 * 4) blocks = 148 * 4;
-  score_stats_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(score, stats, Bh, L, pitch, C);
+  if (blocks > 132 * 4) blocks = 132 * 4;
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 6, (cudaStream_t)stream)) return rc;
+  score_stats_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(score, stats, Bh, L, pitch, C, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("score_stats");
   return 0;
 }
@@ -559,7 +578,7 @@ extern "C" int rave_score_grad(const float *score, const float *dstats, void *go
   RAVE_CHECK_ARG(score && dstats && gout_bf16 && Bh > 0 && L > 0 && pitch >= L && C > 0 && C % 8 == 0,
                  "score_grad: bad argument");
   long blocks = ((long)Bh * pitch + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   score_grad_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(score, dstats, (__nv_bfloat16 *)gout_bf16, Bh, L,
                                                                    pitch, C);
   RAVE_CHECK_LAUNCH("score_grad");
@@ -757,7 +776,7 @@ namespace rave {
 
 __global__ void __launch_bounds__(256)
 l1_stats_f32_kernel(const float *__restrict__ t, const float *__restrict__ v, float *__restrict__ stats, long n,
-                    int vec) {
+                    int vec, const BlockSum bs) {
   __shared__ float red0[8], red1[8];
   float s0 = 0.f, s1 = 0.f;
   if (!vec) {           // operands not 16-byte aligned (odd-sized slices): scalar pass
@@ -790,9 +809,10 @@ l1_stats_f32_kernel(const float *__restrict__ t, const float *__restrict__ v, fl
   if (threadIdx.x == 0) {
     float u0 = 0.f, u1 = 0.f;
     for (int i = 0; i < 8; ++i) { u0 += red0[i]; u1 += red1[i]; }
-    atomicAdd(stats, u0);
-    atomicAdd(stats + 1, u1);
+    block_sum_put(bs, 0, u0);
+    block_sum_put(bs, 1, u1);
   }
+  block_sum_finish(bs, stats);
 }
 
 __device__ __forceinline__ float sgnf(float x) { return (x > 0.f ? 1.f : 0.f) - (x < 0.f ? 1.f : 0.f); }
@@ -817,9 +837,12 @@ extern "C" int rave_l1_stats_f32(const float *t, const float *v, float *stats, l
   RAVE_CHECK_ARG(t && v && stats && n > 0, "l1_stats: bad argument");
   const int vec = ((((uintptr_t)t | (uintptr_t)v) & 15) == 0) ? 1 : 0;
   long blocks = ((vec ? (n >> 2) : n) + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   if (blocks < 1) blocks = 1;
-  l1_stats_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(t, v, stats, n, vec);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 2, (cudaStream_t)stream)) return rc;
+  l1_stats_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(t, v, stats, n, vec, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("l1_stats");
   return 0;
 }
@@ -829,7 +852,7 @@ extern "C" int rave_l1_grad_f32(const float *t, const float *v, const float *d, 
   using namespace rave;
   RAVE_CHECK_ARG(t && v && d && (gt || gv) && n > 0, "l1_grad: bad argument");
   long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   l1_grad_f32_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(t, v, d, gt, gv, n);
   RAVE_CHECK_LAUNCH("l1_grad");
   return 0;
@@ -1053,7 +1076,7 @@ extern "C" int rave_time_stack_nhwc(const float *x, void *out_bf16, int B, int C
   const int vec = (C % 8 == 0) && ((uintptr_t)x & 15) == 0 && sb % 4 == 0 && st % 4 == 0;
   const long total = (long)B * T * Fp * (Cp / 8);
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   time_stack_nhwc_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)out_bf16, sb, st, C, T, F, Fp,
                                                                         Cp, kt, pt, total, vec);
   RAVE_CHECK_LAUNCH("time_stack_nhwc");
@@ -1068,7 +1091,7 @@ extern "C" int rave_time_stack_nhwc_bwd(const void *g_bf16, float *gx, int B, in
   const int vec = (C % 8 == 0) && ((uintptr_t)gx & 15) == 0;
   const long total = vec ? (long)B * T * F * (C / 8) : (long)B * T * F * C;
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   time_stack_nhwc_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)g_bf16, gx, C, T, F, Fp,
                                                                             Cp, kt, pt, total, vec);
   RAVE_CHECK_LAUNCH("time_stack_nhwc_bwd");
@@ -1090,7 +1113,7 @@ __device__ __forceinline__ float dlk(float a, float slope) { return a > 0.f ? 1.
 
 __global__ void __launch_bounds__(256)
 leaky_fm_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, float *__restrict__ stats, long H, float slope,
-                    int vec) {
+                    int vec, const BlockSum bs) {
   __shared__ float red0[8], red1[8];
   float s0 = 0.f, s1 = 0.f;
   const long H4 = vec ? (H >> 2) : 0;
@@ -1123,9 +1146,10 @@ leaky_fm_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, float *_
   if (threadIdx.x == 0) {
     float u0 = 0.f, u1 = 0.f;
     for (int i = 0; i < 8; ++i) { u0 += red0[i]; u1 += red1[i]; }
-    atomicAdd(stats, u0);
-    atomicAdd(stats + 1, u1);
+    block_sum_put(bs, 0, u0);
+    block_sum_put(bs, 1, u1);
   }
+  block_sum_finish(bs, stats);
 }
 
 // The same tap that ALSO writes the next MRD conv's operand (rave_time_stack_nhwc of its own output, kt = 3, pt = 1):
@@ -1140,7 +1164,8 @@ __device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
 
 __global__ void __launch_bounds__(256)
 leaky_fm_stack_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, float *__restrict__ stats,
-                          __nv_bfloat16 *__restrict__ xs, long Rh, int T, int F, int C, int Fp, float slope) {
+                          __nv_bfloat16 *__restrict__ xs, long Rh, int T, int F, int C, int Fp, float slope,
+                          const BlockSum bs) {
   __shared__ float red0[8], red1[8];
   float s0 = 0.f, s1 = 0.f;
   const int C4 = C >> 2;
@@ -1194,9 +1219,10 @@ leaky_fm_stack_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, fl
   if (threadIdx.x == 0) {
     float u0 = 0.f, u1 = 0.f;
     for (int i = 0; i < 8; ++i) { u0 += red0[i]; u1 += red1[i]; }
-    atomicAdd(stats, u0);
-    atomicAdd(stats + 1, u1);
+    block_sum_put(bs, 0, u0);
+    block_sum_put(bs, 1, u1);
   }
+  block_sum_finish(bs, stats);
 }
 
 __device__ __forceinline__ void leaky_fm_bwd_one(float ar, float af, float gr, float gf, float d0, float d1, float slope,
@@ -1292,8 +1318,11 @@ extern "C" int rave_leaky_fm_fwd(const float *x, float *a, float *stats, long H,
   RAVE_CHECK_ARG(x && a && stats && H > 0 && slope > 0.f, "leaky_fm_fwd: bad argument");
   const int vec = (H % 4 == 0) && (((uintptr_t)x | (uintptr_t)a) & 15) == 0;
   long blocks = ((vec ? H / 4 : H) + 255) / 256;
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
-  leaky_fm_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, a, stats, H, slope, vec);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 2, (cudaStream_t)stream)) return rc;
+  leaky_fm_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, a, stats, H, slope, vec, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("leaky_fm_fwd");
   return 0;
 }
@@ -1305,9 +1334,12 @@ extern "C" int rave_leaky_fm_stack_fwd(const float *x, float *a, float *stats, v
                      slope > 0.f && (((uintptr_t)x | (uintptr_t)a) & 15) == 0 && ((uintptr_t)xs_bf16 & 7) == 0,
                  "leaky_fm_stack_fwd: bad argument (C %% 4 == 0, rows = whole batch entries of T steps, aligned buffers)");
   long blocks = (Rh * F * (C / 4) + 255) / 256;
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 2, (cudaStream_t)stream)) return rc;
   leaky_fm_stack_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, a, stats, (__nv_bfloat16 *)xs_bf16, Rh, T, F, C,
-                                                                          Fp, slope);
+                                                                          Fp, slope, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("leaky_fm_stack_fwd");
   return 0;
 }
@@ -1320,7 +1352,7 @@ extern "C" int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, con
                      ((uintptr_t)gxs_bf16 & 7) == 0,
                  "leaky_fm_stack_bwd: bad argument (C %% 4 == 0, rows = whole batch entries of T steps, aligned buffers)");
   long blocks = (Rh * F * (C / 4) + 255) / 256;
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 8 ? 148 * 8 : blocks);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
   leaky_fm_stack_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, (const __nv_bfloat16 *)gxs_bf16, ga, d, gx, Rh,
                                                                           T, F, C, Fp, slope);
   RAVE_CHECK_LAUNCH("leaky_fm_stack_bwd");
@@ -1333,7 +1365,7 @@ extern "C" int rave_leaky_fm_bwd(const float *a, const float *g, const float *d,
   RAVE_CHECK_ARG(a && gx && (g || d) && H > 0 && slope > 0.f, "leaky_fm_bwd: bad argument");
   const int vec = (H % 4 == 0) && (((uintptr_t)a | (uintptr_t)gx | (uintptr_t)g) & 15) == 0;
   long blocks = ((vec ? H / 4 : H) + 255) / 256;
-  blocks = blocks < 1 ? 1 : (blocks > 148 * 16 ? 148 * 16 : blocks);
+  blocks = blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks);
   leaky_fm_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, g, d, gx, H, slope, vec);
   RAVE_CHECK_LAUNCH("leaky_fm_bwd");
   return 0;

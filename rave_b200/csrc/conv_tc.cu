@@ -1,4 +1,4 @@
-// tcgen05 conv1d engine (sm_100a): im2col-free implicit GEMM with the TIME axis on the MMA M dimension.
+// wgmma conv1d engine (sm_90a): im2col-free implicit GEMM with the TIME axis on the MMA M dimension.
 //
 //   D[m = (b,l)][n = co] = sum_{tap k} sum_{ci}  A_k[(b,l)][ci] * W_k[co][ci]
 //   A_k[(b,l)][ci] = xa[b][l*stride + k*dil - pad_l][ci]            (zero outside [0, Lin))
@@ -7,10 +7,11 @@
 // offset of a K-major operand tile, which TMA expresses with a 4-D tensor map (c, phase, l/stride, b)
 // -- out-of-range rows (the conv padding) are zero-filled by the TMA unit, so there is no F.pad and no
 // im2col buffer.  Weights are tap-major bf16 wt[k][co][ci] (K-major B operand).  Both operand tiles use
-// the canonical K-major swizzled layout (row = one swizzle span = BLOCK_K*2 bytes), accumulators live
-// in TMEM (2 stages of BLOCK_N fp32 columns), and the epilogue (bias, residual, dual write of the
-// pre-activation fp32 stream and the bf16 activated operand of the NEXT conv) reads them back with
-// tcgen05.ld.  Warp roles: 0 = TMA producer, 1 = MMA issuer (+TMEM alloc), 2..5 = epilogue.
+// the canonical K-major swizzled layout (row = one swizzle span = BLOCK_K*2 bytes).  One warpgroup issues the
+// wgmma of a 128-row tile (two m64 halves) and keeps the accumulators in registers; a finished tile goes to a
+// shared-memory buffer from which the epilogue (bias, residual, dual write of the pre-activation fp32 stream and the
+// bf16 activated operand of the NEXT conv) reads it row by row while the warpgroup already runs the next tile.
+// Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
@@ -24,9 +25,8 @@ namespace rave {
 namespace tc {
 
 constexpr int BLOCK_M = 128;
-constexpr int NUM_THREADS = 192;
-constexpr int NUM_THREADS2 = 352;      // CTA-pair kernel: producer, MMA issuer, up to 8 epilogue warps (2 per TMEM quadrant), chunk loader
-constexpr int ACC_STAGES = 2;
+constexpr int NUM_THREADS = 288;       // MMA warpgroup, producer warp, 4 epilogue warps
+constexpr int SMEM_MAX = 227 * 1024;   // dynamic shared memory a CTA may opt into on sm_90
 
 struct TcParams {
   int B, Cin, Lin, Cout, Lout, K, stride, dil, pad_l;
@@ -54,20 +54,6 @@ struct TcParams {
                            // Cout, or 2*Cout in x3 mode
   int act_cs;              // x3: channels per POSITION of an output row (Cout; Cout/stride when the row holds the phases
                            // of a transposed conv side by side): column n = q*cs + c lives at q*2cs + c (hi), +cs (lo)
-  int stages;              // pipeline depth actually used (<= the layout's STAGES); RAVE_TC_STAGES overrides
-  // TMA-staged epilogue (CTA-pair kernel): the bf16 row segments the epilogue reads (LeakyReLU' mask, feature-matching
-  // partner, gradient skip, operand skip) and writes (out_act) move as [128 rows x 64 channels] chunks between HBM and
-  // shared memory by cp.async.bulk.tensor -- per-thread row accesses touch 32 different 128-byte lines per
-  // instruction and the L1 wavefront rate, not HBM, bounded the backward launches (DESIGN.md section 5.3)
-  int etma;                // 0 = per-thread global loads / stores
-  int in0_kind;            // chunk operand slot A: 0 none, 1 dact_src, 2 res_act
-  int in1_kind;            // chunk operand slot B: 0 none, 1 feature-matching partner rows, 2 res_bf16
-  int emode;               // compiled epilogue specialisation (tc_epi_chunk_tma) or -1: run-time flags
-  int e_stages;            // chunk buffers in flight (1 or 2)
-  int epi_off, bar_off;    // byte offsets of the chunk buffers / the barriers in (1024-aligned) shared memory
-  int dbg;                 // ablation switches for scripts/ablate_tc.py: 1 = no epilogue, 8 = no L2 prefetch, 2 = skip the
-                           // activation TMA loads, 4 = skip the weight TMA loads (results are garbage); TMA-staged
-                           // epilogue: 16 = do not wait for earlier bulk stores, 32 = no named barriers, 64 = no TMEM load
 };
 
 template <int BLOCK_N, int BLOCK_K, bool X3 = false>
@@ -79,18 +65,20 @@ struct SmemLayout {
   static constexpr int B_BYTES = PARTS * BLOCK_N * BLOCK_K * 2;          // bytes the TMA unit delivers
   static constexpr int B_BYTES_PAD = PARTS * B_PART;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES_PAD;
-  static constexpr int MAX_STAGES = (200 * 1024) / STAGE_BYTES;
+  static constexpr int ACC_LD = acc_pitch(BLOCK_N);
+  static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;                 // fp32 accumulator hand-over buffer
+  static constexpr int MAX_STAGES = (SMEM_MAX - ACC_BYTES - 256 - 1024) / STAGE_BYTES;
   static constexpr int STAGES = MAX_STAGES > 8 ? 8 : MAX_STAGES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int ACC_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // + barriers + alignment slack
+  static_assert(STAGES >= 2, "not enough shared memory for a 2-stage pipeline");
 };
 
-// Epilogue of one 128 x BLOCK_N accumulator tile: this thread owns TMEM lane `taddr.lane` = one output row.
+// Epilogue of one 128 x BLOCK_N accumulator tile: this thread owns row (taddr >> 16) + lane of the accumulator buffer.
 // One chunk = CW (16 or 32) consecutive channels.  All global loads of the chunk (residual, gradient skip,
-// LeakyReLU' mask, feature-matching partner row) are issued BEFORE the TMEM load so that their latency overlaps it.
-// Row segments move as 256-bit vectors (LDG/STG.E.ENL2.256, sm_100): one full 32-byte sector per lane and
-// instruction -- with 128-bit accesses every store was a HALF-sector L2 transaction and the HBM-bound layers ran
-// at ~2.4 TB/s of store traffic (profiles/r1_ablation_conv_tc2.txt: "no epilogue stores").
+// LeakyReLU' mask, feature-matching partner row) are issued BEFORE the accumulator load so that their latency overlaps it.
+// Row segments move as whole 32-byte sectors per lane (two 128-bit accesses each).
 template <int NWORDS>
 __device__ __forceinline__ void ld_words(const void *ptr, uint32_t *w) {
   static_assert(NWORDS % 8 == 0, "256-bit granules");
@@ -128,7 +116,7 @@ __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, 
     if (!X3 && p.dact_src) ld_words<NW>(p.dact_src + off, dm);
   }
   if (CW == 32) tmem_ld_32x32(taddr, v);
-  else tmem_ld_32x16(taddr, v);       // warp-collective: every lane participates, valid or not
+  else tmem_ld_32x16(taddr, v);
   if (!valid) return;
   if (p.bias) {
     const float4 *b4 = reinterpret_cast<const float4 *>(p.bias + co);
@@ -214,220 +202,22 @@ __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, 
   }
 }
 
-// TMA-staged variant of tc_epi_chunk (32 rows x 32 channels per warp): the bf16 operands come from the chunk buffers
-// the loader warp filled ([128 rows][128 bytes], SWIZZLE_128B: 16-byte unit u of row r sits at r*128 + ((u ^ (r & 7)) << 4),
-// so the 8 lanes of a shared-memory phase hit 8 different bank groups), the activated output is returned packed in
-// `pk` for the caller to stage.  fp32 streams (res, out_f32) are rare and small: per-thread accesses, generic mode only.
-//
-// The epilogue of the HBM-bound launches is ISSUE-bound (ncu source view, profiles/r2_epilogue_issue.md: ~310
-// instructions per warp and 32 x 32 chunk with runtime flags, 2 warps per scheduler), so the frequent operand
-// combinations are compiled as specialisations (MODE >= 0: bit 0 bias, bit 1 LeakyReLU output, bits 2-3 in0_kind,
-// bits 4-5 in1_kind; no fp32 streams, no ablation switches) and the arithmetic runs on packed pairs: add / mul as
-// f32x2 (sm_100 FADD2 / FMUL2), LeakyReLU as max(bf16x2(t), bf16x2(s t)) -- rounding is monotone, so this equals
-// bf16(max(t, s t)) bit for bit.  MODE = -1 keeps every flag at run time.
-constexpr int ECH_BYTES = 128 * 128;      // one [128 x 64] bf16 chunk
-template <int MODE>
-__device__ __forceinline__ void tc_epi_chunk_tma(const TcParams &p, uint32_t taddr, int co, bool valid, size_t orow,
-                                                 int fm_side, const uint8_t *in0, const uint8_t *in1, uint32_t rowoff,
-                                                 uint32_t rx, int half, uint32_t *pk) {
-  constexpr bool GEN = MODE < 0;
-  const bool has_bias = GEN ? (p.bias != nullptr) : ((MODE & 1) != 0);
-  const bool leaky = GEN ? (p.act == RAVE_ACT_LEAKY) : ((MODE & 2) != 0);
-  const int k0 = GEN ? p.in0_kind : ((MODE >> 2) & 3);
-  const int k1 = GEN ? p.in1_kind : ((MODE >> 4) & 3);
-  float v[32];
-  uint32_t a0w[16], a1w[16], rf[32];
-  const size_t off = orow * p.Cout + co;
-  if (k0) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) lds128(in0 + rowoff + ((((uint32_t)(half * 4 + q)) ^ rx) << 4), a0w + 4 * q);
-  }
-  if (k1) {
-#pragma unroll
-    for (int q = 0; q < 4; ++q) lds128(in1 + rowoff + ((((uint32_t)(half * 4 + q)) ^ rx) << 4), a1w + 4 * q);
-  }
-  if (GEN && p.res && valid) ld_words<32>(p.res + off, rf);
-  if (!GEN || !(p.dbg & 64)) tmem_ld_32x32(taddr, v);
-  if (has_bias) {
-    const float4 *b4 = reinterpret_cast<const float4 *>(p.bias + co);
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 bb = __ldg(b4 + i);
-      const float2 t0 = __fadd2_rn(make_float2(v[4 * i], v[4 * i + 1]), make_float2(bb.x, bb.y));
-      const float2 t1 = __fadd2_rn(make_float2(v[4 * i + 2], v[4 * i + 3]), make_float2(bb.z, bb.w));
-      v[4 * i] = t0.x; v[4 * i + 1] = t0.y; v[4 * i + 2] = t1.x; v[4 * i + 3] = t1.y;
-    }
-  }
-  if (k0 == 1) {       // LeakyReLU' from the sign bits of the saved operand
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float2 m = make_float2((a0w[w] & 0x00008000u) ? p.slope : 1.f, (a0w[w] & 0x80000000u) ? p.slope : 1.f);
-      const float2 t = __fmul2_rn(make_float2(v[2 * w], v[2 * w + 1]), m);
-      v[2 * w] = t.x; v[2 * w + 1] = t.y;
-    }
-  }
-  if (k1 == 1) {       // feature-matching gradient (see tc_epi_chunk)
-    const float d0 = __ldg(p.fm_d), d1 = fm_side > 0 ? __ldg(p.fm_d + 1) : 0.f;
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float as = h ? bf_hi(a0w[w]) : bf_lo(a0w[w]);
-        const float ap = h ? bf_hi(a1w[w]) : bf_lo(a1w[w]);
-        const float t = (as > ap ? 1.f : 0.f) - (as < ap ? 1.f : 0.f);
-        const float sr = (as > 0.f ? 1.f : 0.f) - (as < 0.f ? 1.f : 0.f);
-        v[2 * w + h] = fmaf(d1, sr, fmaf(d0, t, v[2 * w + h]));
-      }
-    }
-  }
-  if (k1 == 2) {
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float2 t = __fadd2_rn(make_float2(v[2 * w], v[2 * w + 1]), make_float2(bf_lo(a1w[w]), bf_hi(a1w[w])));
-      v[2 * w] = t.x; v[2 * w + 1] = t.y;
-    }
-  }
-  if (k0 == 2) {       // residual skip from the unit's own bf16 operand: undo the LeakyReLU
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float a0 = bf_lo(a0w[w]), a1 = bf_hi(a0w[w]);
-      v[2 * w] += fminf(a0, a0 * p.res_inv_slope);
-      v[2 * w + 1] += fminf(a1, a1 * p.res_inv_slope);
-    }
-  }
-  if (GEN && p.res && valid) {
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] += __uint_as_float(rf[i]);
-  }
-  if (GEN && p.out_f32 && valid) {
-    uint32_t o[32];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(v[i]);
-    st_words<32>(p.out_f32 + off, o);
-  }
-  if (leaky) {
-    const float2 s2 = make_float2(p.slope, p.slope);
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const float2 t = make_float2(v[2 * w], v[2 * w + 1]);
-      const float2 u = __fmul2_rn(t, s2);
-      const __nv_bfloat162 h = __hmax2(__floats2bfloat162_rn(t.x, t.y), __floats2bfloat162_rn(u.x, u.y));
-      pk[w] = *reinterpret_cast<const uint32_t *>(&h);
-    }
-  } else {
-#pragma unroll
-    for (int w = 0; w < 16; ++w) {
-      const __nv_bfloat162 h = __floats2bfloat162_rn(v[2 * w], v[2 * w + 1]);
-      pk[w] = *reinterpret_cast<const uint32_t *>(&h);
-    }
-  }
-}
-
-// The epilogue warps' whole tile loop of the TMA-staged path (8 warps: TMEM quadrant x 32-column half of a chunk).
-struct EtmaCtx {
-  uint8_t *smem;
-  uint64_t *tfull_bar, *tempty_bar, *efull_bar, *eempty_bar;
-  uint32_t tmem_base, rank;
-  int warp, lane, pair, num_pairs, num_tiles, n_mt;
-  const CUtensorMap *tmap_eo;
-};
-
-template <int BLOCK_N, int MODE>
-__device__ __forceinline__ void etma_epilogue(const TcParams &p, const EtmaCtx &x) {
-  constexpr bool GEN = MODE < 0;
-  constexpr int NCHUNK = (BLOCK_N + 63) / 64;
-  constexpr int ACC2 = (512 / BLOCK_N) > 4 ? 4 : (512 / BLOCK_N);
-  const int warp = x.warp, lane = x.lane;
-  const int quad = warp & 3;
-  const int half = (warp - 2) >> 2;
-  const int row = quad * 32 + lane;
-  const uint32_t rowoff = (uint32_t)row * 128u, rx = (uint32_t)(row & 7);
-  const int k0 = GEN ? p.in0_kind : ((MODE >> 2) & 3);
-  const int k1 = GEN ? p.in1_kind : ((MODE >> 4) & 3);
-  const int n_in = (k0 ? 1 : 0) + (k1 ? 1 : 0);
-  const uint32_t stage_stride = (uint32_t)(n_in + 1) * ECH_BYTES;
-  const bool issuer = threadIdx.x == 64;       // first epilogue thread: issues and tracks the bulk stores
-  const int dbg = GEN ? p.dbg : 0;
-  int es = 0;
-  uint32_t eph = 0;
-  int it = 0;
-  for (int tile = x.pair; tile < x.num_tiles; tile += x.num_pairs, ++it) {
-    const int acc = it % ACC2;
-    const uint32_t acc_phase = (it / ACC2) & 1;
-    const int nt = tile % p.n_nt;
-    const int mt = (tile / p.n_nt) * 2 + (int)x.rank;
-    const int lt = mt % p.n_lt;
-    const int bg = mt / p.n_lt;
-    const int n0 = nt * BLOCK_N;
-    const int l0 = lt * p.BL, b0 = bg * p.BB;
-    const int b = b0 + row / p.BL;
-    const int l = l0 + row % p.BL;
-    const bool valid = (mt < x.n_mt) && (b < p.B) && (l < p.Lout) && !(dbg & 1);
-    const size_t orow = (size_t)b * p.out_rows + (size_t)l;
-    const int fm_side = k1 == 1 ? (b < p.fm_bh ? 1 : -1) : 0;
-    mbar_wait(&x.tfull_bar[acc], acc_phase);
-    tc_fence_after();
-    const uint32_t taddr = x.tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BLOCK_N;
-#pragma unroll 1
-    for (int c = 0; c < NCHUNK; ++c) {
-      uint8_t *st = x.smem + p.epi_off + es * stage_stride;
-      uint8_t *outb = st + n_in * ECH_BYTES;
-      const int ccol = c * 64 + half * 32;
-      const bool active = ccol < BLOCK_N;      // BLOCK_N = 96: the last chunk has one 32-column half
-      uint32_t pk[16];
-      if (n_in) mbar_wait(&x.efull_bar[es], eph);
-      if (active)
-        tc_epi_chunk_tma<MODE>(p, taddr + ccol, n0 + ccol, valid, orow, fm_side, st, st + (k0 ? ECH_BYTES : 0), rowoff, rx,
-                               half, pk);
-      if (c == NCHUNK - 1) {                   // accumulator stage read out: hand it back to the MMA issuer
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_remote(&x.tempty_bar[acc], 0);
-      }
-      if (n_in) {                              // operand chunk consumed (registers hold what is needed)
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&x.eempty_bar[es]);
-      }
-      // the bulk store that last read this output buffer must be done reading it
-      if (issuer && !(dbg & 16)) {
-        if (p.e_stages == 2) bulk_wait_read<1>();
-        else bulk_wait_read<0>();
-      }
-      if (!(dbg & 32)) named_bar_sync(1, 256);
-      if (active && !(dbg & 1)) {
-#pragma unroll
-        for (int q = 0; q < 4; ++q) sts128(outb + rowoff + ((((uint32_t)(half * 4 + q)) ^ rx) << 4), pk + 4 * q);
-      }
-      fence_proxy_async();
-      if (!(dbg & 32)) named_bar_sync(1, 256);
-      if (issuer && !(dbg & 1)) {
-        tma_store_3d(x.tmap_eo, outb, n0 + c * 64, l0, b0);
-        bulk_commit();
-      }
-      if (++es == p.e_stages) { es = 0; eph ^= 1; }
-    }
-  }
-  if (issuer) bulk_wait_all();
-}
-
-// `part` of `parts` warps share one TMEM lane quadrant and take alternate 32-column chunks (the epilogue is
-// latency-bound -- tcgen05.ld, convert, store with ONE warp per scheduler -- so the CTA-pair kernel runs two)
 template <int BLOCK_N, bool X3>
 __device__ __forceinline__ void tc_epilogue(const TcParams &p, uint32_t taddr, int n0, bool valid, size_t orow,
-                                            int fm_side, int part = 0, int parts = 1) {
+                                            int fm_side) {
   constexpr int MAIN = BLOCK_N / 32 * 32;
   if (X3 && (p.act_cs & 31)) {
     // split-operand rows whose positions are 16 (mod 32) channels wide (capacity-48 transposed convs: 48 channels per
     // position): a 32-column chunk would straddle a [hi | lo] boundary -> 16-column chunks
 #pragma unroll 1
-    for (int c0 = part * 16; c0 < BLOCK_N; c0 += parts * 16)
+    for (int c0 = 0; c0 < BLOCK_N; c0 += 16)
       tc_epi_chunk<16, X3>(p, taddr + c0, n0 + c0, valid, orow, fm_side);
     return;
   }
 #pragma unroll 1
-  for (int c0 = part * 32; c0 < MAIN; c0 += parts * 32)
+  for (int c0 = 0; c0 < MAIN; c0 += 32)
     tc_epi_chunk<32, X3>(p, taddr + c0, n0 + c0, valid, orow, fm_side);
-  if (MAIN < BLOCK_N && part == 0) tc_epi_chunk<16, X3>(p, taddr + MAIN, n0 + MAIN, valid, orow, fm_side);
+  if (MAIN < BLOCK_N) tc_epi_chunk<16, X3>(p, taddr + MAIN, n0 + MAIN, valid, orow, fm_side);
 }
 
 template <int BLOCK_N, int BLOCK_K, bool X3>
@@ -437,46 +227,37 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
   constexpr int STAGES = L::STAGES;
   constexpr int SWZ = BLOCK_K * 2;
-  constexpr uint32_t TMEM_COLS = (ACC_STAGES * BLOCK_N <= 32) ? 32 : (ACC_STAGES * BLOCK_N <= 64) ? 64
-                                 : (ACC_STAGES * BLOCK_N <= 128) ? 128 : (ACC_STAGES * BLOCK_N <= 256) ? 256 : 512;
-  static_assert(ACC_STAGES * BLOCK_N <= 512, "TMEM overflow");
-  static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 256, "invalid UMMA N");
+  static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + L::BAR_OFFSET);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tfull_bar = empty_bar + STAGES;
-  uint64_t *tempty_bar = tfull_bar + ACC_STAGES;
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(tempty_bar + ACC_STAGES);
+  uint64_t *tfull_bar = empty_bar + STAGES;      // MMA warpgroup -> epilogue: the accumulator buffer holds a tile
+  uint64_t *tempty_bar = tfull_bar + 1;          // epilogue -> MMA warpgroup: the buffer has been read
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.n_lt * p.n_bg * p.n_nt;
   const int kblocks = p.K * p.num_kb;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);               // one arrival per MMA warp
     }
-    for (int s = 0; s < ACC_STAGES; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 4);
-    }
+    mbar_init(tfull_bar, 128);
+    mbar_init(tempty_bar, 4);
     fence_barrier_init();
+    acc_bind(smem + L::ACC_OFFSET, L::ACC_LD);
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   griddep_launch_dependents();      // dependents may begin their prologue ...
   griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
 
-  if (warp == 0) {
+  if (warp == 4) {
     // =========================== TMA producer (warp-uniform loop, elected lane issues) ===========================
     int stage = 0;
     uint32_t phase = 0;
@@ -512,55 +293,59 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer (warp-uniform loop, elected lane issues) ===========================
-    constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BLOCK_N);
+  } else if (warp < 4) {
+    // =========================== MMA warpgroup ===========================
+    // rows 64 h .. 64 h + 63 of an operand tile start 64 swizzle spans further: + (64 * SWZ) >> 4 in the address field
+    constexpr uint64_t A_HALF = (64 * SWZ) >> 4;
     const uint32_t smem_base = smem_u32(smem);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
+    float d[2][BLOCK_N / 2];
     int stage = 0;
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_u + acc * BLOCK_N;
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
         const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
         const uint64_t adesc = make_kmajor_desc(sa, SWZ);
         const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
-        if (elect_one()) {
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
+          // advance 16 bf16 = 32 bytes inside the swizzle span: +2 in the (addr >> 4) field
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
+        }
+        if (X3) {        // a*w ~ a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the lo*lo term is below fp32 accumulation noise)
+          const uint64_t adesc_lo = make_kmajor_desc(sa + L::A_PART, SWZ);
+          const uint64_t bdesc_lo = make_kmajor_desc(sa + L::A_BYTES + L::B_PART, SWZ);
 #pragma unroll
           for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
-            // advance 16 bf16 = 32 bytes inside the swizzle span: +2 in the (addr >> 4) field
-            umma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-          }
-          if (X3) {        // a*w ~ a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the lo*lo term is below fp32 accumulation noise)
-            const uint64_t adesc_lo = make_kmajor_desc(sa + L::A_PART, SWZ);
-            const uint64_t bdesc_lo = make_kmajor_desc(sa + L::A_BYTES + L::B_PART, SWZ);
 #pragma unroll
-            for (int kk = 0; kk < BLOCK_K / 16; ++kk) umma_f16(tmem_d, adesc_lo + 2 * kk, bdesc + 2 * kk, idesc, 1u);
-#pragma unroll
-            for (int kk = 0; kk < BLOCK_K / 16; ++kk) umma_f16(tmem_d, adesc + 2 * kk, bdesc_lo + 2 * kk, idesc, 1u);
+            for (int h = 0; h < 2; ++h) {
+              Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc_lo + h * A_HALF + 2 * kk, bdesc + 2 * kk, 1u);
+              Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc_lo + 2 * kk, 1u);
+            }
           }
-          umma_commit(&empty_bar[stage]);                       // frees the smem slot when the MMAs retire
-          if (kb == kblocks - 1) umma_commit(&tfull_bar[acc]);  // accumulator ready for the epilogue
         }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+        wgmma_fence_regs<BLOCK_N / 2>(d[1]);
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);           // this warp's MMAs no longer read the slot
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      mbar_wait(tempty_bar, (it & 1) ^ 1);                       // the epilogue has read the previous tile
+      acc_store<BLOCK_N>(d, threadIdx.x);
+      mbar_arrive(tfull_bar);
     }
   } else {
     // =========================== epilogue (4 warps) ===========================
-    const int quad = warp & 3;           // TMEM lane quadrant this warp may access
+    const int quad = warp & 3;           // rows quad * 32 .. quad * 32 + 31 of the tile
     const int row = quad * 32 + lane;    // row of the 128-row tile
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
       const int nt = tile % p.n_nt;
       const int mt = tile / p.n_nt;
       const int lt = mt % p.n_lt;
@@ -571,364 +356,12 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const bool valid = (b < p.B) && (l < p.Lout);
       const size_t orow = (size_t)b * p.out_rows + (size_t)l * p.out_row_stride + p.out_row_offset;
 
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BLOCK_N;
+      mbar_wait(tfull_bar, it & 1);
+      const uint32_t taddr = (uint32_t)(quad * 32) << 16;
       tc_epilogue<BLOCK_N, X3>(p, taddr, n0, valid, orow, p.fm_d ? (b < p.fm_bh ? 1 : -1) : 0);
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
+      if (lane == 0) mbar_arrive(tempty_bar);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
-}
-
-// =============================================================================================
-// CTA-pair variant (tcgen05 cta_group::2): two SMs of one TPC compute a 256 x BLOCK_N tile.
-// Each CTA loads ITS 128 activation rows and HALF of the weight tile (BLOCK_N/2 rows) -- the pair's
-// tensor cores read both halves, so per-SM shared-memory fill drops from (16 + 32) KB to (16 + 16) KB
-// per k-block at BLOCK_N = 256, which is what lifts the single-CTA ~52 % tensor-pipe ceiling
-// (profiles/r1_ncu_conv_tc_msd384_768.md).  Leader CTA (cluster rank 0) issues every MMA and owns the
-// `full` and `tmem-empty` barriers; `empty` / `tmem-full` barriers are replicated and signalled with a
-// multicast tcgen05.commit.
-// =============================================================================================
-template <int BLOCK_N, int BLOCK_K, bool X3 = false>
-struct SmemLayout2 {
-  // One pipeline stage always carries 64 reduction channels' worth of operands: UNITS = 64 / BLOCK_K
-  // (tap, channel-block) units, each with its own TMA box pair and BLOCK_K/16 MMAs, behind ONE barrier round
-  // trip -- a 32-channel block alone is only 2 MMAs (~190 clk at N = 192), less than the round trip costs.
-  static constexpr int UNITS = 64 / BLOCK_K;
-  static constexpr int PARTS = X3 ? 2 : 1;                              // x3: [hi units][lo units] of each operand
-  static constexpr int A_UNIT = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_UNIT = (BLOCK_N / 2) * BLOCK_K * 2;           // this CTA's half of the weight tile
-  static constexpr int A_BYTES = PARTS * UNITS * A_UNIT;
-  static constexpr int B_BYTES = PARTS * UNITS * B_UNIT;
-  static constexpr int B_BYTES_PAD = (B_BYTES + 1023) / 1024 * 1024;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES_PAD;
-  static constexpr int MAX_STAGES = (200 * 1024) / STAGE_BYTES;
-  static constexpr int STAGES = MAX_STAGES > 8 ? 8 : MAX_STAGES;
-  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;
-};
-
-template <int BLOCK_N, int BLOCK_K, bool X3>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(NUM_THREADS2, 1)
-conv_tc2_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                const __grid_constant__ CUtensorMap tmap_e0, const __grid_constant__ CUtensorMap tmap_e1,
-                const __grid_constant__ CUtensorMap tmap_eo, const TcParams p) {
-  using L = SmemLayout2<BLOCK_N, BLOCK_K, X3>;
-  constexpr int STAGES = L::STAGES;
-  constexpr int UNITS = L::UNITS;
-  constexpr int SWZ = BLOCK_K * 2;
-  // accumulator stages: as many as the 512 TMEM columns hold (up to 4).  A tile's accumulator is owned by the epilogue
-  // from the MMAs' commit until its last TMEM read; on the HBM-bound layers (few MMAs per tile) that hand-over chain,
-  // not the tensor pipe, paces the kernel, and its throughput is (stages x BLOCK_N) columns per chain latency.
-  constexpr int ACC2 = (512 / BLOCK_N) > 4 ? 4 : (512 / BLOCK_N);
-  constexpr uint32_t TMEM_COLS = (ACC2 * BLOCK_N <= 32) ? 32 : (ACC2 * BLOCK_N <= 64) ? 64
-                                 : (ACC2 * BLOCK_N <= 128) ? 128 : (ACC2 * BLOCK_N <= 256) ? 256 : 512;
-  static_assert(BLOCK_N % 32 == 0 && BLOCK_N <= 256, "cta_group::2 needs N % 32 == 0 (16 rows of B per CTA granule)");
-
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + p.bar_off);
-  uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tfull_bar = empty_bar + STAGES;
-  uint64_t *tempty_bar = tfull_bar + ACC2;
-  uint64_t *efull_bar = tempty_bar + ACC2;       // chunk operands landed (loader warp -> epilogue)
-  uint64_t *eempty_bar = efull_bar + 2;                // chunk operands consumed (epilogue -> loader warp)
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(eempty_bar + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x >> 1;
-  const int num_pairs = gridDim.x >> 1;
-  const int n_mt = p.n_lt * p.n_bg;
-  const int n_mp = (n_mt + 1) >> 1;                  // M tile pairs
-  const int num_tiles = n_mp * p.n_nt;
-  const int kblocks = p.K * p.num_kb;
-  // 4 or 8 epilogue warps (launch configuration); the TMA-staged epilogue adds a chunk-loader warp after them
-  const int epi_warps = (int)(blockDim.x >> 5) - 2 - (p.etma ? 1 : 0);
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    if (p.etma) {
-      tma_prefetch_desc(&tmap_eo);
-      if (p.in0_kind) tma_prefetch_desc(&tmap_e0);
-      if (p.in1_kind) tma_prefetch_desc(&tmap_e1);
-    }
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full_bar[s], 2);        // leader's: its own arrive.expect_tx + the peer's remote arrive
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int s = 0; s < ACC2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], 2 * epi_warps);       // leader's: the epilogue warps of both CTAs
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&efull_bar[s], 1);
-      mbar_init(&eempty_bar[s], epi_warps);
-    }
-    fence_barrier_init();
-  }
-  cluster_sync_all();
-  if (warp == 1) tmem_alloc_2sm(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
-  griddep_launch_dependents();      // dependents may begin their prologue ...
-  griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
-
-  if (warp == 0) {
-    // =========================== TMA producer (both CTAs; warp-uniform loop) ===========================
-    int stage = 0;
-    uint32_t phase = 0;
-    const uint32_t unit_tx = 2 * L::PARTS * (((p.dbg & 2) ? 0 : L::A_UNIT) + ((p.dbg & 4) ? 0 : L::B_UNIT));
-    for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-      const int nt = tile % p.n_nt;
-      const int mt = (tile / p.n_nt) * 2 + (int)rank;      // this CTA's M tile (may be >= n_mt: zero-filled)
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int l0 = lt * p.BL;
-      const int b0 = bg * p.BB;
-      const int n0 = nt * BLOCK_N + (int)rank * (BLOCK_N / 2);
-      // running (tap, channel block) counters: all index arithmetic stays OUTSIDE the elected region (uniform
-      // registers, one division per tap) -- the producer has to turn a stage around in well under the ~400 clk
-      // the tensor pipe needs to consume it
-      int k = 0, kb = 0;
-      int j = (-p.pad_l) / p.stride, ph = (-p.pad_l) - j * p.stride;
-      if (ph < 0) { ph += p.stride; j -= 1; }
-      for (int u0 = 0; u0 < kblocks; u0 += UNITS) {
-        const int nu = min(UNITS, kblocks - u0);
-        int c_kb[UNITS], c_ph[UNITS], c_row[UNITS], c_w[UNITS];
-#pragma unroll
-        for (int u = 0; u < UNITS; ++u) {
-          c_kb[u] = kb * BLOCK_K; c_ph[u] = ph; c_row[u] = l0 + j; c_w[u] = k * p.Cout + n0;
-          if (u < nu) {
-            if (++kb == p.num_kb) {
-              kb = 0; ++k;
-              // input row = l*stride + k*dil - pad_l = (l + j)*stride + ph
-              const int off = k * p.dil - p.pad_l;
-              j = off / p.stride;
-              ph = off - j * p.stride;
-              if (ph < 0) { ph += p.stride; j -= 1; }
-            }
-          }
-        }
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t *sa = smem + stage * L::STAGE_BYTES;
-        uint8_t *sb = sa + L::A_BYTES;
-        if (elect_one()) {
-#pragma unroll
-          for (int u = 0; u < UNITS; ++u) {
-            if (u < nu) {
-              if (!(p.dbg & 2))
-                tma_load_4d_2sm(sa + u * L::A_UNIT, &tmap_a, &full_bar[stage], c_kb[u], c_ph[u], c_row[u], b0);
-              if (!(p.dbg & 4))
-                tma_load_2d_2sm(sb + u * L::B_UNIT, &tmap_b, &full_bar[stage], c_kb[u], c_w[u]);
-              if (X3) {    // lo halves: channels Cin.. of the activation rows, weight slabs K.. (wt is [2][K][Cout][Cin])
-                tma_load_4d_2sm(sa + (UNITS + u) * L::A_UNIT, &tmap_a, &full_bar[stage], p.Cin + c_kb[u], c_ph[u],
-                                c_row[u], b0);
-                tma_load_2d_2sm(sb + (UNITS + u) * L::B_UNIT, &tmap_b, &full_bar[stage], c_kb[u], c_w[u] + p.K * p.Cout);
-              }
-            }
-          }
-          if (leader) mbar_arrive_expect_tx(&full_bar[stage], unit_tx * nu);
-          else mbar_arrive_remote(&full_bar[stage], 0);
-        }
-        __syncwarp();
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1 && leader) {
-    // =========================== MMA issuer (leader only) ===========================
-    constexpr uint32_t idesc = make_idesc_bf16(256, BLOCK_N);
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs, ++it) {
-      const int acc = it % ACC2;
-      const uint32_t acc_phase = (it / ACC2) & 1;
-      mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-      tc_fence_after();
-      const uint32_t tmem_d = tmem_u + acc * BLOCK_N;
-      for (int u0 = 0; u0 < kblocks; u0 += UNITS) {
-        const int nu = min(UNITS, kblocks - u0);
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-        const uint32_t sb = sa + L::A_BYTES;
-        if (elect_one()) {
-#pragma unroll
-          for (int u = 0; u < UNITS; ++u) {
-            if (u < nu) {
-              const uint64_t adesc = make_kmajor_desc(sa + u * L::A_UNIT, SWZ);
-              const uint64_t bdesc = make_kmajor_desc(sb + u * L::B_UNIT, SWZ);
-#pragma unroll
-              for (int kk = 0; kk < BLOCK_K / 16; ++kk)
-                umma_f16_2sm(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (u0 > 0 || u > 0 || kk > 0) ? 1u : 0u);
-              if (X3) {    // + a_lo * w_hi + a_hi * w_lo
-                const uint64_t adesc_lo = make_kmajor_desc(sa + (UNITS + u) * L::A_UNIT, SWZ);
-                const uint64_t bdesc_lo = make_kmajor_desc(sb + (UNITS + u) * L::B_UNIT, SWZ);
-#pragma unroll
-                for (int kk = 0; kk < BLOCK_K / 16; ++kk)
-                  umma_f16_2sm(tmem_d, adesc_lo + 2 * kk, bdesc + 2 * kk, idesc, 1u);
-#pragma unroll
-                for (int kk = 0; kk < BLOCK_K / 16; ++kk)
-                  umma_f16_2sm(tmem_d, adesc + 2 * kk, bdesc_lo + 2 * kk, idesc, 1u);
-              }
-            }
-          }
-          umma_commit_2sm(&empty_bar[stage]);
-          if (u0 + UNITS >= kblocks) umma_commit_2sm(&tfull_bar[acc]);
-        }
-        __syncwarp();
-        if (++stage == p.stages) { stage = 0; phase ^= 1; }
-      }
-    }
-    // the peer's last arrivals must land before this CTA's barriers disappear
-    if (it > 0) {
-      const int last = it - 1;
-      for (int t = (it > ACC2 ? it - ACC2 : 0); t <= last; ++t) mbar_wait(&tempty_bar[t % ACC2], (t / ACC2) & 1);
-    }
-    __syncwarp();
-  } else if (p.etma && warp == 2 + epi_warps) {
-    // =========================== chunk loader (TMA-staged epilogue operands) ===========================
-    // Runs up to e_stages chunks ahead of the epilogue -- across tile boundaries, i.e. the next tile's operand rows
-    // arrive while its MMAs are still running.  Rows / batches beyond the tensor are zero-filled by the TMA unit.
-    const int n_in = (p.in0_kind ? 1 : 0) + (p.in1_kind ? 1 : 0);
-    if (n_in > 0) {
-      constexpr int NCHUNK = (BLOCK_N + 63) / 64;
-      const uint32_t stage_stride = (uint32_t)(n_in + 1) * ECH_BYTES;
-      int es = 0;
-      uint32_t eph = 0;
-      for (int tile = pair; tile < num_tiles; tile += num_pairs) {
-        const int nt = tile % p.n_nt;
-        const int mt = (tile / p.n_nt) * 2 + (int)rank;
-        const int l0 = (mt % p.n_lt) * p.BL;
-        const int b0 = (mt / p.n_lt) * p.BB;
-        const int n0 = nt * BLOCK_N;
-        // feature-matching partner rows: the other batch half ([real; fake] batch), or -- fake-half launches -- the
-        // same coordinates of a tensor map based fm_half elements earlier
-        const int bp = p.fm_bh > 0 ? (b0 < p.fm_bh ? b0 + p.fm_bh : b0 - p.fm_bh) : b0;
-        // With two chunk buffers only ~64 KB of operand rows are in flight per SM: less than HBM latency x bandwidth.
-        // Pull the NEXT tile's chunks into L2 now (one TMA prefetch per box), so that its loads are L2 hits.
-        if (!(p.dbg & 8)) {
-          const int tile2 = tile + num_pairs;
-          if (tile2 < num_tiles && elect_one()) {
-            const int mt2 = (tile2 / p.n_nt) * 2 + (int)rank;
-            const int l2 = (mt2 % p.n_lt) * p.BL, b2 = (mt2 / p.n_lt) * p.BB;
-            const int n2 = (tile2 % p.n_nt) * BLOCK_N;
-            const int bp2 = p.fm_bh > 0 ? (b2 < p.fm_bh ? b2 + p.fm_bh : b2 - p.fm_bh) : b2;
-            for (int c = 0; c < NCHUNK; ++c) {
-              if (p.in0_kind) tma_prefetch_3d(&tmap_e0, n2 + c * 64, l2, b2);
-              if (p.in1_kind) tma_prefetch_3d(&tmap_e1, n2 + c * 64, l2, p.in1_kind == 1 ? bp2 : b2);
-            }
-          }
-          __syncwarp();
-        }
-        for (int c = 0; c < NCHUNK; ++c) {
-          mbar_wait(&eempty_bar[es], eph ^ 1);
-          uint8_t *st = smem + p.epi_off + es * stage_stride;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&efull_bar[es], (uint32_t)n_in * ECH_BYTES);
-            if (p.in0_kind) tma_load_3d(st, &tmap_e0, &efull_bar[es], n0 + c * 64, l0, b0);
-            if (p.in1_kind)
-              tma_load_3d(st + (p.in0_kind ? ECH_BYTES : 0), &tmap_e1, &efull_bar[es], n0 + c * 64, l0,
-                          p.in1_kind == 1 ? bp : b0);
-          }
-          __syncwarp();
-          if (++es == p.e_stages) { es = 0; eph ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 2 && p.etma) {
-    // =========================== epilogue, TMA-staged (8 warps) ===========================
-    if constexpr (!X3) {
-      EtmaCtx x;
-      x.smem = smem; x.tfull_bar = tfull_bar; x.tempty_bar = tempty_bar; x.efull_bar = efull_bar;
-      x.eempty_bar = eempty_bar; x.tmem_base = tmem_base; x.rank = rank; x.warp = warp; x.lane = lane; x.pair = pair;
-      x.num_pairs = num_pairs; x.num_tiles = num_tiles; x.n_mt = n_mt; x.tmap_eo = &tmap_eo;
-      switch (p.emode) {       // see tc_epi_chunk_tma: bias | leaky << 1 | in0_kind << 2 | in1_kind << 4
-        case 2: etma_epilogue<BLOCK_N, 2>(p, x); break;                  // forward, LeakyReLU operand out
-        case 3: etma_epilogue<BLOCK_N, 3>(p, x); break;                  // ... with bias (discriminator layers)
-        case 10: etma_epilogue<BLOCK_N, 10>(p, x); break;                // 1x1 conv of a unit: + skip from the operand
-        case 4: etma_epilogue<BLOCK_N, 4>(p, x); break;                  // dgrad: LeakyReLU' mask
-        case 20: etma_epilogue<BLOCK_N, 20>(p, x); break;                // dgrad + feature-matching gradient
-        case 36: etma_epilogue<BLOCK_N, 36>(p, x); break;                // dgrad + gradient skip
-        default: etma_epilogue<BLOCK_N, -1>(p, x); break;
-      }
-    }
-  } else if (warp >= 2) {
-    // =========================== epilogue (4 warps in each CTA) ===========================
-    const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int part = (warp - 2) >> 2;          // which of the quadrant's warps: alternate 32-column chunks
-    const int parts = epi_warps >> 2;
-    const int row = quad * 32 + lane;
-    int it = 0;
-    for (int tile = pair; tile < num_tiles; tile += num_pairs, ++it) {
-      const int acc = it % ACC2;
-      const uint32_t acc_phase = (it / ACC2) & 1;
-      const int nt = tile % p.n_nt;
-      const int mt = (tile / p.n_nt) * 2 + (int)rank;
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int n0 = nt * BLOCK_N;
-      const int b = bg * p.BB + row / p.BL;
-      const int l = lt * p.BL + row % p.BL;
-      const bool valid = (mt < n_mt) && (b < p.B) && (l < p.Lout) && !(p.dbg & 1);
-      const size_t orow = (size_t)b * p.out_rows + (size_t)l * p.out_row_stride + p.out_row_offset;
-      // The epilogue is a chain of dependent (load -> TMEM read -> math -> store) steps per 32-column chunk with one
-      // or two warps per scheduler: its global loads were served from HBM at full latency (the backward launches,
-      // which read the saved operand rows, ran at ~1.7 TB/s).  Pull the NEXT tile's row segments of every epilogue
-      // operand into L2 now -- a whole tile ahead -- so the loads issued later hit L2.
-      if (part == 0 && !(p.dbg & 8)) {
-        const int tile2 = tile + num_pairs;
-        if (tile2 < num_tiles) {
-          const int mt2 = (tile2 / p.n_nt) * 2 + (int)rank;
-          const int b2 = (mt2 / p.n_lt) * p.BB + row / p.BL;
-          const int l2 = (mt2 % p.n_lt) * p.BL + row % p.BL;
-          if (mt2 < n_mt && b2 < p.B && l2 < p.Lout) {
-            const size_t off2 = ((size_t)b2 * p.out_rows + (size_t)l2 * p.out_row_stride + p.out_row_offset) *
-                                    (X3 ? p.act_ld : p.Cout) + (size_t)(tile2 % p.n_nt) * BLOCK_N;
-#pragma unroll
-            for (int c = 0; c < BLOCK_N; c += 64) {       // 128-byte lines of a bf16 row segment
-              if (!X3 && p.dact_src) prefetch_l2(p.dact_src + off2 + c);
-              if (!X3 && p.fm_d) prefetch_l2(p.dact_src + (b2 < p.fm_bh ? off2 + p.fm_half : off2 - p.fm_half) + c);
-              if (!X3 && p.res_bf16) prefetch_l2(p.res_bf16 + off2 + c);
-              if (p.res_act) prefetch_l2(p.res_act + off2 + c);
-              if (X3 && p.res_act) prefetch_l2(p.res_act + off2 + p.act_cs + c);
-            }
-          }
-        }
-      }
-      mbar_wait(&tfull_bar[acc], acc_phase);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + acc * BLOCK_N;
-      const int fm_side = p.fm_d ? (b < p.fm_bh ? 1 : -1) : 0;
-      tc_epilogue<BLOCK_N, X3>(p, taddr, n0, valid, orow, fm_side, part, parts);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_remote(&tempty_bar[acc], 0);
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, TMEM_COLS);
   }
 }
 
@@ -965,51 +398,19 @@ static int pick_block_k(int Cin) {
 }
 
 static int pick_block_n(int Cout, long m_tiles) {
-  // largest tile that still gives every SM work; Cout must be a multiple of it
-  const int cands[] = {256, 192, 128, 96, 64, 48, 32, 16};
+  // largest tile that still gives every SM work; Cout must be a multiple of it.  N <= 128: the MMA warpgroup holds the
+  // 128 x N accumulator tile in registers (N fp32 per thread)
+  const int cands[] = {128, 96, 64, 48, 32, 16};
+  constexpr int NC = sizeof(cands) / sizeof(cands[0]);
   int best = 0;
   for (int c : cands) {
     if (Cout % c) continue;
     if (!best) best = c;
-    if (m_tiles * (Cout / c) >= 148) return c;
+    if (m_tiles * (Cout / c) >= 132) return c;
   }
   // not enough tiles even at the smallest N: take the smallest valid one >= 32 if any
-  for (int i = 7; i >= 0; --i)
+  for (int i = NC - 1; i >= 0; --i)
     if (Cout % cands[i] == 0 && cands[i] >= 32) return cands[i];
-  return best;
-}
-
-// CTA-pair kernel: pick the N tile by a small cost model instead of "largest tile that fills the machine".
-//   waves(BN) = ceil(pair-tiles / 74),  stage clocks = max(MMA = 2*BN (4 MMAs of a 256 x BN x 16 atom at BN/2 clk),
-//   fill = (16 KB activations + BN*64 B weights per CTA) / ~60 B/clk);  cost = waves * stage clocks.
-// The decoder / encoder blocks with few rows and many channels (768 x 768 at 2048 rows) were given BN = 64 to reach
-// 148 tiles: two waves of fill-bound tiles; BN = 128 does the same work in one wave of better-balanced tiles.
-static int pick_block_n2(int Cout, long m_tiles, int kblocks = 0) {
-  const int cands[] = {256, 192, 128, 96, 64};
-  const long n_mp = (m_tiles + 1) / 2;
-  int best = 0;
-  double best_cost = 0;
-  for (int c : cands) {
-    if (Cout % c) continue;
-    const long tiles = n_mp * (Cout / c);
-    const long waves = (tiles + 73) / 74;
-    const double mma = 2.0 * c, fill = (16384.0 + 64.0 * c) / 60.0;
-    double tile = (kblocks > 0 ? kblocks : 1) * (mma > fill ? mma : fill);
-    if (kblocks > 0) {
-      // accumulator hand-over chain (commit -> epilogue wake-up -> TMEM reads -> release -> MMA wake-up, ~5000 clk
-      // measured on the K = 1 layers): one tile per chain latency / accumulator stages
-      const int acc = (512 / c) > 4 ? 4 : (512 / c);
-      static double chain_clk = -1.0;
-      if (chain_clk < 0) {
-        const char *e = getenv("RAVE_TC_CHAIN");
-        chain_clk = (e && atof(e) > 0) ? atof(e) : 5000.0;
-      }
-      const double chain = chain_clk / acc;
-      if (chain > tile) tile = chain;
-    }
-    const double cost = (double)waves * tile;
-    if (!best || cost < best_cost) { best = c; best_cost = cost; }
-  }
   return best;
 }
 
@@ -1027,7 +428,7 @@ static int launch(const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &
     attr = true;
   }
   const int tiles = p.n_lt * p.n_bg * p.n_nt;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
@@ -1036,93 +437,10 @@ static int launch(const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &
   return 0;
 }
 
-constexpr int SMEM_MAX = 227 * 1024;       // dynamic shared memory a CTA may opt into on sm_100
-
-template <int BN, int BK, bool X3>
-static int launch2(const CUtensorMap &ta, const CUtensorMap &tb, const CUtensorMap *te, const TcParams &p,
-                   cudaStream_t stream) {
-  using L = SmemLayout2<BN, BK, X3>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, BK, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         SMEM_MAX);
-    if (e != cudaSuccess) {
-      set_error("conv1d_tc(2cta): cudaFuncSetAttribute(%d bytes): %s", SMEM_MAX, cudaGetErrorString(e));
-      return 2;
-    }
-    attr = true;
-  }
-  const int n_mp = (p.n_lt * p.n_bg + 1) / 2;
-  const int tiles = n_mp * p.n_nt;
-  int dev = 0, sms = 148;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  int pairs = sms / 2;
-  if (pairs > tiles) pairs = tiles;
-  TcParams q = p;
-  // shared memory: [pipeline stages][chunk buffers of the TMA-staged epilogue][barriers]
-  int epi_bytes = 0;
-  if (q.etma) {
-    const int n_in = (q.in0_kind ? 1 : 0) + (q.in1_kind ? 1 : 0);
-    const int budget = SMEM_MAX - 1024 - 256;
-    // two chunk buffers unless that leaves the mainloop fewer than 4 stages
-    q.e_stages = 2;
-    if ((budget - 2 * (n_in + 1) * ECH_BYTES) / L::STAGE_BYTES < 4) q.e_stages = 1;
-    {
-      const char *e = getenv("RAVE_TC_ESTAGES");
-      if (e && (atoi(e) == 1 || atoi(e) == 2)) q.e_stages = atoi(e);
-    }
-    epi_bytes = q.e_stages * (n_in + 1) * ECH_BYTES;
-    q.stages = (budget - epi_bytes) / L::STAGE_BYTES;
-    if (q.stages > L::STAGES) q.stages = L::STAGES;
-    if (q.stages < 2) {          // does not fit: per-thread epilogue
-      q.etma = 0;
-      epi_bytes = 0;
-    }
-  }
-  if (!q.etma) q.stages = L::STAGES;
-  {
-    const char *e = getenv("RAVE_TC_STAGES");
-    if (e && atoi(e) >= 2 && atoi(e) < q.stages) q.stages = atoi(e);
-  }
-  q.epi_off = q.stages * L::STAGE_BYTES;
-  q.bar_off = q.epi_off + epi_bytes;
-  const int smem_bytes = q.bar_off + 256 + 1024;
-  // epilogue warps: 8 (two per TMEM quadrant) when a tile has little MMA work per output column -- those layers are
-  // bound by the latency of the TMEM-load / convert / store chain -- else 4 (the extra warps only take issue slots
-  // from the tensor-bound loops); RAVE_TC_EPIWARPS overrides.  The TMA-staged epilogue always runs 8 (+ its loader warp).
-  int epi = ((long)p.K * p.Cin <= 1024 || p.dact_src || p.res_bf16 || p.res_act || p.res) ? 8 : 4;
-  {
-    const char *e = getenv("RAVE_TC_EPIWARPS");
-    if (e && (atoi(e) == 4 || atoi(e) == 8)) epi = atoi(e);
-  }
-  if (q.etma) epi = 8;
-  launch_pdl(conv_tc2_kernel<BN, BK, X3>, dim3(2 * pairs), dim3(64 + 32 * epi + (q.etma ? 32 : 0)), smem_bytes, stream, ta, tb,
-             te[0], te[1], te[2], q);
-  RAVE_CHECK_LAUNCH("conv1d_tc(2cta)");
-  return 0;
-}
-
-template <int BK, bool X3>
-static int dispatch_n2(int bn, const CUtensorMap &ta, const CUtensorMap &tb, const CUtensorMap *te, const TcParams &p,
-                       cudaStream_t s) {
-  switch (bn) {
-    case 256: return launch2<256, BK, X3>(ta, tb, te, p, s);
-    case 192: return launch2<192, BK, X3>(ta, tb, te, p, s);
-    case 128: return launch2<128, BK, X3>(ta, tb, te, p, s);
-    case 96: return launch2<96, BK, X3>(ta, tb, te, p, s);
-    case 64: return launch2<64, BK, X3>(ta, tb, te, p, s);
-  }
-  set_error("conv1d_tc(2cta): no kernel for BLOCK_N=%d", bn);
-  return 1;
-}
-
 template <int BK, bool X3>
 static int dispatch_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p,
                       cudaStream_t s) {
   switch (bn) {
-    case 256: return launch<256, BK, X3>(ta, tb, p, s);
-    case 192: return launch<192, BK, X3>(ta, tb, p, s);
     case 128: return launch<128, BK, X3>(ta, tb, p, s);
     case 96: return launch<96, BK, X3>(ta, tb, p, s);
     case 64: return launch<64, BK, X3>(ta, tb, p, s);
@@ -1135,11 +453,7 @@ static int dispatch_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, cons
 }
 
 template <bool X3>
-static int dispatch_all(bool use2, int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const CUtensorMap *te,
-                        const TcParams &p, cudaStream_t s) {
-  if (use2)
-    return BK == 64 ? dispatch_n2<64, X3>(BN, ta, tb, te, p, s) : BK == 32 ? dispatch_n2<32, X3>(BN, ta, tb, te, p, s)
-                                                                           : dispatch_n2<16, X3>(BN, ta, tb, te, p, s);
+static int dispatch_all(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
   switch (BK) {
     case 64: return dispatch_n<64, X3>(BN, ta, tb, p, s);
     case 32: return dispatch_n<32, X3>(BN, ta, tb, p, s);
@@ -1150,13 +464,11 @@ static int dispatch_all(bool use2, int BK, int BN, const CUtensorMap &ta, const 
 }
 
 // The split-operand (x3) instantiations live in their own translation unit (conv_tc_x3.cu includes this file with
-// RAVE_TC_X3_UNIT defined) so that the two sets of ~40 kernels compile in parallel.
-int conv_tc_dispatch_x3(bool use2, int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const CUtensorMap *te,
-                        const TcParams &p, cudaStream_t s);
+// RAVE_TC_X3_UNIT defined) so that the two sets of kernels compile in parallel.
+int conv_tc_dispatch_x3(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s);
 #ifdef RAVE_TC_X3_UNIT
-int conv_tc_dispatch_x3(bool use2, int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const CUtensorMap *te,
-                        const TcParams &p, cudaStream_t s) {
-  return dispatch_all<true>(use2, BK, BN, ta, tb, te, p, s);
+int conv_tc_dispatch_x3(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
+  return dispatch_all<true>(BK, BN, ta, tb, p, s);
 }
 #endif
 
@@ -1171,7 +483,7 @@ extern "C" int rave_conv1d_tc_supported(int Cin, int Cout, int K, int stride, in
   return 1;
 }
 
-// Which kernel instance rave_conv1d_tc_fwd runs for a shape: BLOCK_N | BLOCK_K << 12 | (CTA pair ? 1 << 24 : 0); 0 = none.
+// Which kernel instance rave_conv1d_tc_fwd runs for a shape: BLOCK_N | BLOCK_K << 12; 0 = none.
 extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
   using namespace rave;
   using namespace rave::tc;
@@ -1180,14 +492,9 @@ extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
   int BL = 128;
   while (BL > Lout && BL > 8) BL >>= 1;
   const long m_tiles = (long)ceil_div(Lout, BL) * ceil_div(B, 128 / BL);
-  const char *e = getenv("RAVE_TC_2CTA");
-  const bool want2 = !(e && e[0] == '0');
-  int BN = 0;
-  if (want2 && m_tiles >= 2) BN = pick_block_n2(Cout, m_tiles, K > 0 ? K * ceil_div(Cin, 64) : 0);
-  if (!BN) BN = pick_block_n(Cout, m_tiles);
+  const int BN = pick_block_n(Cout, m_tiles);
   if (!BN) return 0;
-  const bool use2 = want2 && (BN % 32 == 0) && BN >= 64 && m_tiles >= 2;
-  return BN | (BK << 12) | (use2 ? 1 << 24 : 0);
+  return BN | (BK << 12);
 }
 
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,
@@ -1246,7 +553,6 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   p.fm_d = fm_d;
   p.fm_bh = fm_bh > 0 ? fm_bh : 0;                 // fm_bh < 0: every row is a fake row (partner |fm_bh| batches before)
   p.fm_half = (long)(fm_bh > 0 ? fm_bh : -fm_bh) * p.out_rows * Cout;
-  p.stages = 0;
   p.x3 = x3 ? 1 : 0;
   p.act_ld = x3 ? 2 * Cout : Cout;
   p.act_cs = act_cs > 0 ? act_cs : Cout;
@@ -1254,30 +560,15 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
                  "conv1d_tc(x3): %d channels per position do not tile the %d-column rows in 16-column chunks", p.act_cs,
                  Cout);
   RAVE_CHECK_ARG(!x3 || !res_act || p.act_cs == Cout, "conv1d_tc(x3): res_act needs one position per row");
-  p.dbg = 0;
-  {
-    const char *e = getenv("RAVE_TC_DBG");
-    if (e) p.dbg = atoi(e);
-  }
   int BL = 128;
   while (BL > Lout && BL > 8) BL >>= 1;   // power of two <= max(Lout, 8)
   p.BL = BL; p.BB = 128 / BL;
   p.n_lt = ceil_div(Lout, BL);
   p.n_bg = ceil_div(B, p.BB);
-  static int want2 = -1;
-  if (want2 < 0) {
-    const char *e = getenv("RAVE_TC_2CTA");
-    want2 = (e && e[0] == '0') ? 0 : 1;
-  }
-  int BN = 0;
-  if (want2 && (long)p.n_lt * p.n_bg >= 2) BN = pick_block_n2(Cout, (long)p.n_lt * p.n_bg, K * ceil_div(Cin, 64));
-  if (!BN) BN = pick_block_n(Cout, (long)p.n_lt * p.n_bg);
+  const int BN = pick_block_n(Cout, (long)p.n_lt * p.n_bg);
   RAVE_CHECK_ARG(BN > 0, "conv1d_tc: no BLOCK_N for Cout=%d", Cout);
   p.n_nt = Cout / BN;
   p.num_kb = ceil_div(Cin, BK);
-  // CTA pairs (cta_group::2, validated on B200: scripts/check_2cta.py): default on, RAVE_TC_2CTA=0 disables.
-  // Needs N % 32 == 0, a K-block of 64 (the tested configuration) and at least two M tiles.
-  const bool use2 = want2 && (BN % 32 == 0) && BN >= 64 && (long)p.n_lt * p.n_bg >= 2;
 
   // A: channel-last activations viewed as (c, phase, l/stride, b)
   CUtensorMap ta, tb;
@@ -1295,50 +586,16 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   {
     cuuint64_t dims[2] = {(cuuint64_t)Cin, (cuuint64_t)K * Cout * (x3 ? 2 : 1)};
     cuuint64_t strides[1] = {(cuuint64_t)Cin * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)(use2 ? BN / 2 : BN)};
+    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BN};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(&tb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(wt), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(BK * 2), promo,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "conv1d_tc: tensor map B encode failed (%d)", (int)r);
   }
-  // ---- TMA-staged epilogue (see TcParams::etma): bf16 chunk operands and the bf16 output as 3-D maps (c, row, batch)
-  CUtensorMap te[3];
-  memset(te, 0, sizeof(te));
-  p.etma = 0; p.in0_kind = p.in1_kind = 0; p.e_stages = 0; p.epi_off = p.bar_off = 0;
-  {
-    const char *e_etma = getenv("RAVE_TC_ETMA");          // read per call: scripts/ablate_tc.py flips it
-    const int want_etma = (e_etma && e_etma[0] == '0') ? 0 : 1;
-    const bool slots_ok = !(dact_src && res_act) && !(fm_d && res_bf16);
-    const bool fm_ok = !fm_d || p.fm_bh == 0 || (p.fm_bh % p.BB == 0);
-    if (want_etma && use2 && !x3 && out_act && p.out_row_stride == 1 && p.out_row_offset == 0 && slots_ok && fm_ok &&
-        (BN % 64 == 0 || Cout == BN) && Cout >= 64) {
-      p.etma = 1;
-      p.in0_kind = dact_src ? 1 : res_act ? 2 : 0;
-      p.in1_kind = fm_d ? 1 : res_bf16 ? 2 : 0;
-      const void *base[3] = {dact_src ? dact_src : res_act,
-                             fm_d ? (const void *)((const __nv_bfloat16 *)dact_src - (fm_bh < 0 ? p.fm_half : 0)) : res_bf16,
-                             out_act};
-      for (int i = 0; i < 3 && p.etma; ++i) {
-        if (!base[i]) continue;
-        cuuint64_t dims[3] = {(cuuint64_t)Cout, (cuuint64_t)Lout, (cuuint64_t)B};
-        cuuint64_t strides[2] = {(cuuint64_t)Cout * 2, (cuuint64_t)Cout * 2 * p.out_rows};
-        cuuint32_t box[3] = {64, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-        cuuint32_t estr[3] = {1, 1, 1};
-        CUresult r = enc(&te[i], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void *>(base[i]), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        if (r != CUDA_SUCCESS) p.etma = 0;        // e.g. a row pitch the TMA unit cannot express: per-thread epilogue
-      }
-      if (!p.etma) p.in0_kind = p.in1_kind = 0;
-    }
-  }
-  p.emode = -1;
-  if (p.etma && !res && !out_f32 && !p.dbg)
-    p.emode = (bias ? 1 : 0) | (act == RAVE_ACT_LEAKY ? 2 : 0) | (p.in0_kind << 2) | (p.in1_kind << 4);
   cudaStream_t s = (cudaStream_t)stream;
-  if (x3) return conv_tc_dispatch_x3(use2, BK, BN, ta, tb, te, p, s);
-  return dispatch_all<false>(use2, BK, BN, ta, tb, te, p, s);
+  if (x3) return conv_tc_dispatch_x3(BK, BN, ta, tb, p, s);
+  return dispatch_all<false>(BK, BN, ta, tb, p, s);
 }
 
 extern "C" int rave_conv1d_tc_fwd(const void *xa, const void *wt, const float *bias, const float *res,
@@ -1370,7 +627,7 @@ extern "C" int rave_conv1d_tc_fwd_x3(const void *xa, const void *wt, const float
 }
 
 // =============================================================================================
-// wgrad on tcgen05:  dWt[k][m][n] += sum_{(b,l)} P[b][l][m] * Q[b][l*stride + k*dil - pad_l][n]
+// wgrad on wgmma:  dWt[k][m][n] += sum_{(b,l)} P[b][l][m] * Q[b][l*stride + k*dil - pad_l][n]
 //
 // P: channel-last bf16 [B][Lp][Cm] (conv: dy, M = Cout), Q: channel-last bf16 [B][Lq][Cn] (conv: the
 // activated operand xa, N = Cin).  The reduction runs over tensor ROWS, so both operands are MN-major
@@ -1390,8 +647,9 @@ struct WgParams {
   int BL, BB, n_lt, n_bg;   // row chunk = BB batches x BL rows (BL*BB == 64)
   int n_mt, n_nt, splits;
   float *dwt;               // [splits][K][Cm][Cn] fp32 partial sums (every element written exactly once)
-  float *dbias;             // [Cm] pre-zeroed or null: += column sums of P (the bias gradient of a conv layer), added
+  float *dbias;             // [Cm] pre-zeroed or null: += column sums of P (the bias gradient of a conv layer), formed
                             // by the tap-0 / n-tile-0 CTAs from the P tiles they stream anyway
+  float *dbias_part;        // [splits][n_mt * 128] their per-slice partial sums (dbias_sum_kernel adds them up)
 };
 
 template <int BLOCK_N>
@@ -1412,14 +670,12 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
   using L = WgSmem<BLOCK_N>;
   constexpr int STAGES = L::STAGES;
   constexpr int NS = L::NS;
-  constexpr uint32_t TMEM_COLS = BLOCK_N <= 32 ? 32 : BLOCK_N <= 64 ? 64 : BLOCK_N <= 128 ? 128 : 256;
+  static_assert(BLOCK_N % 64 == 0 && BLOCK_N <= 128, "MN-major B operand: whole 64-channel slabs");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + L::BAR_OFFSET);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tfull_bar = empty_bar + STAGES;
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(tfull_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -1438,26 +694,22 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
   const int my_chunks = max(0, ch_end - ch_begin);
   const bool do_cs = p.dbias != nullptr && k == 0 && nt == 0;      // this CTA also reduces its P tiles over rows
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_p);
     tma_prefetch_desc(&tmap_q);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], do_cs ? 5 : 1);     // MMA commit (+ the 4 column-sum warps)
+      mbar_init(&empty_bar[s], do_cs ? 8 : 4);     // the 4 MMA warps (+ the 4 column-sum warps)
     }
-    mbar_init(tfull_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   griddep_launch_dependents();      // dependents may begin their prologue ...
   griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
 
+  float *dst = p.dwt + ((size_t)split * p.K + k) * p.Cm * p.Cn;
   if (my_chunks > 0) {
-    if (warp == 0) {
+    if (warp == 4) {
       // warp-uniform producer loop (see elect_one)
       const int off = k * p.dil - p.pad_l;
       int j = off / p.stride;
@@ -1482,106 +734,79 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    } else if (warp == 1) {
-      // bf16 x bf16 -> fp32, A and B both MN-major (bits 15 / 16); warp-uniform issue loop
-      constexpr uint32_t idesc = make_idesc_bf16(128, BLOCK_N) | (1u << 15) | (1u << 16);
+    } else if (warp < 4) {
+      // MMA warpgroup: bf16 x bf16 -> fp32, A and B both MN-major (transposed operands); M half h = P slab h
       const uint32_t smem_base = smem_u32(smem);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
+      float d[2][BLOCK_N / 2];
       int stage = 0;
       uint32_t phase = 0;
       for (int c = 0; c < my_chunks; ++c) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
         const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-        const uint64_t adesc = make_mnmajor_desc(sa, WG_SLAB);
         const uint64_t bdesc = make_mnmajor_desc(sa + 2 * WG_SLAB, WG_SLAB);
-        if (elect_one()) {
+        wgmma_fence();
 #pragma unroll
-          for (int kk = 0; kk < WG_ROWS / 16; ++kk) {
-            // 16 reduction rows = 2048 bytes -> +128 in the (addr >> 4) field
-            umma_f16(tmem_u, adesc + 128 * kk, bdesc + 128 * kk, idesc, (c > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (c == my_chunks - 1) umma_commit(tfull_bar);
+        for (int kk = 0; kk < WG_ROWS / 16; ++kk) {
+          // 16 reduction rows = 2048 bytes -> +128 in the (addr >> 4) field
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            Wgmma<BLOCK_N, 1, 1>::mma(d[h], make_mnmajor_desc(sa + h * WG_SLAB, WG_SLAB) + 128 * kk, bdesc + 128 * kk,
+                                      (c > 0 || kk > 0) ? 1u : 0u);
         }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+        wgmma_fence_regs<BLOCK_N / 2>(d[1]);
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-    } else {
-      if (do_cs) {
-        // bias gradient: column sums of the P tiles while the tensor core consumes them.  Thread = (8-channel group
-        // cg, row residue rg): rows rg, rg+8, ... of both 64-channel slabs, one 16-byte shared load per row.
-        const int te = (warp - 2) * 32 + lane;
-        const int cg = te & 15, rg = te >> 4;
-        const uint32_t col = (uint32_t)(cg >> 3) * WG_SLAB + (uint32_t)(((cg & 7) ^ rg) << 4);
-        float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int c = 0; c < my_chunks; ++c) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint8_t *sa = smem + stage * L::STAGE_BYTES + col;
+      store_wgrad_tile<BLOCK_N>(d, dst, m0, n0, p.Cm, p.Cn);
+    } else if (do_cs) {
+      // bias gradient: column sums of the P tiles while the tensor core consumes them.  Thread = (8-channel group
+      // cg, row residue rg): rows rg, rg+8, ... of both 64-channel slabs, one 16-byte shared load per row.
+      const int te = (warp - 5) * 32 + lane;
+      const int cg = te & 15, rg = te >> 4;
+      const uint32_t col = (uint32_t)(cg >> 3) * WG_SLAB + (uint32_t)(((cg & 7) ^ rg) << 4);
+      float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int c = 0; c < my_chunks; ++c) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint8_t *sa = smem + stage * L::STAGE_BYTES + col;
 #pragma unroll
-          for (int i = 0; i < WG_ROWS / 8; ++i) {
-            const uint4 q = *reinterpret_cast<const uint4 *>(sa + (rg + 8 * i) * 128);
-            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+        for (int i = 0; i < WG_ROWS / 8; ++i) {
+          const uint4 q = *reinterpret_cast<const uint4 *>(sa + (rg + 8 * i) * 128);
+          const uint32_t w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              cs[2 * j] += __uint_as_float(w[j] << 16);
-              cs[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[stage]);
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        float *scratch = reinterpret_cast<float *>(smem + L::CS_OFFSET);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) scratch[rg * 128 + cg * 8 + j] = cs[j];
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        float t = 0.f;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) t += scratch[r * 128 + te];
-        if (m0 + te < p.Cm) atomicAdd(p.dbias + m0 + te, t);
-      }
-      const int quad = warp & 3;
-      const int m = m0 + quad * 32 + lane;
-      mbar_wait(tfull_bar, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-      float *dst = p.dwt + (((size_t)split * p.K + k) * p.Cm + m) * p.Cn + n0;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BLOCK_N; c0 += 16) {
-        float v[16];
-        tmem_ld_32x16(taddr + c0, v);
-        if (m < p.Cm) {
-          if (n0 + c0 + 16 <= p.Cn && (p.Cn & 3) == 0) {
-            float4 *d4 = reinterpret_cast<float4 *>(dst + c0);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) d4[i] = make_float4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-          } else {
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-              if (n0 + c0 + i < p.Cn) dst[c0 + i] = v[i];
+          for (int j = 0; j < 4; ++j) {
+            cs[2 * j] += __uint_as_float(w[j] << 16);
+            cs[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
           }
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      float *scratch = reinterpret_cast<float *>(smem + L::CS_OFFSET);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) scratch[rg * 128 + cg * 8 + j] = cs[j];
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      float t = 0.f;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) t += scratch[r * 128 + te];
+      p.dbias_part[(size_t)split * p.n_mt * 128 + m0 + te] = t;
     }
-  } else if (warp >= 2) {
+  } else if (do_cs && warp >= 5) {
+    // empty slice: no rows, zero partial bias gradient
+    p.dbias_part[(size_t)split * p.n_mt * 128 + m0 + (warp - 5) * 32 + lane] = 0.f;
+  } else if (warp < 4) {
     // empty slice (more splits than row chunks): this CTA still owns its partial tile -> zeros
-    const int quad = warp & 3;
-    const int m = m0 + quad * 32 + lane;
+    const int m = m0 + threadIdx.x;
     if (m < p.Cm) {
-      float *dst = p.dwt + (((size_t)split * p.K + k) * p.Cm + m) * p.Cn + n0;
       for (int c = 0; c < BLOCK_N; ++c)
-        if (n0 + c < p.Cn) dst[c] = 0.f;
+        if (n0 + c < p.Cn) dst[(size_t)m * p.Cn + n0 + c] = 0.f;
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -1627,15 +852,8 @@ static int launch_wg(const CUtensorMap &tp, const CUtensorMap &tq, const WgParam
 namespace rave {
 namespace tc {
 static int wg_block_n(int Cn) {
-  int BN = 256;
-  if (Cn <= 256) BN = (Cn + 15) / 16 * 16;
-  else if (Cn % 256 == 0) BN = 256;
-  else if (Cn % 192 == 0) BN = 192;
-  else if (Cn % 128 == 0) BN = 128;
-  const int valid_bn[] = {16, 32, 48, 64, 96, 128, 192, 256};
-  for (int v : valid_bn)
-    if (v >= BN) return v;
-  return 256;
+  // whole 64-channel slabs of the MN-major Q operand; N <= 128: the accumulators live in the MMA warpgroup's registers
+  return Cn <= 64 ? 64 : 128;
 }
 static void wg_geometry(int B, int Cm, int Lp, int Cn, int K, int *BL, int *n_lt, int *n_bg, int *n_mt, int *BN,
                         int *n_nt, int *splits) {
@@ -1649,7 +867,7 @@ static void wg_geometry(int B, int Cm, int Lp, int Cn, int K, int *BL, int *n_lt
   *n_nt = ceil_div(Cn, *BN);
   const int tiles = K * (*n_mt) * (*n_nt);
   const int n_chunks = (*n_lt) * (*n_bg);
-  int s = ceil_div(tiles >= 74 ? 148 : 2 * 148, tiles);     // many tiles already: one wave-and-a-bit is enough
+  int s = ceil_div(tiles >= 66 ? 132 : 2 * 132, tiles);     // many tiles already: one wave-and-a-bit is enough
   if (s > 32) s = 32;      // every slice writes a full partial tile that the weight-norm backward re-reads
   // ... and a slice of only a few 64-row chunks is all prologue + partial-tile write (the encoder / decoder blocks:
   // 2.4 GFLOP in 40 us): at least 8 chunks per slice
@@ -1712,18 +930,31 @@ extern "C" int rave_conv1d_tc_wgrad(const void *P, const void *Q, float *dwt, fl
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "wgrad_tc: tensor map Q encode failed (%d)", (int)r);
   }
-  switch (BN) {
-    case 16: return launch_wg<16>(tp, tq, p, s);
-    case 32: return launch_wg<32>(tp, tq, p, s);
-    case 48: return launch_wg<48>(tp, tq, p, s);
-    case 64: return launch_wg<64>(tp, tq, p, s);
-    case 96: return launch_wg<96>(tp, tq, p, s);
-    case 128: return launch_wg<128>(tp, tq, p, s);
-    case 192: return launch_wg<192>(tp, tq, p, s);
-    case 256: return launch_wg<256>(tp, tq, p, s);
+  p.dbias_part = nullptr;
+  if (dbias && cudaMallocAsync((void **)&p.dbias_part, sizeof(float) * p.splits * p.n_mt * 128, s) != cudaSuccess) {
+    set_error("wgrad_tc: cudaMallocAsync of the bias-gradient partials failed");
+    return 2;
   }
-  set_error("wgrad_tc: no kernel for BLOCK_N=%d", BN);
-  return 1;
+  int rc = 1;
+  switch (BN) {
+    case 64: rc = launch_wg<64>(tp, tq, p, s); break;
+    case 128: rc = launch_wg<128>(tp, tq, p, s); break;
+    default: set_error("wgrad_tc: no kernel for BLOCK_N=%d", BN);
+  }
+  if (dbias) {
+    if (rc == 0) {
+      dbias_sum_kernel<<<ceil_div(Cm, 256), 256, 0, s>>>(p.dbias_part, dbias, p.splits, p.n_mt * 128, Cm);
+      cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) {
+        set_error("wgrad_tc: dbias_sum launch failed: %s", cudaGetErrorString(e));
+        rc = 2;
+      } else {
+        count_launch();
+      }
+    }
+    cudaFreeAsync(p.dbias_part, s);
+  }
+  return rc;
 }
 
 extern "C" int rave_tapmajor_to_weight_f32(const float *dwt, float *dw, int Cm, int Cn, int K, int transpose,
@@ -1732,7 +963,7 @@ extern "C" int rave_tapmajor_to_weight_f32(const float *dwt, float *dw, int Cm, 
   RAVE_CHECK_ARG(dwt && dw && Cm > 0 && Cn > 0 && K > 0, "tapmajor_to_weight: bad argument");
   const long total = (long)K * Cm * Cn;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   RAVE_CHECK_ARG(splits >= 1, "tapmajor_to_weight: splits must be >= 1");
   tc::tapmajor_to_weight_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(dwt, dw, Cm, Cn, K, transpose, splits);
   RAVE_CHECK_LAUNCH("tapmajor_to_weight");

@@ -74,11 +74,11 @@ act_fwd_kernel(const float *__restrict__ x, float *__restrict__ y, int C, int L,
     y[base + t] = act_apply(x[base + t], act, slope, al);
 }
 
-// dx = dy * act'(x); Snake: dalpha[c] += sum dy * d/dalpha  (atomic over CTAs; dalpha pre-zeroed)
+// dx = dy * act'(x); Snake: dalpha[c] += sum dy * d/dalpha  (block-order sum over CTAs; dalpha pre-zeroed)
 __global__ void __launch_bounds__(256)
 act_bwd_kernel(const float *__restrict__ dy, const float *__restrict__ x, float *__restrict__ dx,
                float *__restrict__ dalpha, int C, int L, int act, float slope,
-               const float *__restrict__ alpha) {
+               const float *__restrict__ alpha, const BlockSum bs) {
   __shared__ float red[32];
   const int c = blockIdx.y, b = blockIdx.z;
   const float al = (act == RAVE_ACT_SNAKE) ? alpha[c] : 0.f;
@@ -94,9 +94,10 @@ act_bwd_kernel(const float *__restrict__ dy, const float *__restrict__ x, float 
       s += g * (xv * sinf(2.f * al * xv) / ae - sn * sn / (ae * ae));
     }
   }
-  if (act == RAVE_ACT_SNAKE && dalpha) {
+  if (act == RAVE_ACT_SNAKE && dalpha) {      // uniform over the grid
     const float tot = block_reduce_sum(s, red);
-    if (threadIdx.x == 0) atomicAdd(dalpha + c, tot);
+    if (threadIdx.x == 0) block_sum_put(bs, 0, tot);
+    block_sum_finish(bs, dalpha);             // one group per channel (grid y)
   }
 }
 
@@ -168,7 +169,7 @@ am_tanh_bwd_kernel(const float *__restrict__ dy, const float *__restrict__ x, fl
 // (the reference's ~14 elementwise / reduction launches on a 0.26 M element tensor).  kl_sum must be zeroed by the caller.
 __global__ void __launch_bounds__(256)
 reparam_fwd_kernel(const float *__restrict__ z, const float *__restrict__ eps, float *__restrict__ zs,
-                   float *__restrict__ kl_sum, long CL, long total) {
+                   float *__restrict__ kl_sum, long CL, long total, const BlockSum bs) {
   __shared__ float red[32];
   float acc = 0.f;
   for (long i = blockIdx.x * 256L + threadIdx.x; i < total; i += (long)gridDim.x * 256) {
@@ -182,7 +183,8 @@ reparam_fwd_kernel(const float *__restrict__ z, const float *__restrict__ eps, f
     acc += mean * mean + var - logf(var) - 1.f;
   }
   const float tot = block_reduce_sum(acc, red);
-  if (threadIdx.x == 0) atomicAdd(kl_sum, tot);
+  if (threadIdx.x == 0) block_sum_put(bs, 0, tot);
+  block_sum_finish(bs, kl_sum);
 }
 
 // y = bf16(act(x)); grid (ceil(L/2048), C, B), 2 elements per thread-iteration
@@ -246,7 +248,7 @@ extern "C" int rave_act_fwd(const float *x, float *y, int B, int C, int L, int a
     const long n = (long)B * C * L;
     const int vec = (((uintptr_t)x | (uintptr_t)y) & 15) == 0;
     long blocks = ((vec ? n / 4 : n) + 255) / 256;
-    blocks = blocks < 1 ? 1 : (blocks > 148 * 16 ? 148 * 16 : blocks);
+    blocks = blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks);
     act_flat_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, y, n, act, slope, vec);
     RAVE_CHECK_LAUNCH("act_fwd");
     return 0;
@@ -267,14 +269,19 @@ extern "C" int rave_act_bwd(const float *dy, const float *x, float *dx, float *d
     const long n = (long)B * C * L;
     const int vec = (((uintptr_t)x | (uintptr_t)dy | (uintptr_t)dx) & 15) == 0;
     long blocks = ((vec ? n / 4 : n) + 255) / 256;
-    blocks = blocks < 1 ? 1 : (blocks > 148 * 16 ? 148 * 16 : blocks);
+    blocks = blocks < 1 ? 1 : (blocks > 132 * 16 ? 132 * 16 : blocks);
     act_flat_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(dy, x, dx, n, act, slope, vec);
     RAVE_CHECK_LAUNCH("act_bwd");
     return 0;
   }
   if (act == RAVE_ACT_SNAKE && dalpha) cudaMemsetAsync(dalpha, 0, sizeof(float) * C, (cudaStream_t)stream);
   dim3 grid(ceil_div(L, 1024), C, B);
-  act_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dy, x, dx, dalpha, C, L, act, slope, alpha);
+  BlockSum bs;
+  memset(&bs, 0, sizeof(bs));
+  if (dalpha)
+    if (int rc = block_sum_begin(&bs, (long)grid.x * grid.y * grid.z, 1, (cudaStream_t)stream, 1)) return rc;
+  act_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(dy, x, dx, dalpha, C, L, act, slope, alpha, bs);
+  if (dalpha) block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("act_bwd");
   return 0;
 }
@@ -284,7 +291,7 @@ extern "C" int rave_am_tanh_fwd(const float *x, float *y, int B, int C, int L, v
   RAVE_CHECK_ARG(x && y && B > 0 && C > 0 && L > 0, "am_tanh_fwd: bad argument");
   const long total = (long)B * C * L;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   am_tanh_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(x, y, C, L, total);
   RAVE_CHECK_LAUNCH("am_tanh_fwd");
   return 0;
@@ -296,7 +303,7 @@ extern "C" int rave_am_tanh_bwd(const float *dy, const float *x, float *dx, int 
   RAVE_CHECK_ARG(dy && x && dx && B > 0 && C > 0 && L > 0, "am_tanh_bwd: bad argument");
   const long total = (long)B * C * L;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   am_tanh_bwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(dy, x, dx, C, L, total);
   RAVE_CHECK_LAUNCH("am_tanh_bwd");
   return 0;
@@ -307,10 +314,13 @@ extern "C" int rave_reparam_fwd(const float *z, const float *eps, float *zs, flo
   using namespace rave;
   RAVE_CHECK_ARG(z && eps && zs && kl_sum && B > 0 && C > 0 && L > 0, "reparam_fwd: bad argument");
   const long total = (long)B * C * L;
-  int blocks = (int)((total + 1023) / 1024);            // ~4 elements per thread: few atomics, still every SM busy
-  if (blocks > 148 * 4) blocks = 148 * 4;
+  int blocks = (int)((total + 1023) / 1024);            // ~4 elements per thread: few partials, still every SM busy
+  if (blocks > 132 * 4) blocks = 132 * 4;
   if (blocks < 1) blocks = 1;
-  reparam_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z, eps, zs, kl_sum, (long)C * L, total);
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 1, (cudaStream_t)stream)) return rc;
+  reparam_fwd_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(z, eps, zs, kl_sum, (long)C * L, total, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("reparam_fwd");
   return 0;
 }
@@ -334,7 +344,7 @@ extern "C" int rave_weight_to_tapmajor_bf16(const float *w, void *wt_bf16, int C
   RAVE_CHECK_ARG(w && wt_bf16 && Cout > 0 && Cin > 0 && K > 0, "weight_to_tapmajor: bad argument");
   const long total = (long)K * Cout * Cin;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   weight_tapmajor_kernel<<<blocks, 256, 0, (cudaStream_t)stream>>>(w, (__nv_bfloat16 *)wt_bf16, Cout, Cin,
                                                                   K, transpose, flip);
   RAVE_CHECK_LAUNCH("weight_to_tapmajor");
@@ -603,8 +613,7 @@ extern "C" int rave_weight_norm_bwd_tapmajor(const float *dwt, const float *v, c
 
 // ---------------------------------------------------------------------------------------------
 // multi-tensor variants: ONE launch prepares (or back-propagates through the weight norm of) every
-// layer of a chain.  Per-layer launches of these tiny kernels were 11 % of the bf16 training step
-// (profiles/r1_launches_bf16_summary.md); the descriptor table travels by value in the kernel
+// layer of a chain instead of one launch per layer of these tiny kernels; the descriptor table travels by value in the kernel
 // parameters (<= 64 layers per launch).
 // ---------------------------------------------------------------------------------------------
 namespace rave {
@@ -819,7 +828,7 @@ __global__ void __launch_bounds__(1024) mt_wn_bwd_kernel(const __grid_constant__
 }  // namespace rave
 
 // ---------------------------------------------------------------------------------------------
-// Snake on the engine's channel-last bf16 streams (v3 chains on the tcgen05 kernels): the producing conv writes the
+// Snake on the engine's channel-last bf16 streams (v3 chains on the wgmma kernels): the producing conv writes the
 // pre-activation h as bf16, these kernels turn it into the operand a = h + sin^2(alpha h) / (alpha + 1e-9) of the next
 // conv (rave/blocks.py:852-860; alpha per channel) and back: g_h = g_a (1 + alpha sin(2 alpha h) / (alpha + 1e-9)) + add,
 // dalpha[c] += sum_rows g_a (h sin(2 alpha h) / (alpha+eps) - sin^2(alpha h) / (alpha+eps)^2).  Rows = B * pitch (slack
@@ -851,7 +860,7 @@ snake_cl_fwd_kernel(const __nv_bfloat16 *__restrict__ h, const float *__restrict
 __global__ void __launch_bounds__(256)
 snake_cl_bwd_kernel(const __nv_bfloat16 *__restrict__ ga, const __nv_bfloat16 *__restrict__ h,
                     const float *__restrict__ alpha, const __nv_bfloat16 *__restrict__ add,
-                    __nv_bfloat16 *__restrict__ gh, float *__restrict__ dalpha, long rows, int C, int rows_per_block) {
+                    __nv_bfloat16 *__restrict__ gh, float *__restrict__ dalpha, long rows, int C, int rows_per_block, const BlockSum bs) {
   __shared__ float red[32][64 + 1];
   const int cvl = threadIdx.x & 7, rl = threadIdx.x >> 3;
   const int c0 = blockIdx.x * 64 + cvl * 8;
@@ -893,7 +902,7 @@ snake_cl_bwd_kernel(const __nv_bfloat16 *__restrict__ ga, const __nv_bfloat16 *_
       *reinterpret_cast<uint4 *>(gh + o) = make_uint4(out[0], out[1], out[2], out[3]);
     }
   }
-  if (!dalpha) return;
+  if (!dalpha) return;                      // uniform over the grid
 #pragma unroll
   for (int j = 0; j < 8; ++j) red[rl][cvl * 8 + j] = part[j];
   __syncthreads();
@@ -901,9 +910,9 @@ snake_cl_bwd_kernel(const __nv_bfloat16 *__restrict__ ga, const __nv_bfloat16 *_
     float t = 0.f;
 #pragma unroll
     for (int r = 0; r < 32; ++r) t += red[r][threadIdx.x];
-    const int c = blockIdx.x * 64 + threadIdx.x;
-    if (c < C) atomicAdd(dalpha + c, t);
+    block_sum_put(bs, threadIdx.x, t);
   }
+  block_sum_finish(bs, dalpha);             // one group of 64 channels per grid column
 }
 
 }  // namespace rave
@@ -914,14 +923,14 @@ extern "C" int rave_snake_cl_fwd(const void *h_bf16, const float *alpha, void *a
                      (((uintptr_t)h_bf16 | (uintptr_t)a_bf16) & 15) == 0, "snake_cl_fwd: bad argument (C %% 8, 16-byte rows)");
   const long n_vec = rows * (C / 8);
   long blocks = (n_vec + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   snake_cl_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)h_bf16, alpha,
                                                                      (__nv_bfloat16 *)a_bf16, n_vec, C / 8);
   RAVE_CHECK_LAUNCH("snake_cl_fwd");
   return 0;
 }
 
-// dalpha [C] fp32 must be zeroed by the caller (accumulated with atomics); `add` (bf16, same shape) may be null.
+// dalpha [C] fp32 must be zeroed by the caller (accumulated across blocks); `add` (bf16, same shape) may be null.
 extern "C" int rave_snake_cl_bwd(const void *ga_bf16, const void *h_bf16, const float *alpha, const void *add_bf16,
                                  void *gh_bf16, float *dalpha, long rows, int C, void *stream) {
   using namespace rave;
@@ -930,13 +939,20 @@ extern "C" int rave_snake_cl_bwd(const void *ga_bf16, const void *h_bf16, const 
                  "snake_cl_bwd: bad argument (C %% 8, 16-byte rows)");
   const int gx = (C + 63) / 64;
   long gy = (rows + 255) / 256;                 // >= 256 rows per block
-  const long cap = (148L * 8 + gx - 1) / gx;
+  const long cap = (132L * 8 + gx - 1) / gx;
   if (gy > cap) gy = cap;
   if (gy < 1) gy = 1;
   const int rpb = (int)((rows + gy - 1) / gy);
+  BlockSum bs;
+  memset(&bs, 0, sizeof(bs));
+  if (dalpha) {
+    if (int rc = block_sum_begin(&bs, (long)gx * gy, 64, (cudaStream_t)stream, 0)) return rc;
+    bs.limit = C;
+  }
   snake_cl_bwd_kernel<<<dim3(gx, (unsigned)gy), 256, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16 *)ga_bf16, (const __nv_bfloat16 *)h_bf16, alpha, (const __nv_bfloat16 *)add_bf16,
-      (__nv_bfloat16 *)gh_bf16, dalpha, rows, C, rpb);
+      (__nv_bfloat16 *)gh_bf16, dalpha, rows, C, rpb, bs);
+  if (dalpha) block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("snake_cl_bwd");
   return 0;
 }

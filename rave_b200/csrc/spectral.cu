@@ -3,7 +3,7 @@
 // the input (X) and of the reconstruction (Y), one scale per launch:
 //     lin = mean((|X|-|Y|)^2) / mean(|X|^2)          log = mean(| log(|X|+eps) - log(|Y|+eps) |)
 // forward : stats[0] += sum (|X|-|Y|)^2, stats[1] += sum |X|^2, stats[2] += sum |log(|X|+eps) - log(|Y|+eps)|;
-//           the last block to finish (ticket in stats[3]) writes the distance stats[4] = s0/s1 + s2/n, so the
+//           the last block to finish (block-order sums, see BlockSum) writes the distance stats[4] = s0/s1 + s2/n, so the
 //           scalar tail costs no extra launches
 // backward: dY = ( c_lin * -2 (|X|-|Y|) + c_log * -sgn(logX - logY) / (|Y|+eps) ) * Y/|Y|, c_lin = g/s1, c_log = g/n
 //           with the upstream gradient g read from device memory
@@ -15,7 +15,7 @@ namespace rave {
 
 __global__ void __launch_bounds__(256)
 spectral_stats_kernel(const float2 *__restrict__ X, const float2 *__restrict__ Y, float *__restrict__ stats, long n,
-                      float eps) {
+                      float eps, const BlockSum bs) {
   __shared__ float red[3][8];
   float s0 = 0.f, s1 = 0.f, s2 = 0.f;
   for (long i = blockIdx.x * 256L + threadIdx.x; i < n; i += (long)gridDim.x * 256) {
@@ -39,18 +39,9 @@ spectral_stats_kernel(const float2 *__restrict__ X, const float2 *__restrict__ Y
   if (threadIdx.x < 3) {
     float t = 0.f;
     for (int i = 0; i < 8; ++i) t += red[threadIdx.x][i];
-    atomicAdd(stats + threadIdx.x, t);
-    __threadfence();
+    block_sum_put(bs, threadIdx.x, t);
   }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned ticket = atomicAdd(reinterpret_cast<unsigned *>(stats + 3), 1u);
-    if (ticket == gridDim.x - 1) {
-      __threadfence();
-      const float s0 = atomicAdd(stats, 0.f), s1 = atomicAdd(stats + 1, 0.f), s2 = atomicAdd(stats + 2, 0.f);
-      stats[4] = s0 / s1 + s2 / (float)n;
-    }
-  }
+  if (block_sum_finish(bs, stats) && threadIdx.x == 0) stats[4] = stats[0] / stats[1] + stats[2] / (float)n;
 }
 
 __global__ void __launch_bounds__(256)
@@ -165,7 +156,7 @@ extern "C" int rave_rfft_bwd_scale(const void *G_c64, void *Z_c64, long N, int F
   RAVE_CHECK_ARG(G_c64 && Z_c64 && N > 0 && F > 0 && bins > 1, "rfft_bwd_scale: bad argument");
   const long total = N * F * bins;
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   rfft_bwd_scale_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const float2 *)G_c64, (float2 *)Z_c64, total, F,
                                                                        bins, sN, sF, sB, (float)(2 * (bins - 1)));
   RAVE_CHECK_LAUNCH("rfft_bwd_scale");
@@ -181,7 +172,7 @@ extern "C" int rave_stft_frames(const float *x, const float *window, float *fram
   const int F = 1 + T / hop;
   const long total4 = (long)N * F * (n_fft / 4);
   long blocks = (total4 + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   const int vec_ok = (T % 4 == 0) && (((uintptr_t)x & 15) == 0);
   stft_frames_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, window, frames, total4, T, n_fft, hop, F, vec_ok);
   RAVE_CHECK_LAUNCH("stft_frames");
@@ -196,7 +187,7 @@ extern "C" int rave_stft_frames_bwd(const float *dframes, const float *window, f
   const int F = 1 + T / hop;
   const long total = (long)N * T;
   long blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   stft_frames_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(dframes, window, dx, total, T, n_fft, hop, F);
   RAVE_CHECK_LAUNCH("stft_frames_bwd");
   return 0;
@@ -206,9 +197,12 @@ extern "C" int rave_spectral_stats(const void *X, const void *Y, float *stats, l
   using namespace rave;
   RAVE_CHECK_ARG(X && Y && stats && n > 0, "spectral_stats: bad argument");
   long blocks = (n + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
+  BlockSum bs;
+  if (int rc = block_sum_begin(&bs, blocks, 3, (cudaStream_t)stream)) return rc;
   spectral_stats_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const float2 *)X, (const float2 *)Y, stats, n,
-                                                                       eps);
+                                                                       eps, bs);
+  block_sum_end(bs, (cudaStream_t)stream);
   RAVE_CHECK_LAUNCH("spectral_stats");
   return 0;
 }
@@ -218,7 +212,7 @@ extern "C" int rave_spectral_grad(const void *X, const void *Y, void *dY, const 
   using namespace rave;
   RAVE_CHECK_ARG(X && Y && dY && stats && gup && n > 0, "spectral_grad: bad argument");
   long blocks = (n + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   spectral_grad_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const float2 *)X, (const float2 *)Y,
                                                                       (float2 *)dY, stats, gup, n, eps);
   RAVE_CHECK_LAUNCH("spectral_grad");

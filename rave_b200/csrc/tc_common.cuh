@@ -1,12 +1,14 @@
-// Raw PTX wrappers for the Blackwell (sm_100a) tensor-core path: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences) and the UMMA shared-memory + instruction descriptors.
-// Bit layouts follow the PTX ISA "tcgen05 matrix descriptors" (the same fields CUTLASS' cute::UMMA
-// SmemDescriptor / InstrDescriptor expose).
+// Raw PTX wrappers for the Hopper (sm_90a) tensor-core path: mbarrier, TMA (cp.async.bulk.tensor), wgmma (fence /
+// commit / wait, shared-memory matrix descriptors) and the shared-memory accumulator hand-over between the MMA
+// warpgroup and the epilogue warps.  Bit layouts follow the PTX ISA "Matrix Descriptor Format" of wgmma (the fields
+// CUTLASS' cute::GMMA::GmmaDescriptor exposes).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
+
+#include "wgmma_sm90.cuh"
 
 namespace rave {
 namespace tc {
@@ -56,25 +58,25 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   }
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): one full 32-byte sector per lane; 32-byte aligned addresses
+// 32-byte row segments (32-byte aligned) as two 128-bit accesses
 __device__ __forceinline__ void ldg256(const void *p, uint32_t *r) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "l"(p));
+  asm volatile("ld.global.nc.v4.b32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
+               : "l"(reinterpret_cast<const uint8_t *>(p) + 16));
 }
 __device__ __forceinline__ void stg256(void *p, const uint32_t *r) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]),
-               "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]) : "memory");
+  asm volatile("st.global.v4.b32 [%0], {%1,%2,%3,%4};" ::"l"(reinterpret_cast<uint8_t *>(p) + 16), "r"(r[4]), "r"(r[5]),
+               "r"(r[6]), "r"(r[7])
                : "memory");
 }
 
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
-// One lane of a fully converged warp.  The producer / MMA-issue loops run WARP-UNIFORM (all 32 lanes execute the
-// loop, only the UTMALDG / UTCHMMA / UTCBAR instructions are predicated on the elected lane): stage indices, shared
-// memory addresses and descriptors then live in uniform registers.  Inside an `if (lane == 0)` region the compiler
-// treats them as per-thread values and wraps every UTC/UTMA instruction in an ELECT + R2UR.BROADCAST waterfall loop
-// (~25 instructions per MMA: the issue thread, not the tensor pipe, bounded the small-N / BLOCK_K=32 layers).
+// One lane of a fully converged warp.  The producer loops run WARP-UNIFORM (all 32 lanes execute the loop, only the
+// TMA instructions are predicated on the elected lane): stage indices, shared-memory addresses and coordinates then
+// live in uniform registers instead of being broadcast from one lane per instruction.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -145,148 +147,100 @@ __device__ __forceinline__ void sts128(void *p, const uint32_t *r) {
                : "memory");
 }
 
-// ------------------------------------------------------------------ tcgen05
-__device__ __forceinline__ void tmem_alloc(uint32_t *dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, bf16/fp16 operands, fp32 accumulate; single thread issues
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// same, tf32 operands (fp32 bit patterns in shared memory)
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once every tcgen05 op previously issued by this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t *bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// 32 lanes x 32 columns of fp32 accumulators -> 32 registers per thread (thread i <-> TMEM lane base+i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float *v) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// ------------------------------------------------------------------ wgmma (sm_90a)
+// One warpgroup (4 warps, 128 threads) issues every MMA of a 128-row tile as two m64 halves and holds the fp32
+// accumulators in registers: d[h][N/2] for rows 64 h .. 64 h + 63.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float *d) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float *v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ------------------------------------------------------------------ CTA pairs (cta_group::2)
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
+// Accumulator hand-over.  The warps of an epilogue own one ROW of a 128-row tile each (thread = row quad * 32 + lane)
+// and read consecutive columns; wgmma leaves row pieces spread over the lanes of its warpgroup.  The MMA warpgroup
+// therefore stores a finished tile to a shared-memory buffer [128][ld] fp32 (ld = 4 mod 32 words: the 8 lanes of a
+// 16-byte-load phase hit disjoint banks) and the epilogue reads it back with acc_ld_*.  An accumulator address is
+// (row << 16) | column, relative to the buffer set by acc_bind.
+static __shared__ uint32_t s_acc_addr, s_acc_ld;
+__host__ __device__ constexpr int acc_pitch(int cols) { return (cols + 31) / 32 * 32 + 4; }
+__device__ __forceinline__ void acc_bind(const void *buf, int ld) {    // one thread, before the block-wide barrier
+  s_acc_addr = smem_u32(buf);
+  s_acc_ld = (uint32_t)ld;
 }
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
+// store the warpgroup's accumulators of a 128 x N tile (wgmma fragment: d[4j + {0,1}] at row 16 warp + lane / 4,
+// columns 8 j + 2 (lane % 4) + {0,1}; d[4j + {2,3}] eight rows further down) at column `col0` of the buffer
+template <int N>
+__device__ __forceinline__ void acc_store(const float (*d)[N / 2], int wg_thread, int col0 = 0) {
+  const int w = wg_thread >> 5, l = wg_thread & 31;
+  const uint32_t ld = s_acc_ld;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const uint32_t r0 = (uint32_t)(64 * h + 16 * w + (l >> 2));
+#pragma unroll
+    for (int j = 0; j < N / 8; ++j) {
+      const uint32_t c = (uint32_t)(col0 + 8 * j + 2 * (l & 3));
+      const uint32_t a0 = s_acc_addr + (r0 * ld + c) * 4u, a1 = a0 + 8u * ld * 4u;
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0), "f"(d[h][4 * j]), "f"(d[h][4 * j + 1]) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a1), "f"(d[h][4 * j + 2]), "f"(d[h][4 * j + 3]) : "memory");
+    }
+  }
 }
-// shared::cluster address of `bar` in the LEADER CTA of the pair (peer bit cleared)
-__device__ __forceinline__ uint32_t leader_bar_addr(const uint64_t *bar) { return smem_u32(bar) & 0xFEFFFFFFu; }
-// arrive on the barrier at the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint64_t *bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t"
-      ".reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t"
-      "}" ::"r"(smem_u32(bar)),
-      "r"(rank)
-      : "memory");
+// NC consecutive fp32 accumulators of row (taddr >> 16) + lane, from column taddr & 0xFFFF
+template <int NC>
+__device__ __forceinline__ void acc_ld(uint32_t taddr, float *v) {
+  const uint32_t row = (taddr >> 16) + (threadIdx.x & 31), col = taddr & 0xFFFFu;
+  const uint32_t a = s_acc_addr + (row * s_acc_ld + col) * 4u;
+#pragma unroll
+  for (int i = 0; i < NC / 4; ++i)
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                 : "=f"(v[4 * i]), "=f"(v[4 * i + 1]), "=f"(v[4 * i + 2]), "=f"(v[4 * i + 3])
+                 : "r"(a + 16u * i)
+                 : "memory");
 }
-// TMA loads issued by either CTA of a pair; the bytes are accounted on the LEADER's barrier
-__device__ __forceinline__ void tma_load_2d_2sm(void *smem, const CUtensorMap *m, uint64_t *bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(m), "r"(leader_bar_addr(bar)), "r"(c0), "r"(c1)
-      : "memory");
+__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float *v) { acc_ld<32>(taddr, v); }
+__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float *v) { acc_ld<16>(taddr, v); }
+
+// Stores the warpgroup's 128 x BLOCK_N accumulator tile (wgmma fragment layout, see acc_store) into dst rows m0 ..
+// (row pitch Cn, columns from n0), clipped to Cm x Cn.  Cn is a multiple of 8, so a fragment pair is valid as a whole.
+template <int BLOCK_N>
+__device__ __forceinline__ void store_wgrad_tile(const float (*d)[BLOCK_N / 2], float *dst, int m0, int n0, int Cm,
+                                                 int Cn) {
+  const int w = (threadIdx.x & 127) >> 5, l = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int m = m0 + 64 * h + 16 * w + (l >> 2) + 8 * r;
+      if (m >= Cm) continue;
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (l & 3);
+        if (n < Cn)
+          *reinterpret_cast<float2 *>(dst + (size_t)m * Cn + n) = make_float2(d[h][4 * j + 2 * r], d[h][4 * j + 2 * r + 1]);
+      }
+    }
+  }
 }
-__device__ __forceinline__ void tma_load_4d_2sm(void *smem, const CUtensorMap *m, uint64_t *bar, int c0, int c1,
-                                                int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(smem)), "l"(m), "r"(leader_bar_addr(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t *dst_smem, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem of both CTAs] (+)= A * B^T with M = 256 split over the pair; issued by the leader only
-__device__ __forceinline__ void umma_f16_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive (once all prior MMAs of this thread retired) on the barrier at the same offset in BOTH CTAs
-__device__ __forceinline__ void umma_commit_2sm(uint64_t *bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
+
+// Bias gradient of the weight-gradient kernels: the column-sum CTAs of every split-K slice write their partial sums to
+// part[split][m] (no atomics: the slices would add in arrival order), this kernel adds them up in slice order.
+template <int UNUSED = 0>
+__global__ void __launch_bounds__(256) dbias_sum_kernel(const float *__restrict__ part, float *__restrict__ dbias,
+                                                        int splits, int pitch, int Cm) {
+  const int m = blockIdx.x * 256 + threadIdx.x;
+  if (m >= Cm) return;
+  float t = 0.f;
+  for (int s = 0; s < splits; ++s) t += part[(size_t)s * pitch + m];
+  dbias[m] += t;
 }
 
 // ------------------------------------------------------------------ programmatic dependent launch
-// Every tcgen05 kernel finishes its prologue (barrier init, TMEM allocation, tensor-map prefetch) and then WAITS for the
+// Every tensor-core kernel finishes its prologue (barrier init, tensor-map prefetch) and then WAITS for the
 // grids it depends on (griddepcontrol.wait: full completion + memory flush of the previous kernels in the stream); it
 // also lets its own dependents start early (launch_dependents).  Launched with the programmatic-stream-serialization
 // attribute (launch_pdl), the next kernel's CTAs take SMs as soon as this one's CTAs leave them, so its launch latency
@@ -329,17 +283,19 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
 }
 
 // ------------------------------------------------------------------ descriptors
-// layout_type: 2 = SWIZZLE_128B, 4 = SWIZZLE_64B, 6 = SWIZZLE_32B (cute::UMMA::LayoutType)
-__host__ __device__ constexpr uint32_t umma_layout_for_swizzle(int swizzle_bytes) {
-  return swizzle_bytes == 128 ? 2u : (swizzle_bytes == 64 ? 4u : (swizzle_bytes == 32 ? 6u : 0u));
+// wgmma shared-memory matrix descriptor: start address, LBO, SBO (all >> 4), layout type in bits 62-63
+// (1 = SWIZZLE_128B, 2 = SWIZZLE_64B, 3 = SWIZZLE_32B).  The swizzle is a function of the absolute shared-memory
+// address (as TMA writes it), so a start address moved by whole rows or by 32 bytes inside a row stays valid.
+__host__ __device__ constexpr uint64_t wgmma_layout_for_swizzle(int swizzle_bytes) {
+  return swizzle_bytes == 128 ? 1ull : (swizzle_bytes == 64 ? 2ull : (swizzle_bytes == 32 ? 3ull : 0ull));
 }
 // K-major operand tile whose rows are exactly one swizzle span wide: SBO = 8 rows * span, LBO unused
 __device__ __forceinline__ uint64_t make_kmajor_desc(uint32_t smem_addr, int swizzle_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
+  d |= (uint64_t)1 << 16;
   d |= (uint64_t)(((8u * (uint32_t)swizzle_bytes) >> 4) & 0x3FFF) << 32;  // stride byte offset
-  d |= 1ull << 46;                                                         // descriptor version (sm_100)
-  d |= (uint64_t)umma_layout_for_swizzle(swizzle_bytes) << 61;
+  d |= wgmma_layout_for_swizzle(swizzle_bytes) << 62;
   return d;
 }
 // MN-major operand (the reduction runs over tile ROWS, channels are contiguous): 64-channel slabs of 128-byte rows,
@@ -349,16 +305,8 @@ __device__ __forceinline__ uint64_t make_mnmajor_desc(uint32_t smem_addr, uint32
   d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;   // stride between 64-channel slabs
   d |= (uint64_t)((1024u >> 4) & 0x3FFF) << 32;        // stride between 8-row groups
-  d |= 1ull << 46;
-  d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
+  d |= 1ull << 62;                                     // SWIZZLE_128B
   return d;
-}
-// instruction descriptor: bf16 x bf16 -> fp32, both operands K-major, M x N tile
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t make_idesc_tf32(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
 }
 
 }  // namespace tc

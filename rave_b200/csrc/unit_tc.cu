@@ -1,27 +1,29 @@
-// Fused Residual(DilatedUnit) forward on tcgen05 (sm_100a):
+// Fused Residual(DilatedUnit) forward on wgmma (sm_90a):
 //
 //     out = x + Conv1x1( LeakyReLU( Conv3_dil( LeakyReLU(x) ) ) )            rave/blocks.py:31-45 (Residual), 83-112 (DilatedUnit)
 //
 // in ONE kernel.  The reference runs 2 cuDNN convs + 2 activations + pads + the add (7 kernels, 5 HBM round trips);
-// the per-layer tcgen05 path (conv_tc.cu) still needed 2 launches with the intermediate operand a1 = LeakyReLU(conv3)
+// the per-layer tensor-core path (conv_tc.cu) still needed 2 launches with the intermediate operand a1 = LeakyReLU(conv3)
 // going through HBM.  Here a CTA owns a tile of 128 time steps x ALL C channels:
 //
-//   phase 1   acc[128 x NC] (TMEM) = sum_{tap k<3} sum_kb  A_k[128 x BK] (TMA, rows shifted by k*dil - pad) * W3_k[NC x BK]^T
-//   epilogue1 TMEM -> LeakyReLU -> bf16 -> shared memory, written directly in the K-major swizzled layout the tensor
+//   phase 1   acc[128 x NC] (registers of the MMA warpgroup) = sum_{tap k<3} sum_kb  A_k[128 x BK] (TMA, rows shifted by
+//             k*dil - pad) * W3_k[NC x BK]^T
+//   epilogue1 acc -> LeakyReLU -> bf16 -> shared memory, written directly in the K-major swizzled layout the tensor
 //             core reads (the A operand of phase 2 never leaves the SM); optionally also to HBM (training keeps a1 for the
 //             backward: write-only, no read)
 //   phase 2   acc[128 x NC] = sum_kb  A2[128 x BK] (shared memory) * W1[NC x BK]^T
-//   epilogue2 TMEM + skip -> out (bf16 operand of the next layer and / or the fp32 stream); the skip h = x is
+//   epilogue2 acc + skip -> out (bf16 operand of the next layer and / or the fp32 stream); the skip h = x is
 //             recovered from the unit's own input operand a = LeakyReLU(x) (inverse LeakyReLU), as conv_tc.cu does
 //
-// C = 384 runs both phases in two N chunks of 192 (UMMA N <= 256; the 128 x 384 bf16 A2 tile is 96 KB of shared memory).
-// Two 256-column TMEM buffers alternate between consecutive (phase, chunk) jobs, so the epilogue of one job overlaps
-// the MMAs of the next -- except at the phase-1 -> phase-2 boundary of a tile, where phase 2 needs the complete A2.
+// The channels run in N chunks of NC = 96 (the accumulators of a 128 x NC chunk are NC registers per MMA thread); the
+// 128 x C bf16 A2 tile stays resident (96 KB at C = 384).  A finished chunk goes to a shared-memory buffer that the
+// epilogue reads while the warpgroup computes the next chunk -- except at the phase-1 -> phase-2 boundary of a tile,
+// where phase 2 needs the complete A2.
 // Algorithmic HBM bytes per unit: 2 B*L*C (operand in) + 2 B*L*C (operand out) [+ 2 B*L*C a1 when training] + 8 C^2
-// (weights) -- C = 96, L = 4096, B = 32: 50 MB instead of 126 MB for the two-launch form.
+// (weights) -- C = 96, L = 4096, B = 32: 50 MB of HBM traffic instead of 126 MB for the two-launch form.
 //
-// Warp roles (320 threads): 0 = TMA producer, 1 = MMA issuer (+ TMEM alloc), 2..9 = epilogue (two warps per TMEM lane
-// quadrant, alternate 32-column chunks).
+// Warp roles (416 threads): 0-3 = MMA warpgroup, 4 = TMA producer, 5..12 = epilogue (two warps per 32-row quarter of
+// the tile, alternate 32-column chunks).
 #include <stdlib.h>
 #include <string.h>
 
@@ -31,8 +33,9 @@
 namespace rave {
 namespace tc {
 
-constexpr int U_THREADS = 320;
+constexpr int U_THREADS = 416;
 constexpr int U_EPI_WARPS = 8;
+constexpr int U_SMEM_MAX = 227 * 1024;
 
 struct UnitParams {
   int B, C, L, pitch;          // channel-last [B][pitch][C] operand tensors; L valid rows
@@ -50,7 +53,7 @@ struct UnitParams {
 
 template <int C, int BK>
 struct UnitCfg {
-  static constexpr int NC = C <= 256 ? C : C / 2;             // N chunk (UMMA N <= 256)
+  static constexpr int NC = 96;                               // N chunk: NC accumulator registers per MMA thread
   static constexpr int NCH = C / NC;
   static constexpr int KB = C / BK;                           // K blocks per tap
   static constexpr int SWZ = BK * 2;
@@ -60,13 +63,16 @@ struct UnitCfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_PAD;
   static constexpr int A2_SLAB = 128 * BK * 2;
   static constexpr int A2_BYTES = KB * A2_SLAB;               // the whole [128 x C] bf16 tile
-  static constexpr int MAX_STAGES = (222 * 1024 - A2_BYTES) / STAGE_BYTES;
+  static constexpr int ACC_LD = acc_pitch(NC);
+  static constexpr int ACC_BYTES = 128 * ACC_LD * 4;          // fp32 accumulator hand-over buffer
+  static constexpr int MAX_STAGES = (U_SMEM_MAX - 256 - 1024 - A2_BYTES - ACC_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
   static constexpr int A2_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = A2_OFFSET + A2_BYTES;
+  static constexpr int ACC_OFFSET = A2_OFFSET + A2_BYTES;
+  static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;
   static_assert(STAGES >= 2, "not enough shared memory for a 2-stage pipeline");
-  static_assert(NC % 32 == 0 && NC <= 256, "chunk must be a multiple of 32 columns");
+  static_assert(NC % 32 == 0 && C % NC == 0, "chunk must be a multiple of 32 columns and tile C");
 };
 
 __device__ __forceinline__ float bfl(uint32_t w) { return __uint_as_float(w << 16); }
@@ -78,48 +84,41 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
                        const __grid_constant__ CUtensorMap tmap_w1, const UnitParams p) {
   using L = UnitCfg<C, BK>;
   constexpr int STAGES = L::STAGES, NC = L::NC, NCH = L::NCH, KB = L::KB, SWZ = L::SWZ;
-  constexpr uint32_t TMEM_COLS = 512;                   // two accumulator buffers at columns 0 and 256
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t *a2 = smem + L::A2_OFFSET;
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + L::BAR_OFFSET);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tfull_bar = empty_bar + STAGES;             // [2]
-  uint64_t *tempty_bar = tfull_bar + 2;                 // [2]
-  uint64_t *a2_ready = tempty_bar + 2;                  // epilogue -> MMA: the tile's A2 operand is complete
+  uint64_t *tfull_bar = empty_bar + STAGES;             // MMA -> epilogue: the accumulator buffer holds a chunk
+  uint64_t *tempty_bar = tfull_bar + 1;                 // epilogue -> MMA: the buffer has been read
+  uint64_t *a2_ready = tempty_bar + 1;                  // epilogue -> MMA: the tile's A2 operand is complete
   uint64_t *a2_free = a2_ready + 1;                     // MMA -> epilogue: phase 2 has finished reading A2
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(a2_free + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.n_lt * p.n_bg;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w3);
     tma_prefetch_desc(&tmap_w1);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);                      // one arrival per MMA warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], U_EPI_WARPS);
-    }
+    mbar_init(tfull_bar, 128);
+    mbar_init(tempty_bar, U_EPI_WARPS);
     mbar_init(a2_ready, U_EPI_WARPS);
-    mbar_init(a2_free, 1);
+    mbar_init(a2_free, 4);
     fence_barrier_init();
+    acc_bind(smem + L::ACC_OFFSET, L::ACC_LD);
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   griddep_launch_dependents();      // dependents may begin their prologue ...
   griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
 
-  if (warp == 0) {
+  if (warp == 4) {
     // =========================== TMA producer ===========================
     int stage = 0;
     uint32_t phase = 0;
@@ -155,70 +154,75 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    constexpr uint32_t idesc = make_idesc_bf16(128, NC);
+  } else if (warp < 4) {
+    // =========================== MMA warpgroup ===========================
+    constexpr uint64_t A_HALF = (64 * SWZ) >> 4;         // rows 64 .. 127 of a K-major operand tile
     const uint32_t smem_base = smem_u32(smem);
     const uint32_t a2_base = smem_u32(a2);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
+    float d[2][NC / 2];
     int stage = 0;
     uint32_t phase = 0;
     int job = 0, it = 0;
+    // hand a finished chunk to the epilogue once it has read the previous one
+    auto hand_over = [&]() {
+      mbar_wait(tempty_bar, (job & 1) ^ 1);
+      acc_store<NC>(d, threadIdx.x);
+      mbar_arrive(tfull_bar);
+      ++job;
+    };
+    auto release = [&](bool free_a2) {
+      wgmma_commit();
+      wgmma_wait<0>();
+      wgmma_fence_regs<NC / 2>(d[0]);
+      wgmma_fence_regs<NC / 2>(d[1]);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[stage]);
+        if (free_a2) mbar_arrive(a2_free);               // this warp's MMAs no longer read A2
+      }
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    };
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      for (int ch = 0; ch < NCH; ++ch, ++job) {          // ---- phase 1
-        const int buf = job & 1;
-        mbar_wait(&tempty_bar[buf], ((job >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_u + buf * 256;
+      for (int ch = 0; ch < NCH; ++ch) {                 // ---- phase 1
         for (int u = 0; u < 3 * KB; ++u) {
           mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
           const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
           const uint64_t adesc = make_kmajor_desc(sa, SWZ);
           const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
-          if (elect_one()) {
+          wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk)
-              umma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (u > 0 || kk > 0) ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-            if (u == 3 * KB - 1) umma_commit(&tfull_bar[buf]);
+          for (int kk = 0; kk < BK / 16; ++kk) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              Wgmma<NC, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (u > 0 || kk > 0) ? 1u : 0u);
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          release(false);
         }
+        hand_over();
       }
       mbar_wait(a2_ready, it & 1);                       // every epilogue warp has written (and fenced) its A2 rows
-      tc_fence_after();
-      for (int ch = 0; ch < NCH; ++ch, ++job) {          // ---- phase 2
-        const int buf = job & 1;
-        mbar_wait(&tempty_bar[buf], ((job >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_u + buf * 256;
+      for (int ch = 0; ch < NCH; ++ch) {                 // ---- phase 2
         for (int kb = 0; kb < KB; ++kb) {
           mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
           const uint32_t sb = smem_base + stage * L::STAGE_BYTES + L::A_BYTES;
           const uint64_t adesc = make_kmajor_desc(a2_base + kb * L::A2_SLAB, SWZ);
           const uint64_t bdesc = make_kmajor_desc(sb, SWZ);
-          if (elect_one()) {
+          wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk)
-              umma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-            if (kb == KB - 1) {
-              umma_commit(&tfull_bar[buf]);
-              if (ch == NCH - 1) umma_commit(a2_free);   // all MMAs that read A2 have retired when this fires
-            }
+          for (int kk = 0; kk < BK / 16; ++kk) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              Wgmma<NC, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          release(ch == NCH - 1 && kb == KB - 1);
         }
+        hand_over();
       }
     }
   } else {
     // =========================== epilogue (8 warps) ===========================
-    const int quad = warp & 3;                           // TMEM lane quadrant this warp may access
-    const int part = (warp - 2) >> 2;                    // 0 / 1: alternate 32-column chunks
+    const int quad = warp & 3;                           // rows quad * 32 .. quad * 32 + 31 of the tile
+    const int part = (warp - 5) >> 2;                    // 0 / 1: alternate 32-column chunks
     const int row = quad * 32 + lane;
     // byte offset of this row's 16-byte chunk c16 inside an A2 slab: row * SWZ + ((c16 ^ swz(row)) << 4)
     const uint32_t row_xor = (SWZ == 128) ? (uint32_t)(row & 7) : (SWZ == 64) ? (uint32_t)((row >> 1) & 3)
@@ -233,10 +237,8 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
       if (it > 0) mbar_wait(a2_free, (it - 1) & 1);      // the previous tile's phase 2 no longer reads A2
       // ---- epilogue 1: acc -> LeakyReLU -> bf16 -> A2 (swizzled K-major rows) [+ HBM copy for the backward]
       for (int ch = 0; ch < NCH; ++ch, ++job) {
-        const int buf = job & 1;
-        mbar_wait(&tfull_bar[buf], (job >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * 256;
+        mbar_wait(tfull_bar, job & 1);
+        const uint32_t taddr = (uint32_t)(quad * 32) << 16;
 #pragma unroll 1
         for (int c0 = part * 32; c0 < NC; c0 += 64) {
           float v[32];
@@ -261,17 +263,15 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             stg256(p.a1_out + grow + col + 16, pk + 8);
           }
         }
-        tc_fence_before();
         if (ch == NCH - 1) fence_proxy_async();          // generic-proxy smem writes -> visible to the tensor core
         __syncwarp();
         if (lane == 0) {
-          mbar_arrive(&tempty_bar[buf]);
+          mbar_arrive(tempty_bar);
           if (ch == NCH - 1) mbar_arrive(a2_ready);
         }
       }
       // ---- epilogue 2: acc + skip -> outputs
       for (int ch = 0; ch < NCH; ++ch, ++job) {
-        const int buf = job & 1;
         // skip rows of this thread's chunks: issue the loads before waiting for the accumulator
         uint32_t sk[(NC + 63) / 64][16];
 #pragma unroll
@@ -282,9 +282,8 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             ldg256(p.xa + grow + ch * NC + c0 + 16, sk[i] + 8);
           }
         }
-        mbar_wait(&tfull_bar[buf], (job >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * 256;
+        mbar_wait(tfull_bar, job & 1);
+        const uint32_t taddr = (uint32_t)(quad * 32) << 16;
 #pragma unroll
         for (int i = 0; i < (NC + 63) / 64; ++i) {
           const int c0 = part * 32 + 64 * i;
@@ -324,31 +323,26 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
             }
           }
         }
-        tc_fence_before();
         __syncwarp();
-        if (lane == 0) mbar_arrive(&tempty_bar[buf]);
+        if (lane == 0) mbar_arrive(tempty_bar);
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
 // =============================================================================================
 // Weight-stationary variant for the narrow units (C = 96: the six longest launches of the encoder / generator forward).
 // dilated_unit_tc_kernel re-streams, for EVERY 128-row tile, the three tap-shifted copies of the activation rows
-// (3 x 24 KB) and the whole weight set (W3 54 KB + W1 18 KB) from L2: 144 KB per tile, 35 B/clk/SM sustained -- the
-// L2 -> SM path (~42 B/clk/SM), not the tensor pipe (18 % active) or HBM, bounded it (profiles/r2_ncu_unit96.md).
-// Here the weights are loaded ONCE per CTA and stay in shared memory (72 KB), and each tile brings ONE haloed
-// activation tile (128 + 2 dil rows): tap k is the same tile read (k dil) rows further down -- K-major operand, 64-byte
-// swizzle, descriptor start address moved by whole rows (the swizzle is a function of the absolute shared-memory
-// address, which is how TMA wrote it).  29 KB instead of 144 KB per tile.
+// (3 x 24 KB) and the whole weight set (W3 54 KB + W1 18 KB) from L2: 144 KB per tile.  Here the weights are loaded
+// ONCE per CTA and stay in shared memory (72 KB), and each tile brings ONE haloed activation tile (128 + 2 dil rows):
+// tap k is the same tile read (k dil) rows further down -- K-major operand, 64-byte swizzle, descriptor start address
+// moved by whole rows (the swizzle is a function of the absolute shared-memory address, which is how TMA wrote it).
+// 29 KB instead of 144 KB per tile.  The MMA warpgroup runs the epilogues itself, straight from its accumulator
+// registers: the intermediate a1 goes into the swizzled A2 tile (the phase-2 A operand, and the source of its TMA store
+// to HBM), the skip comes from the centre rows of the haloed tile, the bf16 output leaves through a staging tile and TMA.
+// Warp roles (160 threads): 0-3 = MMA warpgroup + epilogues, 4 = TMA producer.
 // =============================================================================================
+constexpr int UW_THREADS = 160;
 constexpr int UW_AROWS = 152;                       // 128 + 2 * dil rows, dil <= 12
 constexpr int UW_ASLAB = UW_AROWS * 64;             // one 32-channel K block of the haloed tile (64-byte rows)
 constexpr int UW_WSLAB = 96 * 64;                   // one (tap, K block) weight slab: 96 rows x 32 channels
@@ -358,56 +352,49 @@ constexpr int UW_A2_OFF = UW_A_OFF + UW_STAGES * 3 * UW_ASLAB;
 constexpr int UW_OUT_OFF = UW_A2_OFF + 3 * (128 * 64);      // staging tile of the bf16 output (TMA store source)
 constexpr int UW_BAR_OFF = UW_OUT_OFF + 3 * (128 * 64);
 constexpr int UW_TOTAL = UW_BAR_OFF + 256 + 1024;
+static_assert(UW_TOTAL <= U_SMEM_MAX, "weight-stationary unit: shared memory");
 
-__global__ void __launch_bounds__(U_THREADS, 1)
+// byte offset of channel c (even) of row `row` in a [rows][32 ch] 64-byte-swizzled K-block sequence of `slab` bytes
+__device__ __forceinline__ uint32_t sw64_off(int row, int c, uint32_t slab) {
+  return (uint32_t)(c >> 5) * slab + (uint32_t)row * 64u + ((((uint32_t)(c & 31) >> 3) ^ (((uint32_t)row >> 1) & 3u)) << 4) +
+         (uint32_t)(c & 7) * 2u;
+}
+
+__global__ void __launch_bounds__(UW_THREADS, 1)
 dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w3,
                          const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_out,
                          const __grid_constant__ CUtensorMap tmap_a1, const UnitParams p) {
   constexpr int C = 96, BK = 32, KB = 3, SWZ = 64, A2_SLAB = 128 * 64;
-  constexpr uint32_t TMEM_COLS = 512;
+  constexpr uint64_t A_HALF = (64 * SWZ) >> 4;        // rows 64 .. 127 of a K-major operand tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t *a2 = smem + UW_A2_OFF;
+  uint8_t *outb = smem + UW_OUT_OFF;
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + UW_BAR_OFF);
   uint64_t *empty_bar = full_bar + UW_STAGES;
-  uint64_t *tfull_bar = empty_bar + UW_STAGES;          // [2]
-  uint64_t *tempty_bar = tfull_bar + 2;                 // [2]
-  uint64_t *a2_ready = tempty_bar + 2;
-  uint64_t *a2_free = a2_ready + 1;
-  uint64_t *w_bar = a2_free + 1;                        // the resident weights have landed
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(w_bar + 1);
+  uint64_t *w_bar = empty_bar + UW_STAGES;              // the resident weights have landed
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.n_lt * p.n_bg;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_w3);
     tma_prefetch_desc(&tmap_w1);
     for (int s = 0; s < UW_STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], U_EPI_WARPS);     // released by the epilogue: it reads the skip rows from the tile
+      mbar_init(&empty_bar[s], 4);      // released by the MMA warps once the epilogue has read the skip rows
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&tfull_bar[s], 1);
-      mbar_init(&tempty_bar[s], U_EPI_WARPS);
-    }
-    mbar_init(a2_ready, U_EPI_WARPS);
-    mbar_init(a2_free, 1);
     mbar_init(w_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   griddep_launch_dependents();
   griddep_wait();
   const int arows = 128 + 2 * p.dil;                    // rows of the haloed tile actually loaded
 
-  if (warp == 0) {
+  if (warp == 4) {
     // =========================== TMA producer ===========================
     if (elect_one()) {                                   // weights: once
       mbar_arrive_expect_tx(w_bar, 12 * UW_WSLAB);
@@ -431,216 +418,129 @@ dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
       __syncwarp();
       if (++stage == UW_STAGES) { stage = 0; phase ^= 1; }
     }
-  } else if (warp == 1) {
-    // =========================== MMA issuer ===========================
-    constexpr uint32_t idesc = make_idesc_bf16(128, C);
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t a2_base = smem_u32(a2);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    mbar_wait(w_bar, 0);
-    int stage = 0;
-    uint32_t phase = 0;
-    int job = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      {                                                   // ---- phase 1: conv3 over the haloed tile
-        const int buf = job & 1;
-        mbar_wait(&tempty_bar[buf], ((job >> 1) & 1) ^ 1);
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_u + buf * 256;
-        const uint32_t sa = smem_base + UW_A_OFF + stage * 3 * UW_ASLAB;
-        if (elect_one()) {
+    return;
+  }
+  // =========================== MMA warpgroup + epilogues ===========================
+  // fragment of this thread (see acc_store): rows r0 + 8 e + 64 h, columns 8 j + 2 (lane % 4) + {0, 1}
+  const int r0 = 16 * warp + (lane >> 2), cq = 2 * (lane & 3);
+  const bool issuer = threadIdx.x == 0;
+  const uint32_t smem_base = smem_u32(smem);
+  float d[2][C / 2];
+  mbar_wait(w_bar, 0);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int lt = tile % p.n_lt, b = tile / p.n_lt;
+    const int l0 = lt * 128;
+    // ---- phase 1: conv3 over the haloed tile
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t sa = smem_base + UW_A_OFF + stage * 3 * UW_ASLAB;
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 3; ++k) {
+    for (int k = 0; k < 3; ++k) {
 #pragma unroll
-            for (int kb = 0; kb < KB; ++kb) {
-              const uint64_t adesc = make_kmajor_desc(sa + kb * UW_ASLAB + (uint32_t)(k * p.dil) * 64u, SWZ);
-              const uint64_t bdesc = make_kmajor_desc(smem_base + UW_W3_OFF + (k * KB + kb) * UW_WSLAB, SWZ);
+      for (int kb = 0; kb < KB; ++kb) {
+        const uint64_t adesc = make_kmajor_desc(sa + kb * UW_ASLAB + (uint32_t)(k * p.dil) * 64u, SWZ);
+        const uint64_t bdesc = make_kmajor_desc(smem_base + UW_W3_OFF + (k * KB + kb) * UW_WSLAB, SWZ);
 #pragma unroll
-              for (int kk = 0; kk < BK / 16; ++kk)
-                umma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (k > 0 || kb > 0 || kk > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(&tfull_bar[buf]);
-        }
-        __syncwarp();
-        if (++stage == UW_STAGES) { stage = 0; phase ^= 1; }
-        ++job;
-      }
-      mbar_wait(a2_ready, it & 1);
-      tc_fence_after();
-      {                                                   // ---- phase 2: 1x1 conv on the resident A2 / W1
-        const int buf = job & 1;
-        mbar_wait(&tempty_bar[buf], ((job >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_u + buf * 256;
-        if (elect_one()) {
+        for (int kk = 0; kk < BK / 16; ++kk)
 #pragma unroll
-          for (int kb = 0; kb < KB; ++kb) {
-            const uint64_t adesc = make_kmajor_desc(a2_base + kb * A2_SLAB, SWZ);
-            const uint64_t bdesc = make_kmajor_desc(smem_base + UW_W1_OFF + kb * UW_WSLAB, SWZ);
-#pragma unroll
-            for (int kk = 0; kk < BK / 16; ++kk)
-              umma_f16(tmem_d, adesc + 2 * kk, bdesc + 2 * kk, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(&tfull_bar[buf]);
-          umma_commit(a2_free);
-        }
-        __syncwarp();
-        ++job;
+          for (int h = 0; h < 2; ++h)
+            Wgmma<C, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (k > 0 || kb > 0 || kk > 0) ? 1u : 0u);
       }
     }
-  } else {
-    // =========================== epilogue (8 warps) ===========================
-    // Per-thread row accesses to global memory touch 32 different 128-byte lines per instruction (L1 wavefront bound:
-    // the skip read and the output write were ~1.6k clocks each per tile).  Here the skip comes from the haloed tile
-    // that is already in shared memory (its centre rows), and both bf16 outputs leave through TMA: a1 straight from
-    // the A2 tile (same K-major swizzled layout as its tensor map's boxes), the unit's output from a staging tile.
-    const int quad = warp & 3;
-    const int part = (warp - 2) >> 2;
-    const int row = quad * 32 + lane;
-    const uint32_t row_xor = (uint32_t)((row >> 1) & 3);          // 64-byte swizzle of tile row `row`
-    const int srow = row + p.pad_l;                               // the same position inside the haloed tile
-    const uint32_t srow_off = (uint32_t)srow * 64u, srow_xor = (uint32_t)((srow >> 1) & 3);
-    const bool issuer = threadIdx.x == 64;
-    uint8_t *outb = smem + UW_OUT_OFF;
-    int job = 0, it = 0;
-    int stage = 0;
-    uint32_t sphase = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int lt = tile % p.n_lt, b = tile / p.n_lt;
-      const int l0 = lt * 128;
-      const int l = l0 + row;
-      const bool valid = (b < p.B) && (l < p.L);
-      const size_t grow = ((size_t)b * p.pitch + l) * C;
-      if (it > 0) mbar_wait(a2_free, (it - 1) & 1);
-      if (p.a1_out && it > 0) {                                   // the a1 store of the previous tile has read A2
-        if (issuer) {                                             // (bulk groups complete in order: a1, out, a1, out ...)
-          if (p.out_act) bulk_wait_read<1>();
-          else bulk_wait_read<0>();
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs<C / 2>(d[0]);
+    wgmma_fence_regs<C / 2>(d[1]);
+    // ---- epilogue 1: LeakyReLU -> bf16 -> A2 (swizzled K-major rows).  The previous tile's phase 2 has retired (same
+    // warpgroup); its a1 store must be done reading A2 (bulk groups complete in order: a1, out, a1, out ...)
+    if (p.a1_out && issuer) {
+      if (p.out_act) bulk_wait_read<1>();
+      else bulk_wait_read<0>();
+    }
+    named_bar_sync(1, 128);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int row = 64 * h + r0 + 8 * e;
+#pragma unroll
+        for (int j = 0; j < C / 8; ++j) {
+          const float v0 = d[h][4 * j + 2 * e], v1 = d[h][4 * j + 2 * e + 1];
+          const __nv_bfloat162 a = __floats2bfloat162_rn(fmaxf(v0, v0 * p.slope_mid), fmaxf(v1, v1 * p.slope_mid));
+          *reinterpret_cast<__nv_bfloat162 *>(a2 + sw64_off(row, 8 * j + cq, A2_SLAB)) = a;
         }
-        named_bar_sync(2, 256);
       }
-      {   // ---- epilogue 1: acc -> LeakyReLU -> bf16 -> A2 (swizzled K-major rows)
-        const int buf = job & 1;
-        mbar_wait(&tfull_bar[buf], (job >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * 256;
-        const float2 s2 = make_float2(p.slope_mid, p.slope_mid);
-#pragma unroll 1
-        for (int c0 = part * 32; c0 < C; c0 += 64) {
-          float v[32];
-          tmem_ld_32x32(taddr + c0, v);
-          uint32_t pk[16];
+    fence_proxy_async();                                  // generic-proxy smem writes -> tensor core / TMA
+    named_bar_sync(1, 128);
+    if (p.a1_out && issuer) {                             // training: keep a1 for the backward (write-only)
 #pragma unroll
-          for (int w = 0; w < 16; ++w) {
-            const float2 t = make_float2(v[2 * w], v[2 * w + 1]);
-            const float2 u = __fmul2_rn(t, s2);
-            const __nv_bfloat162 h = __hmax2(__floats2bfloat162_rn(t.x, t.y), __floats2bfloat162_rn(u.x, u.y));
-            pk[w] = *reinterpret_cast<const uint32_t *>(&h);
-          }
+      for (int kb = 0; kb < KB; ++kb) tma_store_4d(&tmap_a1, a2 + kb * A2_SLAB, kb * BK, 0, l0, b);
+      bulk_commit();
+    }
+    // ---- phase 2: 1x1 conv on the resident A2 / W1
+    wgmma_fence();
 #pragma unroll
-          for (int q = 0; q < 4; ++q)      // chunk c0 = K block c0 / 32: 16-byte unit q of this row
-            sts128(a2 + (uint32_t)(c0 / BK) * A2_SLAB + (uint32_t)row * SWZ + (((uint32_t)q ^ row_xor) << 4), pk + 4 * q);
-        }
-        tc_fence_before();
-        fence_proxy_async();
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&tempty_bar[buf]);
-          mbar_arrive(a2_ready);
-        }
-        if (p.a1_out) {                                           // training: keep a1 for the backward (write-only)
-          named_bar_sync(2, 256);
-          if (issuer) {
+    for (int kb = 0; kb < KB; ++kb) {
+      const uint64_t adesc = make_kmajor_desc(smem_base + UW_A2_OFF + kb * A2_SLAB, SWZ);
+      const uint64_t bdesc = make_kmajor_desc(smem_base + UW_W1_OFF + kb * UW_WSLAB, SWZ);
 #pragma unroll
-            for (int kb = 0; kb < KB; ++kb) tma_store_4d(&tmap_a1, a2 + kb * A2_SLAB, kb * BK, 0, l0, b);
-            bulk_commit();
-          }
-        }
-        ++job;
-      }
-      {   // ---- epilogue 2: acc + skip -> outputs
-        const int buf = job & 1;
-        mbar_wait(&tfull_bar[buf], (job >> 1) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + buf * 256;
-        const uint8_t *sa = smem + UW_A_OFF + stage * 3 * UW_ASLAB;      // this tile's haloed activation rows
-        mbar_wait(&full_bar[stage], sphase);                     // (long complete: makes the TMA writes visible here)
-        if (p.out_act) {                                          // the previous tile's output store has read `outb`
-          if (issuer) {
-            if (p.a1_out) bulk_wait_read<1>();                    // ... this tile's a1 store may still be running
-            else bulk_wait_read<0>();
-          }
-          named_bar_sync(1, 256);
-        }
-#pragma unroll 1
-        for (int c0 = part * 32; c0 < C; c0 += 64) {
-          uint32_t sk[16];
+      for (int kk = 0; kk < BK / 16; ++kk)
 #pragma unroll
-          for (int q = 0; q < 4; ++q)
-            lds128(sa + (uint32_t)(c0 / BK) * UW_ASLAB + srow_off + (((uint32_t)q ^ srow_xor) << 4), sk + 4 * q);
-          float v[32];
-          tmem_ld_32x32(taddr + c0, v);
+        for (int h = 0; h < 2; ++h)
+          Wgmma<C, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs<C / 2>(d[0]);
+    wgmma_fence_regs<C / 2>(d[1]);
+    // ---- epilogue 2: acc + skip (centre rows of the haloed tile) -> outputs
+    if (p.out_act && issuer) {                            // the previous tile's output store has read `outb`
+      if (p.a1_out) bulk_wait_read<1>();                  // ... this tile's a1 store may still be running
+      else bulk_wait_read<0>();
+    }
+    if (p.out_act) named_bar_sync(1, 128);
+    const uint8_t *sah = smem + UW_A_OFF + stage * 3 * UW_ASLAB;
 #pragma unroll
-          for (int w = 0; w < 16; ++w) {
-            const float s0 = bfl(sk[w]), s1 = bfh(sk[w]);
-            v[2 * w] += fminf(s0, s0 * p.slope_in_inv);          // inverse LeakyReLU of the input operand
-            v[2 * w + 1] += fminf(s1, s1 * p.slope_in_inv);
-          }
-          if (p.out_f32 && valid) {
-            uint32_t o[32];
+    for (int h = 0; h < 2; ++h)
 #pragma unroll
-            for (int j = 0; j < 32; ++j) o[j] = __float_as_uint(v[j]);
+      for (int e = 0; e < 2; ++e) {
+        const int row = 64 * h + r0 + 8 * e;
+        const int l = l0 + row;
+        const bool valid = l < p.L;
+        const size_t grow = ((size_t)b * p.pitch + l) * C;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) stg256(p.out_f32 + grow + c0 + 8 * j, o + 8 * j);
-          }
+        for (int j = 0; j < C / 8; ++j) {
+          const int c = 8 * j + cq;
+          const __nv_bfloat162 sk = *reinterpret_cast<const __nv_bfloat162 *>(sah + sw64_off(row + p.pad_l, c, UW_ASLAB));
+          const float s0 = __low2float(sk), s1 = __high2float(sk);
+          float v0 = d[h][4 * j + 2 * e] + fminf(s0, s0 * p.slope_in_inv);     // inverse LeakyReLU of the input
+          float v1 = d[h][4 * j + 2 * e + 1] + fminf(s1, s1 * p.slope_in_inv);
+          if (p.out_f32 && valid) *reinterpret_cast<float2 *>(p.out_f32 + grow + c) = make_float2(v0, v1);
           if (p.out_act) {
-            uint32_t pk[16];
-            const float2 so = make_float2(p.slope_out, p.slope_out);
-#pragma unroll
-            for (int w = 0; w < 16; ++w) {
-              const float2 t = make_float2(v[2 * w], v[2 * w + 1]);
-              __nv_bfloat162 h = __floats2bfloat162_rn(t.x, t.y);
-              if (p.act_out == RAVE_ACT_LEAKY) {
-                const float2 u = __fmul2_rn(t, so);
-                h = __hmax2(h, __floats2bfloat162_rn(u.x, u.y));
-              }
-              pk[w] = *reinterpret_cast<const uint32_t *>(&h);
+            if (p.act_out == RAVE_ACT_LEAKY) {
+              v0 = fmaxf(v0, v0 * p.slope_out);
+              v1 = fmaxf(v1, v1 * p.slope_out);
             }
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-              sts128(outb + (uint32_t)(c0 / BK) * A2_SLAB + (uint32_t)row * SWZ + (((uint32_t)q ^ row_xor) << 4), pk + 4 * q);
+            *reinterpret_cast<__nv_bfloat162 *>(outb + sw64_off(row, c, A2_SLAB)) = __floats2bfloat162_rn(v0, v1);
           }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&tempty_bar[buf]);
-          mbar_arrive(&empty_bar[stage]);                          // skip rows read: the producer may refill this stage
-        }
-        if (p.out_act) {
-          fence_proxy_async();
-          named_bar_sync(1, 256);
-          if (issuer) {
-#pragma unroll
-            for (int kb = 0; kb < KB; ++kb) tma_store_4d(&tmap_out, outb + kb * A2_SLAB, kb * BK, 0, l0, b);
-            bulk_commit();
-          }
-        }
-        ++job;
       }
-      if (++stage == UW_STAGES) { stage = 0; sphase ^= 1; }
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[stage]);      // skip rows read: the producer may refill this stage
+    if (p.out_act) {
+      fence_proxy_async();
+      named_bar_sync(1, 128);
+      if (issuer) {
+#pragma unroll
+        for (int kb = 0; kb < KB; ++kb) tma_store_4d(&tmap_out, outb + kb * A2_SLAB, kb * BK, 0, l0, b);
+        bulk_commit();
+      }
     }
-    if (issuer) bulk_wait_all();
+    if (++stage == UW_STAGES) { stage = 0; phase ^= 1; }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
+  if (issuer) bulk_wait_all();
 }
 
 typedef CUresult (*EncodeTiledFnU)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
@@ -674,7 +574,7 @@ static int launch_unit(const CUtensorMap &ta, const CUtensorMap &t3, const CUten
     attr = true;
   }
   const int tiles = p.n_lt * p.n_bg;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
@@ -725,7 +625,7 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
   p.out_act = (__nv_bfloat16 *)out_act;
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  const int NC = C <= 256 ? C : C / 2;
+  const int NC = 96;
   CUtensorMap ta, t3, t1;
   {
     cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
@@ -747,67 +647,64 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc: weight tensor map encode failed (%d)", (int)r);
   }
   cudaStream_t s = (cudaStream_t)stream;
-  {
-    const char *e = getenv("RAVE_UNIT_WS");
-    if (C == 96 && p.BB == 1 && dil <= 12 && !(e && e[0] == '0')) {
-      // weight-stationary kernel: its activation map carries the haloed box (128 + 2 dil rows), its weight maps one
-      // (tap, K block) slab per box
-      CUtensorMap tah, t3s, t1s;
-      {
-        cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
-        cuuint32_t box[4] = {32, 1, (cuuint32_t)(128 + 2 * dil), 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(&tah, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xa), dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): tensor map A encode failed (%d)", (int)r);
-      }
-      for (int which = 0; which < 2; ++which) {
-        cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
-        cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-        cuuint32_t box[2] = {32, 96};
-        cuuint32_t estr[2] = {1, 1};
-        CUresult r = enc(which == 0 ? &t3s : &t1s, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                         const_cast<void *>(which == 0 ? w3t : w1t), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): weight tensor map encode failed (%d)", (int)r);
-      }
-      static bool attr = false;
-      if (!attr) {
-        cudaError_t er = cudaFuncSetAttribute(dilated_unit_ws96_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, UW_TOTAL);
-        if (er != cudaSuccess) {
-          set_error("dilated_unit_tc(ws): cudaFuncSetAttribute(%d bytes): %s", UW_TOTAL, cudaGetErrorString(er));
-          return 2;
-        }
-        attr = true;
-      }
-      const int tiles = p.n_lt * p.n_bg;
-      int dev = 0, sms = 148;
-      cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-      // bf16 outputs leave through TMA: [B][pitch][96] viewed as (c, 1, row, b) boxes of one 32-channel K block x 128 rows
-      // (rows >= L and batches >= B are clipped by the TMA unit)
-      CUtensorMap tout, ta1;
-      memset(&tout, 0, sizeof(tout));
-      memset(&ta1, 0, sizeof(ta1));
-      for (int which = 0; which < 2; ++which) {
-        void *base = which == 0 ? out_act : a1_out;
-        if (!base) continue;
-        cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
-        cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
-        cuuint32_t box[4] = {32, 1, 128, 1};
-        cuuint32_t estr[4] = {1, 1, 1, 1};
-        CUresult r = enc(which == 0 ? &tout : &ta1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): output tensor map encode failed (%d)", (int)r);
-      }
-      launch_pdl(dilated_unit_ws96_kernel, dim3(tiles < sms ? tiles : sms), dim3(U_THREADS), UW_TOTAL, s, tah, t3s, t1s,
-                 tout, ta1, p);
-      RAVE_CHECK_LAUNCH("dilated_unit_tc(ws)");
-      return 0;
+  if (C == 96 && p.BB == 1 && dil <= 12) {
+    // weight-stationary kernel: its activation map carries the haloed box (128 + 2 dil rows), its weight maps one
+    // (tap, K block) slab per box
+    CUtensorMap tah, t3s, t1s;
+    {
+      cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
+      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
+      cuuint32_t box[4] = {32, 1, (cuuint32_t)(128 + 2 * dil), 1};
+      cuuint32_t estr[4] = {1, 1, 1, 1};
+      CUresult r = enc(&tah, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xa), dims, strides, box, estr,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): tensor map A encode failed (%d)", (int)r);
     }
+    for (int which = 0; which < 2; ++which) {
+      cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
+      cuuint64_t strides[1] = {(cuuint64_t)C * 2};
+      cuuint32_t box[2] = {32, 96};
+      cuuint32_t estr[2] = {1, 1};
+      CUresult r = enc(which == 0 ? &t3s : &t1s, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+                       const_cast<void *>(which == 0 ? w3t : w1t), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                       CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): weight tensor map encode failed (%d)", (int)r);
+    }
+    static bool attr = false;
+    if (!attr) {
+      cudaError_t er = cudaFuncSetAttribute(dilated_unit_ws96_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, UW_TOTAL);
+      if (er != cudaSuccess) {
+        set_error("dilated_unit_tc(ws): cudaFuncSetAttribute(%d bytes): %s", UW_TOTAL, cudaGetErrorString(er));
+        return 2;
+      }
+      attr = true;
+    }
+    const int tiles = p.n_lt * p.n_bg;
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    // bf16 outputs leave through TMA: [B][pitch][96] viewed as (c, 1, row, b) boxes of one 32-channel K block x 128 rows
+    // (rows >= L and batches >= B are clipped by the TMA unit)
+    CUtensorMap tout, ta1;
+    memset(&tout, 0, sizeof(tout));
+    memset(&ta1, 0, sizeof(ta1));
+    for (int which = 0; which < 2; ++which) {
+      void *base = which == 0 ? out_act : a1_out;
+      if (!base) continue;
+      cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
+      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
+      cuuint32_t box[4] = {32, 1, 128, 1};
+      cuuint32_t estr[4] = {1, 1, 1, 1};
+      CUresult r = enc(which == 0 ? &tout : &ta1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, estr,
+                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
+                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): output tensor map encode failed (%d)", (int)r);
+    }
+    launch_pdl(dilated_unit_ws96_kernel, dim3(tiles < sms ? tiles : sms), dim3(UW_THREADS), UW_TOTAL, s, tah, t3s, t1s,
+               tout, ta1, p);
+    RAVE_CHECK_LAUNCH("dilated_unit_tc(ws)");
+    return 0;
   }
   switch (C) {
     case 96: return launch_unit<96, 32>(ta, t3, t1, p, s);

@@ -1,18 +1,17 @@
-// Multi-tap weight gradient on tcgen05 (sm_100a):
+// Multi-tap weight gradient on wgmma (sm_90a):
 //
 //     dWt[k][m][n] = sum_{(b,l)} P[b][l][m] * Q[b][l*stride + k*dil - pad_l][n]          for ALL taps k of a group at once
 //
 // The per-tap kernel (conv_tc.cu: wgrad_tc_kernel) gives every tap its own CTA: each one streams the P rows (the output
-// gradient) and its own shifted Q rows (the saved operand) from L2 -- K times the bytes of one pass, and the L2 -> SM path
-// (~42 B/clk/SM: twice HBM), not the tensor pipe, bounded the discriminator's weight gradients (profiles/r2: 145 GFLOP
-// in 331 us = 3 GB of L2 reads).  Here a CTA owns a (128 x BN) tile of dW for a GROUP of up to 8 taps:
+// gradient) and its own shifted Q rows (the saved operand) from L2 -- K times the bytes of one pass.  Here a CTA owns a
+// (128 x BN) tile of dW for a GROUP of taps (as many as its accumulator registers hold):
 //
 //   * the P tile [64 rows x 128 channels] is loaded ONCE per 64-row chunk and feeds every tap's MMAs;
 //   * taps that read the same phase of Q (row = (l + j) * stride + ph) share ONE haloed Q tile: rows l0 + jmin ...
 //     l0 + 63 + jmax of that phase.  Both operands are MN-major (the reduction runs over tile rows), so tap j is the same
 //     tile with the descriptor's start address moved down (j - jmin) rows of 128 bytes: the 128-byte swizzle is a
 //     function of the absolute shared-memory address (TMA wrote it that way), no copy, no re-layout;
-//   * every tap has its own fp32 accumulator in TMEM (taps x BN <= 512 columns).
+//   * every tap has its own fp32 accumulator tile in the MMA warpgroup's registers (taps x BN <= 128 per thread).
 //
 // K = 15 / stride 4 in the row-widened form the engine uses (4 unit-stride taps over 4x wider rows): P 16 KB + Q 17 KB
 // per 4 x 256 MMA clocks = 33 B/clk instead of 4 x 40 KB per the same work.  Split-K over row slices as before: every
@@ -29,13 +28,13 @@
 namespace rave {
 namespace tc {
 
-constexpr int WM_THREADS = 192;          // warp 0: TMA producer, warp 1: MMA issuer (+ TMEM), warps 2-5: column sums, epilogue
+constexpr int WM_THREADS = 288;          // warps 0-3: MMA warpgroup (+ result store), warp 4: TMA producer, warps 5-8: column sums
+constexpr int WM_ACC = 128;              // accumulator registers per MMA thread: taps x BLOCK_N
 constexpr int WM_MAXT = 8;               // taps per CTA
 constexpr int WM_ROWS = 64;              // reduction rows per pipeline stage
 constexpr int WM_PSLAB = WM_ROWS * 128;  // [64 rows][64 ch] bf16
 constexpr int WM_QROWS = 80;             // rows of a haloed Q slab: 64 + at most 16 halo rows (all batch segments)
 constexpr int WM_QSLAB = WM_QROWS * 128;
-constexpr int WM_MAXTILES = 8;
 
 struct WmParams {
   int B, Cm, Lp, Cn, Lq, K, stride, dil, pad_l;
@@ -46,6 +45,7 @@ struct WmParams {
   int stages, stage_bytes;
   float *dwt;                  // [splits][K][Cm][Cn]
   float *dbias;
+  float *dbias_part;           // [splits][n_mt * 128] per-slice partial bias gradients (see dbias_sum_kernel)
   // per tap: Q tile (index within its group) and row shift inside that tile; per group: first tile, tile count;
   // per tile: phase and first row offset j
   unsigned char tap_tile[32], tap_shift[32];
@@ -59,14 +59,14 @@ __global__ void __launch_bounds__(WM_THREADS, 1)
 wgrad_mt_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constant__ CUtensorMap tmap_q,
                 const WmParams p) {
   constexpr int NS = (BLOCK_N + 63) / 64;
+  constexpr int MAXT = WM_ACC / BLOCK_N;               // taps per CTA this instance can hold
   constexpr int MAX_STAGES = 8;
+  static_assert(BLOCK_N % 64 == 0 && MAXT >= 1, "MN-major B operand: whole 64-channel slabs");
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int bar_off = p.stages * p.stage_bytes;
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + bar_off);
   uint64_t *empty_bar = full_bar + MAX_STAGES;
-  uint64_t *tfull_bar = empty_bar + MAX_STAGES;
-  uint32_t *tmem_ptr_smem = reinterpret_cast<uint32_t *>(tfull_bar + 1);
   float *cs_scratch = reinterpret_cast<float *>(smem + bar_off + 256);          // [8][128] fp32
 
   const int warp = threadIdx.x >> 5;
@@ -90,26 +90,21 @@ wgrad_mt_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
   const bool do_cs = p.dbias != nullptr && grp == 0 && nt == 0;
   const int qrows = p.BL + p.halo;                     // rows per batch segment of a Q box
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_p);
     tma_prefetch_desc(&tmap_q);
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], do_cs ? 5 : 1);     // MMA commit (+ the 4 column-sum warps)
+      mbar_init(&empty_bar[s], do_cs ? 8 : 4);     // the 4 MMA warps (+ the 4 column-sum warps)
     }
-    mbar_init(tfull_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr_smem, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
   griddep_launch_dependents();      // dependents may begin their prologue ...
   griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
 
   if (my_chunks > 0) {
-    if (warp == 0) {
+    if (warp == 4) {
       // =========================== TMA producer ===========================
       const uint32_t tx = 2 * WM_PSLAB + (uint32_t)n_tiles * NS * (uint32_t)(qrows * p.BB * 128);
       int stage = 0;
@@ -134,106 +129,91 @@ wgrad_mt_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
         __syncwarp();
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-    } else if (warp == 1) {
-      // =========================== MMA issuer ===========================
-      // bf16 x bf16 -> fp32, A and B both MN-major (bits 15 / 16)
-      constexpr uint32_t idesc = make_idesc_bf16(128, BLOCK_N) | (1u << 15) | (1u << 16);
+    } else if (warp < 4) {
+      // =========================== MMA warpgroup ===========================
+      // bf16 x bf16 -> fp32, A and B both MN-major (transposed operands); M half h = P slab h
       const uint32_t smem_base = smem_u32(smem);
-      const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
+      float d[MAXT][2][BLOCK_N / 2];
       int stage = 0;
       uint32_t phase = 0;
       for (int c = 0; c < my_chunks; ++c) {
         mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
         const uint32_t sa = smem_base + stage * p.stage_bytes;
         const uint32_t sq = sa + 2 * WM_PSLAB;
-        for (int i = 0; i < nk; ++i) {
-          const uint32_t qt = sq + (uint32_t)p.tap_tile[k0 + i] * NS * WM_QSLAB;
-          const int shift = p.tap_shift[k0 + i];
-          if (elect_one()) {
+        wgmma_fence();
+#pragma unroll
+        for (int i = 0; i < MAXT; ++i) {
+          if (i < nk) {
+            const uint32_t qt = sq + (uint32_t)p.tap_tile[k0 + i] * NS * WM_QSLAB;
+            const int shift = p.tap_shift[k0 + i];
 #pragma unroll
             for (int kk = 0; kk < WM_ROWS / 16; ++kk) {
               // reduction rows 16 kk .. 16 kk + 15 = batch segment (16 kk) / BL, rows (16 kk) % BL ...: the same rows of
               // the Q box, `shift` rows further down
               const int r = 16 * kk;
               const int qrow = (r / p.BL) * qrows + (r % p.BL) + shift;
-              const uint64_t adesc = make_mnmajor_desc(sa + r * 128, WM_PSLAB);
               const uint64_t bdesc = make_mnmajor_desc(qt + qrow * 128, WM_QSLAB);
-              umma_f16(tmem_u + i * BLOCK_N, adesc, bdesc, idesc, (c > 0 || kk > 0) ? 1u : 0u);
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                Wgmma<BLOCK_N, 1, 1>::mma(d[i][h], make_mnmajor_desc(sa + h * WM_PSLAB + r * 128, WM_PSLAB), bdesc,
+                                          (c > 0 || kk > 0) ? 1u : 0u);
             }
           }
-          __syncwarp();
         }
-        if (elect_one()) {
-          umma_commit(&empty_bar[stage]);
-          if (c == my_chunks - 1) umma_commit(tfull_bar);
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int i = 0; i < MAXT; ++i) {
+          wgmma_fence_regs<BLOCK_N / 2>(d[i][0]);
+          wgmma_fence_regs<BLOCK_N / 2>(d[i][1]);
         }
         __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
         if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
-    } else {
-      if (do_cs) {
-        // bias gradient: column sums of the P tiles while the tensor core consumes them (as in wgrad_tc_kernel)
-        const int te = (warp - 2) * 32 + lane;
-        const int cg = te & 15, rg = te >> 4;
-        const uint32_t col = (uint32_t)(cg >> 3) * WM_PSLAB + (uint32_t)(((cg & 7) ^ rg) << 4);
-        float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        int stage = 0;
-        uint32_t phase = 0;
-        for (int c = 0; c < my_chunks; ++c) {
-          mbar_wait(&full_bar[stage], phase);
-          const uint8_t *sa = smem + stage * p.stage_bytes + col;
 #pragma unroll
-          for (int i = 0; i < WM_ROWS / 8; ++i) {
-            const uint4 q = *reinterpret_cast<const uint4 *>(sa + (rg + 8 * i) * 128);
-            const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+      for (int i = 0; i < MAXT; ++i)
+        if (i < nk)
+          store_wgrad_tile<BLOCK_N>(d[i], p.dwt + ((size_t)split * p.K + (k0 + i)) * p.Cm * p.Cn, m0, n0, p.Cm, p.Cn);
+    } else if (do_cs) {
+      // bias gradient: column sums of the P tiles while the tensor core consumes them (as in wgrad_tc_kernel)
+      const int te = (warp - 5) * 32 + lane;
+      const int cg = te & 15, rg = te >> 4;
+      const uint32_t col = (uint32_t)(cg >> 3) * WM_PSLAB + (uint32_t)(((cg & 7) ^ rg) << 4);
+      float cs[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int c = 0; c < my_chunks; ++c) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint8_t *sa = smem + stage * p.stage_bytes + col;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              cs[2 * j] += __uint_as_float(w[j] << 16);
-              cs[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
-            }
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
+        for (int i = 0; i < WM_ROWS / 8; ++i) {
+          const uint4 q = *reinterpret_cast<const uint4 *>(sa + (rg + 8 * i) * 128);
+          const uint32_t w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
-        for (int j = 0; j < 8; ++j) cs_scratch[rg * 128 + cg * 8 + j] = cs[j];
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        float tsum = 0.f;
-#pragma unroll
-        for (int r = 0; r < 8; ++r) tsum += cs_scratch[r * 128 + te];
-        if (m0 + te < p.Cm) atomicAdd(p.dbias + m0 + te, tsum);
-      }
-      const int quad = warp & 3;
-      const int m = m0 + quad * 32 + lane;
-      mbar_wait(tfull_bar, 0);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16);
-      for (int i = 0; i < nk; ++i) {
-        float *dst = p.dwt + (((size_t)split * p.K + (k0 + i)) * p.Cm + m) * p.Cn + n0;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BLOCK_N; c0 += 16) {
-          float v[16];
-          tmem_ld_32x16(taddr + i * BLOCK_N + c0, v);
-          if (m < p.Cm) {
-            if (n0 + c0 + 16 <= p.Cn && (p.Cn & 3) == 0) {
-              float4 *d4 = reinterpret_cast<float4 *>(dst + c0);
-#pragma unroll
-              for (int q = 0; q < 4; ++q) d4[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            } else {
-#pragma unroll
-              for (int q = 0; q < 16; ++q)
-                if (n0 + c0 + q < p.Cn) dst[c0 + q] = v[q];
-            }
+          for (int j = 0; j < 4; ++j) {
+            cs[2 * j] += __uint_as_float(w[j] << 16);
+            cs[2 * j + 1] += __uint_as_float(w[j] & 0xFFFF0000u);
           }
         }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        if (++stage == p.stages) { stage = 0; phase ^= 1; }
       }
+#pragma unroll
+      for (int j = 0; j < 8; ++j) cs_scratch[rg * 128 + cg * 8 + j] = cs[j];
+      asm volatile("bar.sync 1, 128;" ::: "memory");
+      float tsum = 0.f;
+#pragma unroll
+      for (int r = 0; r < 8; ++r) tsum += cs_scratch[r * 128 + te];
+      p.dbias_part[(size_t)split * p.n_mt * 128 + m0 + te] = tsum;
     }
-  } else if (warp >= 2) {
+  } else if (do_cs && warp >= 5) {
+    // empty slice: no rows, zero partial bias gradient
+    p.dbias_part[(size_t)split * p.n_mt * 128 + m0 + (warp - 5) * 32 + lane] = 0.f;
+  } else if (warp < 4) {
     // empty slice (more splits than row chunks): this CTA still owns its partial tiles -> zeros
-    const int quad = warp & 3;
-    const int m = m0 + quad * 32 + lane;
+    const int m = m0 + threadIdx.x;
     if (m < p.Cm) {
       for (int i = 0; i < nk; ++i) {
         float *dst = p.dwt + (((size_t)split * p.K + (k0 + i)) * p.Cm + m) * p.Cn + n0;
@@ -241,13 +221,6 @@ wgrad_mt_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
           if (n0 + c < p.Cn) dst[c] = 0.f;
       }
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -268,21 +241,11 @@ static EncodeTiledFnW wm_encode_fn() {
 }
 
 // N tile and taps per CTA from the shape alone (the split count the caller allocates for must not depend on stride /
-// dilation / padding): as many taps as share one P tile, accumulators filling the 512 TMEM columns
+// dilation / padding): whole 64-channel slabs of Q, as many taps as share one P tile within the WM_ACC accumulator
+// registers of an MMA thread
 static void wm_tile(int Cn, int K, int *BN, int *tpg) {
-  const int want = K < WM_MAXT ? K : WM_MAXT;
-  const int cands[] = {256, 192, 128, 96, 64, 48, 32, 16};
-  const int cn16 = (Cn + 15) / 16 * 16;
-  int bn = 16;
-  for (int c : cands)
-    if (c * want <= 512) { bn = c; break; }
-  if (bn > cn16) {                       // narrower operand: the smallest valid tile that covers it
-    bn = 16;
-    for (int i = 7; i >= 0; --i)
-      if (cands[i] >= cn16) { bn = cands[i]; break; }
-  }
-  int t = 512 / bn;
-  if (t > WM_MAXT) t = WM_MAXT;
+  const int bn = (Cn <= 64 || K > 1) ? 64 : 128;
+  int t = WM_ACC / bn;
   if (t > K) t = K;
   *BN = bn;
   *tpg = t;
@@ -301,7 +264,7 @@ static void wm_geometry(int B, int Cm, int Lp, int Cn, int K, int *BL, int *n_lt
   *n_groups = ceil_div(K, *tpg);
   const int tiles = (*n_groups) * (*n_mt) * (*n_nt);
   const int n_chunks = (*n_lt) * (*n_bg);
-  int s = ceil_div(tiles >= 74 ? 148 : 2 * 148, tiles);
+  int s = ceil_div(tiles >= 66 ? 132 : 2 * 132, tiles);
   if (s > 32) s = 32;
   if (s > n_chunks / 4) s = n_chunks / 4;      // at least 4 chunks of 64 rows per slice
   if (s > n_chunks) s = n_chunks;
@@ -385,12 +348,8 @@ static bool wm_build_tiles(rave::tc::WmParams &p, int BN, int K, int stride, int
 // 1 when the multi-tap kernel takes this shape (rows per batch >= 16 ... see the checks below); the per-tap kernel
 // covers the rest.  RAVE_WG_MT=0 disables it.
 extern "C" int rave_conv1d_tc_wgrad_mt_supported(int B, int Cm, int Lp, int Cn, int K) {
-  // OPT-IN (RAVE_WG_MT=1).  Measured on B200 (profiles/r2_wgrad_mt.md): numerically right (tests/test_gpu_tc.py runs it),
-  // but slower than the per-tap kernel on the shipped shapes -- D-step weight gradients 5.6 ms instead of 3.7 ms: with
-  // M = 128 single-CTA MMAs the tensor core re-reads the P tile from shared memory for every tap (N <= 128 per tap is
-  // shared-memory-read bound: (128 + N) x 32 B per N/2 clocks), the 96-channel layers carry half-empty second slabs,
-  // and the extra split-K slices make the weight-norm backward re-read more partial tiles.  Kept as the starting point
-  // for a CTA-pair (M = 256) version.
+  // OPT-IN (RAVE_WG_MT=1): numerically right (tests/test_gpu_tc.py runs it), but the tensor core re-reads the P tile
+  // from shared memory for every tap and at most two taps fit the register accumulators, so it is not the default.
   const char *e = getenv("RAVE_WG_MT");
   if (!(e && e[0] == '1')) return 0;
   if (K < 1 || K > 32 || Cm % 8 || Cn % 8) return 0;
@@ -469,16 +428,29 @@ extern "C" int rave_conv1d_tc_wgrad_mt(const void *P, const void *Q, float *dwt,
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "wgrad_mt: tensor map Q encode failed (%d)", (int)r);
   }
   cudaStream_t s = (cudaStream_t)stream;
-  switch (BN) {
-    case 16: return launch_wm<16>(tp, tq, p, smem_bytes, s);
-    case 32: return launch_wm<32>(tp, tq, p, smem_bytes, s);
-    case 48: return launch_wm<48>(tp, tq, p, smem_bytes, s);
-    case 64: return launch_wm<64>(tp, tq, p, smem_bytes, s);
-    case 96: return launch_wm<96>(tp, tq, p, smem_bytes, s);
-    case 128: return launch_wm<128>(tp, tq, p, smem_bytes, s);
-    case 192: return launch_wm<192>(tp, tq, p, smem_bytes, s);
-    case 256: return launch_wm<256>(tp, tq, p, smem_bytes, s);
+  p.dbias_part = nullptr;
+  if (dbias && cudaMallocAsync((void **)&p.dbias_part, sizeof(float) * p.splits * p.n_mt * 128, s) != cudaSuccess) {
+    set_error("wgrad_mt: cudaMallocAsync of the bias-gradient partials failed");
+    return 2;
   }
-  set_error("wgrad_mt: no kernel for BLOCK_N=%d", BN);
-  return 1;
+  int rc = 1;
+  switch (BN) {
+    case 64: rc = launch_wm<64>(tp, tq, p, smem_bytes, s); break;
+    case 128: rc = launch_wm<128>(tp, tq, p, smem_bytes, s); break;
+    default: set_error("wgrad_mt: no kernel for BLOCK_N=%d", BN);
+  }
+  if (dbias) {
+    if (rc == 0) {
+      dbias_sum_kernel<<<ceil_div(Cm, 256), 256, 0, s>>>(p.dbias_part, dbias, p.splits, p.n_mt * 128, Cm);
+      cudaError_t e = cudaGetLastError();
+      if (e != cudaSuccess) {
+        set_error("wgrad_mt: dbias_sum launch failed: %s", cudaGetErrorString(e));
+        rc = 2;
+      } else {
+        count_launch();
+      }
+    }
+    cudaFreeAsync(p.dbias_part, s);
+  }
+  return rc;
 }

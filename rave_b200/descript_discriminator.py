@@ -93,7 +93,7 @@ class DiscConv2d(nn.Conv2d):
         proxy.bias = self.bias
 
     def _forward_tc(self, x, B, C, T, Fq):
-        """bf16 mode: the same conv along frequency as a one-layer chain of the tcgen05 engine (forward, dgrad and wgrad
+        """bf16 mode: the same conv along frequency as a one-layer chain of the wgmma engine (forward, dgrad and wgrad
         on the tensor cores; 23 % of the v3 discriminator FLOPs ran on the fp32 CUDA-core kernels: 176 ms of a 280 ms
         G-step).  NCHW in, NCHW (view) out; the MRD itself stays channel-last between layers (`forward_cl`)."""
         from . import engine

@@ -1,5 +1,5 @@
 """Tensor-core execution engine: runs a whole conv chain (EncoderV2.net, GeneratorV2.net, a
-discriminator ConvNet) on the tcgen05 kernels in the engine's own layout and precision.
+discriminator ConvNet) on the wgmma kernels in the engine's own layout and precision.
 
 Layout / precision ("bf16 mode", BASELINE config 3): every tensor between two convs is CHANNEL-LAST
 ([B][L][C]); the operand of each conv is the bf16 tensor `a = act(h)` written by the PRODUCER's
@@ -39,8 +39,8 @@ FUSE_UNITS = _os.environ.get("RAVE_FUSE_UNITS", "1") != "0"
 
 def set_precision(mode: str) -> None:
     """'fp32'   : CUDA-core parity kernels ([B,C,L] fp32, per-layer autograd);
-    'bf16'   : tcgen05 engine (bf16 operands, fp32 accumulate) for every chain it supports (~1e-2 rel-L2 end to end);
-    'bf16x3' : the accurate fast mode -- the same tcgen05 kernels on split operands (x = hi + lo, three MMAs per
+    'bf16'   : wgmma engine (bf16 operands, fp32 accumulate) for every chain it supports (~1e-2 rel-L2 end to end);
+    'bf16x3' : the accurate fast mode -- the same wgmma kernels on split operands (x = hi + lo, three MMAs per
                product: hi*hi + lo*hi + hi*lo, fp32 accumulate), <= 1e-4 rel-L2 end to end like the fp32 path, for the
                FORWARD of the encoder / generator chains (no autograd graph: inference, validation, export warm-up);
                anything that needs gradients runs on the fp32 kernels in this mode."""

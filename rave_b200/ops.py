@@ -1,7 +1,7 @@
 """torch.autograd.Function wrappers around the C ABI (include/rave_b200.h).
 
 PyTorch is plumbing here: it owns the device memory, the stream and the autograd tape; every
-arithmetic operation of the hot path is one of the library's sm_100a kernels.  There is no
+arithmetic operation of the hot path is one of the library's sm_90a kernels.  There is no
 fallback implementation: host tensors or a missing library raise (`_lib.RaveB200Error`).
 """
 import os

@@ -1,5 +1,5 @@
 """PQMF analysis / synthesis -- module surface of rave/pqmf.py (`PQMF`, `CachedPQMF`) on the
-sm_100a kernels of csrc/pqmf.cu.
+sm_90a kernels of csrc/pqmf.cu.
 
 Filter design (host side, once at init; rave/pqmf.py:32-89) is numpy/scipy exactly as the
 reference does it, written against the current scipy API (`firwin(fs=2*pi)` is scipy-1.10's

@@ -1,7 +1,7 @@
 """Algorithmic work of the library's launches: FLOPs and bytes per C-ABI call from its integer arguments (the
 formulas of DESIGN.md section 5: every tensor a launch must read or write, once; weights once).
 
-Used by bench.py (`roofline`, `step_roofline`) and scripts/profile_layers.py together with `_lib.PROFILE`, which logs
+Used by bench.py (`roofline`, `step_roofline`) together with `_lib.PROFILE`, which logs
 (entry point, integer arguments, pointer-presence string, milliseconds) for every call."""
 from typing import Optional, Tuple
 

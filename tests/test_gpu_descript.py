@@ -55,7 +55,7 @@ def test_descript_mrd_vs_oracle():
     g = torch.autograd.grad(sum((a * p.cuda()).sum() for a, p in zip(got, probes)), [xg] + [pg[k] for k in names])
     errs = sorted(((rel_l2(a, b), k) for k, a, b in zip(["x"] + names, g, g_o)), reverse=True)
     print("MRD gradient rel-L2, worst five:", [(k, f"{e:.2e}") for e, k in errs[:5]])
-    # measured on B200 (profiles/r2_gpu_tests.txt): every tensor <= 2e-4 except band 3 / layer 1 (stride-2 (3, 9) conv over
+    # every tensor <= 2e-4 except band 3 / layer 1 (stride-2 (3, 9) conv over
     # the 64-bin band): weight_v 5.9e-4, bias 6.7e-4.  The CPU oracle's own fp32-vs-fp64 distance on these tensors is
     # ~1e-6, so this is kernel summation order on a cancelling sum, not conditioning of the problem; stated bound 1e-3.
     for e, k in errs:
@@ -83,7 +83,7 @@ def test_descript_discriminator_full_vs_oracle():
 
 
 def test_descript_mpd_bf16_engine_vs_oracle():
-    """Descript MPD (1024-channel (5,1) convs: 77 % of the v3 discriminator FLOPs) as ONE tcgen05 chain in bf16 mode
+    """Descript MPD (1024-channel (5,1) convs: 77 % of the v3 discriminator FLOPs) as ONE wgmma chain in bf16 mode
     against the fp32 oracle: features within the bf16-mode tolerance, gradient direction of every large tensor."""
     import rave_b200
     from rave_b200.descript_discriminator import MPD
@@ -122,7 +122,7 @@ def test_descript_mpd_bf16_engine_vs_oracle():
 
 
 def test_descript_mrd_bf16_engine_vs_oracle():
-    """MRD in bf16 mode: every (kt, kf) Conv2d as a one-layer tcgen05 chain (conv along frequency, time taps folded into
+    """MRD in bf16 mode: every (kt, kf) Conv2d as a one-layer wgmma chain (conv along frequency, time taps folded into
     channels) against the fp32 oracle: features within the bf16-mode tolerance, gradient direction."""
     import rave_b200
     from rave_b200.descript_discriminator import MRD

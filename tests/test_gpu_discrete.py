@@ -1,6 +1,6 @@
 """GPU: the `discrete` configuration (BASELINE config 5: EnCodec-style RVQ head, causal padding) on the device --
 DiscreteEncoder + ResidualVectorQuantization against the same modules on CPU (bit-exact on CPU against the reference:
-tests/test_quantization_cpu.py), the causal encoder / generator chains of the tcgen05 engine against the oracle, and the
+tests/test_quantization_cpu.py), the causal encoder / generator chains of the wgmma engine against the oracle, and the
 whole training step of the configuration."""
 import pytest
 import torch

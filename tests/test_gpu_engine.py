@@ -32,7 +32,7 @@ def bf16_mode():
 
 @pytest.mark.parametrize("name,ratios", [("v2", [4, 4, 4, 2]), ("v2", [4, 2, 2, 2]), ("v3", [4, 4, 4, 2])])
 def test_autoencoder_bf16_vs_oracle(name, ratios):
-    """v3: Snake + AdaIN chains on the tcgen05 kernels (rave_snake_cl_fwd / _bwd between the convs)."""
+    """v3: Snake + AdaIN chains on the wgmma kernels (rave_snake_cl_fwd / _bwd between the convs)."""
     from rave_b200 import configs
     from rave_b200.model import _pqmf_decode, _pqmf_encode
     torch.manual_seed(3)

@@ -536,14 +536,14 @@ def test_training_step_matches_reference_goldens_fp32():
         # phase-2 generator step: the gradient is a sum of sign terms through a freshly initialised discriminator -- the
         # reference's own fp32 gradient is 1.1e-2 from an fp64 evaluation, the CPU restatement 2.0e-2 from the reference,
         # the GPU kernels 4.6e-2 (other summation order: other sign flips); the fraction of Adam updates that move by
-        # more than 5 % of lr scales with that distance (measured on B200: 10.6 %)
+        # more than 5 % of lr scales with that distance
         frac = 0.15 if st["name"] == "phase2_gen" else UPD_FRAC[st["name"]]
         assert n_all > 0 and n_bad <= frac * n_all, (st["name"], n_bad, n_all)
         prev = st["state_dict"]
 
 
 def test_training_step_matches_reference_goldens_bf16():
-    """Same three steps on the tcgen05 engine (bf16 operands, fp32 accumulate).  Stated tolerance: losses within
+    """Same three steps on the wgmma engine (bf16 operands, fp32 accumulate).  Stated tolerance: losses within
     3 % (spectral distances, KL) / 10 % (feature matching, adversarial: sums of sign-like terms over bf16 features) of
     the reference's; gradient direction cos >= 0.9 over all stepped tensors."""
     g, out = _run_golden_training_steps("bf16")
@@ -718,7 +718,7 @@ def test_streaming_cached_convs_reproduce_offline():
     x = torch.randn(2, 16, 2048, device="cuda")
     # the transposed conv's symmetric crop is a 2-sample delay even with causal convs around it.  The first samples are
     # a start-up transient in ANY cached-conv implementation: offline, the layers after the transposed conv see zero
-    # padding where the stream carries the two cropped-away samples (measured on B200: only outputs 0..1 differ, 7e-4).
+    # padding where the stream carries the two cropped-away samples.
     y_on, y_off, _ = _stream_vs_offline(stack("causal"), x, 256)
     warm = 16
     assert rel_l2(y_on[..., 2 + warm:], y_off[..., warm:-2]) < 1e-5

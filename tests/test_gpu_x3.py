@@ -1,4 +1,4 @@
-"""GPU: the split-operand ("bf16x3") mode of the tcgen05 conv engine -- the accurate fast mode.  Operands are carried
+"""GPU: the split-operand ("bf16x3") mode of the wgmma conv engine -- the accurate fast mode.  Operands are carried
 as x = hi + lo (two bf16 halves, 16-bit significand) and every product is hi*hi + lo*hi + hi*lo accumulated in fp32 on
 the tensor cores.  Stated tolerance: 2e-5 rel-L2 per conv against the fp32 CPU oracle on UN-rounded operands, 1e-4
 rel-L2 end to end for PQMF + encoder + generator (the north-star tolerance; single-pass bf16 sits at ~1e-2)."""
