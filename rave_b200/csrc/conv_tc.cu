@@ -115,8 +115,7 @@ __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, 
     if (!X3 && p.res_bf16) ld_words<NW>(p.res_bf16 + off, rb);
     if (!X3 && p.dact_src) ld_words<NW>(p.dact_src + off, dm);
   }
-  if (CW == 32) tmem_ld_32x32(taddr, v);
-  else tmem_ld_32x16(taddr, v);
+  acc_ld<CW>(taddr, v);
   if (!valid) return;
   if (p.bias) {
     const float4 *b4 = reinterpret_cast<const float4 *>(p.bias + co);
@@ -303,6 +302,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+      // One wgmma group stays in flight: k-block kb is issued before the group of kb - 1 is waited for, so the tensor
+      // pipe does not drain between k-blocks.  A stage is released once the group that reads it has completed.
+      int prev = 0;                   // stage of the group still in flight (k-block kb - 1)
       for (int kb = 0; kb < kblocks; ++kb) {
         mbar_wait(&full_bar[stage], phase);
         const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
@@ -329,13 +331,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
           }
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs<BLOCK_N / 2>(d[0]);
-        wgmma_fence_regs<BLOCK_N / 2>(d[1]);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);           // this warp's MMAs no longer read the slot
+        wgmma_wait<1>();                                         // the group of k-block kb - 1 has completed
+        if (kb > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);          // this warp's MMAs no longer read that slot
+        }
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+      wgmma_fence_regs<BLOCK_N / 2>(d[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);              // the last k-block's slot
       mbar_wait(tempty_bar, (it & 1) ^ 1);                       // the epilogue has read the previous tile
       acc_store<BLOCK_N>(d, threadIdx.x);
       mbar_arrive(tfull_bar);
@@ -633,7 +641,8 @@ extern "C" int rave_conv1d_tc_fwd_x3(const void *xa, const void *wt, const float
 // activated operand xa, N = Cin).  The reduction runs over tensor ROWS, so both operands are MN-major
 // (the channel axis is contiguous): tiles are stored as 64-channel slabs [64 rows][64 ch] (128-byte
 // rows, SWIZZLE_128B), LBO = slab stride, SBO = 8 rows.  One CTA owns one (m-tile, n-tile, tap) and one
-// slice of the rows (split-K); partial tiles are combined with fp32 atomics into a pre-zeroed dWt.
+// slice of the rows (split-K) and writes its partial tile to its own slice of dWt[splits][K][Cm][Cn] (no atomics);
+// tapmajor_to_weight_kernel adds the slices in slice order.
 // Reference: autograd of F.conv1d / F.conv_transpose1d (weight gradient) at the call sites listed above.
 // =============================================================================================
 namespace rave {
@@ -738,7 +747,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
       // MMA warpgroup: bf16 x bf16 -> fp32, A and B both MN-major (transposed operands); M half h = P slab h
       const uint32_t smem_base = smem_u32(smem);
       float d[2][BLOCK_N / 2];
-      int stage = 0;
+      int stage = 0, prev = 0;        // prev: stage of the group still in flight (as in conv_tc_kernel)
       uint32_t phase = 0;
       for (int c = 0; c < my_chunks; ++c) {
         mbar_wait(&full_bar[stage], phase);
@@ -754,13 +763,19 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
                                       (c > 0 || kk > 0) ? 1u : 0u);
         }
         wgmma_commit();
-        wgmma_wait<0>();
-        wgmma_fence_regs<BLOCK_N / 2>(d[0]);
-        wgmma_fence_regs<BLOCK_N / 2>(d[1]);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+        wgmma_wait<1>();                                         // the group of chunk c - 1 has completed
+        if (c > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
+      wgmma_wait<0>();
+      wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+      wgmma_fence_regs<BLOCK_N / 2>(d[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
       store_wgrad_tile<BLOCK_N>(d, dst, m0, n0, p.Cm, p.Cn);
     } else if (do_cs) {
       // bias gradient: column sums of the P tiles while the tensor core consumes them.  Thread = (8-channel group

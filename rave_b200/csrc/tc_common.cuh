@@ -47,12 +47,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t *bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded spin: a mis-programmed pipeline traps instead of hanging the GPU box (a hang is a strike).
+// Bounded spin: a mis-programmed pipeline traps (the launch fails with an error) instead of hanging the GPU.  No
+// printf by default: a function call anywhere in a kernel makes ptxas serialise every wgmma of it (warning C7510: a wait
+// for completion after each m64nNk16), which costs the tensor pipe most of its overlap.  Building with
+// -DRAVE_MBAR_DEBUG prints the block and thread of a timed-out wait before the trap (slow kernels, diagnosis only).
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
     if (++spins > 20000000u) {
+#ifdef RAVE_MBAR_DEBUG
       printf("rave_b200: mbarrier wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
+#endif
       __trap();
     }
   }
@@ -164,7 +169,7 @@ __device__ __forceinline__ void wgmma_fence_regs(float *d) {
 // Accumulator hand-over.  The warps of an epilogue own one ROW of a 128-row tile each (thread = row quad * 32 + lane)
 // and read consecutive columns; wgmma leaves row pieces spread over the lanes of its warpgroup.  The MMA warpgroup
 // therefore stores a finished tile to a shared-memory buffer [128][ld] fp32 (ld = 4 mod 32 words: the 8 lanes of a
-// 16-byte-load phase hit disjoint banks) and the epilogue reads it back with acc_ld_*.  An accumulator address is
+// 16-byte-load phase hit disjoint banks) and the epilogue reads it back with acc_ld.  An accumulator address is
 // (row << 16) | column, relative to the buffer set by acc_bind.
 static __shared__ uint32_t s_acc_addr, s_acc_ld;
 __host__ __device__ constexpr int acc_pitch(int cols) { return (cols + 31) / 32 * 32 + 4; }
@@ -202,8 +207,6 @@ __device__ __forceinline__ void acc_ld(uint32_t taddr, float *v) {
                  : "r"(a + 16u * i)
                  : "memory");
 }
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, float *v) { acc_ld<32>(taddr, v); }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, float *v) { acc_ld<16>(taddr, v); }
 
 // Stores the warpgroup's 128 x BLOCK_N accumulator tile (wgmma fragment layout, see acc_store) into dst rows m0 ..
 // (row pitch Cn, columns from n0), clipped to Cm x Cn.  Cn is a multiple of 8, so a fragment pair is valid as a whole.

@@ -242,7 +242,7 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 #pragma unroll 1
         for (int c0 = part * 32; c0 < NC; c0 += 64) {
           float v[32];
-          tmem_ld_32x32(taddr + c0, v);
+          acc_ld<32>(taddr + c0, v);
           uint32_t pk[16];
 #pragma unroll
           for (int w = 0; w < 16; ++w) {
@@ -289,7 +289,7 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
           const int c0 = part * 32 + 64 * i;
           if (c0 < NC) {
             float v[32];
-            tmem_ld_32x32(taddr + c0, v);
+            acc_ld<32>(taddr + c0, v);
             if (valid) {
               const int col = ch * NC + c0;
 #pragma unroll
