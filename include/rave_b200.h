@@ -240,15 +240,6 @@ int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, const float *g
 int rave_snake_cl_fwd(const void *h_bf16, const float *alpha, void *a_bf16, long rows, int C, void *stream);
 int rave_snake_cl_bwd(const void *ga_bf16, const void *h_bf16, const float *alpha, const void *add_bf16, void *gh_bf16,
                       float *dalpha, long rows, int C, void *stream);
-/* Multi-tap form (csrc/wgrad_mt.cu): one CTA accumulates up to 8 taps from ONE pass over the P rows and haloed Q tiles
- * shared by the taps of a phase.  rave_conv1d_tc_wgrad_mt_plan returns the split count to allocate dwt with, or 0 when
- * the layer must run on rave_conv1d_tc_wgrad (tap pattern / very short rows); same dwt / dbias contract. */
-int rave_conv1d_tc_wgrad_mt_supported(int B, int Cm, int Lp, int Cn, int K);
-int rave_conv1d_tc_wgrad_mt_splits(int B, int Cm, int Lp, int Cn, int K);
-int rave_conv1d_tc_wgrad_mt_plan(int B, int Cm, int Lp, int Cn, int K, int stride, int dil, int pad_l);
-int rave_conv1d_tc_wgrad_mt(const void *P_bf16, const void *Q_bf16, float *dwt, float *dbias, int B, int Cm, int Lp,
-                            int p_pitch, int Cn, int Lq, int q_pitch, int K, int stride, int dil, int pad_l,
-                            void *stream);
 int rave_conv1d_tc_wgrad(const void *P_bf16, const void *Q_bf16, float *dwt, float *dbias, int B, int Cm, int Lp,
                          int p_pitch, int Cn, int Lq, int q_pitch, int K, int stride, int dil, int pad_l,
                          void *stream);

@@ -610,6 +610,7 @@ __device__ __forceinline__ float c1_src_value(const float *__restrict__ xb, int 
   return pool > 1 ? v / (float)pool : v;
 }
 
+// Per-thread variant, only for shapes whose staged tile (below) exceeds 96 KB of shared memory (large periods).
 // grid (ceil(pitch/256), R), block 256: one thread = one position = one 32-byte row of X (a single 256-bit store);
 // the K source positions of neighbouring threads overlap (K > stride), so the strided reads hit in L1
 __global__ void __launch_bounds__(256)
@@ -637,7 +638,7 @@ im2col_c1_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ X, int
   dst[1] = make_uint4(wds[4], wds[5], wds[6], wds[7]);
 }
 
-// Staged variant (the default): the per-thread gather above issues 16 strided loads per output row -- a warp access
+// Staged variant (every tile up to 96 KB): the per-thread gather above issues 16 strided loads per output row -- a warp access
 // touches 32 addresses (stride * period) floats apart, 8-44 sectors for 128 useful bytes, and the L1 wavefront queue,
 // not HBM, set its pace (40 us for a 33 MB operand).  Here one CTA serves IC_NL output positions of ALL `period` rows
 // of one source batch entry: the contiguous source span is read once, coalesced, and de-interleaved into shared memory
@@ -726,15 +727,10 @@ extern "C" int rave_im2col_c1(const float *x, void *X_bf16, int R, int src_pitch
   RAVE_CHECK_ARG(x && X_bf16 && R > 0 && R <= 65535 && K > 0 && K <= 16 && out_pitch >= Lout && period >= 1 &&
                      pool >= 1 && (period == 1 || pool == 1) && R % period == 0,
                  "im2col_c1: bad argument");
-  static int staged = -1;
-  if (staged < 0) {
-    const char *e = getenv("RAVE_C1_STAGED");          // 0: the per-thread gather (debug / ablation)
-    staged = (e && atoi(e) == 0) ? 0 : 1;
-  }
   const int n_p = (IC_NL - 1) * stride + K;
   const int line = (ic_skew_host(n_p - 1) + 1) | 1;    // odd pitch: the de-interleaving stores spread over the banks
   const size_t smem = (size_t)period * line * sizeof(float);
-  if (staged && stride >= 1 && smem <= 96 * 1024) {
+  if (stride >= 1 && smem <= 96 * 1024) {
     static bool attr = false;
     if (!attr) {
       cudaFuncSetAttribute(im2col_c1_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);

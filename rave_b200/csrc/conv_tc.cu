@@ -15,7 +15,6 @@
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
-#include <stdlib.h>
 #include <string.h>
 
 #include "common.cuh"
@@ -539,12 +538,7 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   const int BK = pick_block_k(Cin);
   // 256-byte L2 promotion over-fetches when a TMA row is a 64-byte (or shorter) span of a 192-byte channel row
   // (measured on the Cin = 96 layers: 209.6 -> 184.7 us); neutral to slightly positive for 128-byte spans.
-  CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  {
-    const char *e = getenv("RAVE_TC_L2PROMO");
-    if (e) promo = atoi(e) == 0 ? CU_TENSOR_MAP_L2_PROMOTION_NONE : atoi(e) == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_64B
-                   : atoi(e) == 128 ? CU_TENSOR_MAP_L2_PROMOTION_L2_128B : CU_TENSOR_MAP_L2_PROMOTION_L2_256B;
-  }
+  const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
   TcParams p;
   p.B = B; p.Cin = Cin; p.Lin = Lin; p.Cout = Cout; p.Lout = Lout; p.K = K; p.stride = stride; p.dil = dil;
   p.pad_l = pad_l; p.act = act; p.slope = slope; p.bias = bias; p.res = res; p.out_f32 = out_f32;

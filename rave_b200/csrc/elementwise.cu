@@ -3,8 +3,6 @@
 // Reference: torch.nn.utils.weight_norm via blocks.normalization (rave/blocks.py:15-22);
 // Snake (blocks.py:852-860); LeakyReLU(.2) (blocks.py:56,90,528,614); GeneratorV2 tail
 // x * sigmoid(a) -> tanh (blocks.py:704-711).
-#include <stdlib.h>
-
 #include "common.cuh"
 
 namespace rave {
@@ -727,7 +725,7 @@ __global__ void __launch_bounds__(256) mt_prep_kernel(const __grid_constant__ Mt
   }
 }
 
-// Shared-memory variant (default when a row fits): the split-K partials are read coalesced along c1 and transposed
+// Shared-memory variant (every row whose tile fits in 96 KB): the split-K partials are read coalesced along c1 and transposed
 // into the parameter's own (c1, k) order in SHARED memory, so that v is read and dv written with unit stride, once.  The
 // global-memory version below walks v / dv with stride K (K = 15: 60 sectors per warp access for 128 useful bytes) and
 // writes dv twice: 0.84 ms of a D-step at ~0.65 TB/s.  Index padding i + i/32 keeps the transposing store conflict-free
@@ -785,7 +783,7 @@ __global__ void __launch_bounds__(1024) mt_wn_bwd_smem_kernel(const __grid_const
   if (threadIdx.x == 0) L.dg[c0] = dot / n;
 }
 
-// block size: RAVE_WN_THREADS (default 256; 1024 threads per row measured slower in the step: 10.39 vs 9.98 ms)
+// Global-memory variant, only for rows whose shared-memory tile would exceed 96 KB (C1 * K above ~23.8 k weights).
 __global__ void __launch_bounds__(1024) mt_wn_bwd_kernel(const __grid_constant__ MtTable t) {
   __shared__ float red[32];
   const int li = mt_find_row(t, blockIdx.x);
@@ -1041,15 +1039,10 @@ extern "C" int rave_weight_norm_bwd_multi(int n, const rave_wprep_layer *layers,
     if (h.C1 * h.K > max_row) max_row = h.C1 * h.K;
   }
   t.total_rows = rows;
-  static int wn_threads = 0, wn_smem = -1;
-  if (!wn_threads) {
-    const char *e = getenv("RAVE_WN_THREADS");
-    wn_threads = (e && atoi(e) >= 64 && atoi(e) <= 1024) ? atoi(e) / 32 * 32 : 256;
-    const char *m = getenv("RAVE_WN_SMEM");             // 0: the global-memory kernel (debug / ablation)
-    wn_smem = (m && atoi(m) == 0) ? 0 : 1;
-  }
+  // 256 threads per row: 1024 measured slower in the step (10.39 vs 9.98 ms)
+  constexpr int wn_threads = 256;
   const size_t smem = (size_t)(max_row + (max_row >> 5) + 1) * sizeof(float);
-  if (wn_smem && smem <= 96 * 1024) {                    // a row of <= ~23.8 k weights; >= 2 CTAs per SM
+  if (smem <= 96 * 1024) {                               // a row of <= ~23.8 k weights; >= 2 CTAs per SM
     static bool attr = false;
     if (!attr) {
       cudaFuncSetAttribute(mt_wn_bwd_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);

@@ -253,16 +253,7 @@ __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wa
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
 #ifndef __CUDA_ARCH__
-#include <stdlib.h>
 #include <utility>
-static inline bool pdl_enabled() {
-  static int on = -1;
-  if (on < 0) {
-    const char *e = getenv("RAVE_PDL");
-    on = (e && e[0] == '0') ? 0 : 1;
-  }
-  return on != 0;
-}
 #endif
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
@@ -278,7 +269,7 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...);
 #else
   return cudaSuccess;

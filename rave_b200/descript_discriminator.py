@@ -9,8 +9,6 @@ time stride is ONE library conv1d along frequency over rows [(b, t)] whose chann
 the input channels (`DiscConv2d`): out[b,:,t,:] = sum_dt conv1d_f(x[b,:,t+dt-pt,:], W[:,:,dt,:]).
 Features are POST-activation (descript_discriminator.py:59-61).  No cuDNN on this path.
 """
-import os
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -19,6 +17,10 @@ import torch.nn.functional as F
 from . import _lib, ops
 from .blocks import weight_norm
 from .discriminator import DiscConv2dK1
+
+# MRD feature taps also write the next conv's time-stacked operand in the same pass where the geometry allows it
+# (_feature_tap_stack); False runs the tap and the stacking as separate passes
+FUSE_TAP_STACK = True
 
 
 def WNConv2dK1(*args, **kwargs):
@@ -152,9 +154,9 @@ def _feature_tap_stack(out, slope, B, T, nxt):
     """_feature_tap that also writes the time-stacked operand of the next MRD conv `nxt` (a DiscConv2d) in the same pass,
     when the geometry allows it (kt = 3, pt = 1, no channel padding on either side): returns (a, stats, xs | None)."""
     C = out.shape[2]
-    if (nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous() and os.environ.get(
-            "RAVE_FUSE_TAP_STACK", "1") != "0" and nxt.kernel_size[0] == 3 and nxt.padding[0] == 1
-            and nxt.in_channels == C and C % 4 == 0 and out.shape[0] == B * T):
+    if (FUSE_TAP_STACK and nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous()
+            and nxt.kernel_size[0] == 3 and nxt.padding[0] == 1 and nxt.in_channels == C and C % 4 == 0
+            and out.shape[0] == B * T):
         Fp, Cp = nxt.stacked_geometry(out.shape[1], C)
         if Cp == 3 * C:
             return ops.leaky_fm_stack(out, slope, T, Fp)

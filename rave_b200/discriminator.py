@@ -10,7 +10,6 @@ copy is the 1-channel input.
 from typing import Callable, Optional, Sequence, Type
 
 import numpy as np
-import os
 
 import torch
 import torch.nn as nn
@@ -18,6 +17,10 @@ import torch.nn as nn
 from . import cc, ops
 from .blocks import normalization
 from ._lib import RaveB200Error
+
+# streams the feature-matching discriminator chains are issued on (CombineDiscriminators.forward_fm); RAVE.compute_losses
+# also moves the spectral losses to a side stream when it is above 1.  1 = everything on the current stream
+DISC_STREAMS = 8
 
 
 class DiscConv1d(nn.Conv1d):
@@ -261,7 +264,7 @@ class CombineDiscriminators(nn.Module):
         jobs = []
         for disc in self.discriminators:
             jobs.extend(disc.fm_jobs())
-        ns = int(os.environ.get("RAVE_DISC_STREAMS", "8"))
+        ns = DISC_STREAMS
         if ns <= 1 or not x.is_cuda:
             return [layer.forward_fm(x, fake_grad_only=fake_grad_only, **kw) for layer, kw in jobs]
         # The nets are independent chains of persistent kernels: issued on a few streams, the tail of one kernel (CTAs

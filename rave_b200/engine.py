@@ -29,12 +29,11 @@ from . import _lib, ops
 _state = {"precision": "fp32", "prep_epoch": 0}
 ACT_DTYPE = torch.bfloat16   # storage type of operand / gradient streams (tests may widen it)
 
-
-import os as _os
-# output positions per tensor-core row of a Cin = 1 first layer (see TcChainFn.forward); 1 = plain 16-channel rows
-C1_GROUP = int(_os.environ.get("RAVE_C1_GROUP", "4"))
-# Residual(DilatedUnit) blocks as ONE launch (csrc/unit_tc.cu) where the width allows it; 0 = two launches per unit
-FUSE_UNITS = _os.environ.get("RAVE_FUSE_UNITS", "1") != "0"
+# output positions per tensor-core row of a Cin = 1 first layer (see TcChainFn.forward); pitches that are not a
+# multiple of it run with one position (plain 16-channel rows)
+C1_GROUP = 4
+# Residual(DilatedUnit) blocks as ONE launch (csrc/unit_tc.cu) where the width allows it, else two launches per unit
+FUSE_UNITS = True
 
 
 def set_precision(mode: str) -> None:
@@ -96,12 +95,6 @@ def chain_supported(specs: List[LayerSpec]) -> bool:
 # ----------------------------------------------------------------------------------------------
 # planning: walk a module list into LayerSpecs
 # ----------------------------------------------------------------------------------------------
-
-def _act_of(m):
-    from . import cc
-    code = cc._act_code(m)
-    return code
-
 
 def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
     """EncoderV2.net / GeneratorV2.net style sequences: activations (LeakyReLU or Snake), cc.Conv1d, cc.ConvTranspose1d,

@@ -12,7 +12,6 @@ import math
 from typing import Callable, Dict, Iterable, Optional
 
 import contextlib
-import os
 
 import torch
 import torch.nn as nn
@@ -289,8 +288,9 @@ class RAVE(nn.Module):
         # The spectral losses (20 STFTs + their small kernels) and the discriminator chains only share their inputs:
         # the former go to a side stream so that they fill the holes between the discriminator's persistent kernels
         # (autograd replays each part's backward on its own stream).
+        from . import discriminator
         side = None
-        if y_raw.is_cuda and self.warmed_up and int(os.environ.get("RAVE_DISC_STREAMS", "8")) > 1:
+        if y_raw.is_cuda and self.warmed_up and discriminator.DISC_STREAMS > 1:
             if getattr(self, "_loss_stream", None) is None:
                 self._loss_stream = torch.cuda.Stream()
             side = self._loss_stream

@@ -4,7 +4,6 @@ PyTorch is plumbing here: it owns the device memory, the stream and the autograd
 arithmetic operation of the hot path is one of the library's sm_90a kernels.  There is no
 fallback implementation: host tensors or a missing library raise (`_lib.RaveB200Error`).
 """
-import os
 from typing import Optional, Tuple
 
 import torch
@@ -608,7 +607,7 @@ class LeakyFmStackFn(torch.autograd.Function):
     entries of T steps (first half of the rows real) -> (a, stats, xs) with xs [(b t), Fp, 3 C] bf16 =
     time_stack_nhwc(a.view(B, T, F, C), kt = 3, pt = 1) (rave_leaky_fm_stack_fwd).  The backward is the composition of the
     two stand-alone backward kernels (adjoint of the time stack, then the tap's fused backward) in ONE kernel
-    (rave_leaky_fm_stack_bwd); RAVE_FUSE_TAP_STACK_BWD=0 runs the two kernels."""
+    (rave_leaky_fm_stack_bwd)."""
 
     @staticmethod
     def forward(ctx, x, slope, T, Fp):
@@ -623,7 +622,7 @@ class LeakyFmStackFn(torch.autograd.Function):
              stream_ptr())
         ctx.save_for_backward(a)
         ctx.slope = float(slope)
-        ctx.cfg = (R2 // T, C, T, F_, Fp, 3 * C)
+        ctx.cfg = (C, T, F_, Fp)
         return a, stats, xs
 
     @staticmethod
@@ -631,25 +630,16 @@ class LeakyFmStackFn(torch.autograd.Function):
         (a,) = ctx.saved_tensors
         if ga is None and dstats is None and gxs is None:
             return None, None, None, None
-        B, C, T, F_, Fp, Cp = ctx.cfg
-        if gxs is not None and os.environ.get("RAVE_FUSE_TAP_STACK_BWD", "1") != "0":
+        C, T, F_, Fp = ctx.cfg
+        ga, dstats = _f32c(ga), _f32c(dstats)
+        gx = torch.empty_like(a)
+        if gxs is not None:
             # one pass: adjoint of the time stack + gradient at the feature + feature-matching terms + LeakyReLU'
             gxs = gxs.contiguous()
-            ga, dstats = _f32c(ga), _f32c(dstats)
-            gx = torch.empty_like(a)
             call("rave_leaky_fm_stack_bwd", ptr(a), ptr(gxs), ptr(ga), ptr(dstats), ptr(gx), a.shape[0] // 2, T, F_, C, Fp,
                  ctx.slope, stream_ptr())
-            return gx, None, None, None
-        if gxs is not None:
-            g_st = torch.empty(B, T, F_, C, dtype=torch.float32, device=a.device)
-            gxs = gxs.contiguous()
-            call("rave_time_stack_nhwc_bwd", ptr(gxs), ptr(g_st), B, C, T, F_, Fp, Cp, 3, 1, stream_ptr())
-            g_st = g_st.view_as(a)
-            ga = g_st if ga is None else g_st.add_(_f32c(ga))
-        ga = _f32c(ga)
-        dstats = _f32c(dstats)
-        gx = torch.empty_like(a)
-        call("rave_leaky_fm_bwd", ptr(a), ptr(ga), ptr(dstats), ptr(gx), a.numel() // 2, ctx.slope, stream_ptr())
+        else:
+            call("rave_leaky_fm_bwd", ptr(a), ptr(ga), ptr(dstats), ptr(gx), a.numel() // 2, ctx.slope, stream_ptr())
         return gx, None, None, None
 
 
@@ -738,14 +728,9 @@ def conv1d_tc_wgrad(P_cl, Q_cl, K, stride=1, dil=1, pad_l=0, Lp=None, Lq=None, d
     Lq = q_pitch if Lq is None else Lq
     if P_cl.dtype != torch.bfloat16 or Q_cl.dtype != torch.bfloat16:
         raise _lib.RaveB200Error("conv1d_tc_wgrad: operands must be bf16")
-    lib = _lib.load()
-    splits = lib.rave_conv1d_tc_wgrad_mt_plan(B, Cm, Lp, Cn, K, stride, dil, pad_l)
-    entry = "rave_conv1d_tc_wgrad_mt"          # all taps of a group from one pass over P (csrc/wgrad_mt.cu)
-    if splits <= 0:
-        splits = lib.rave_conv1d_tc_wgrad_splits(B, Cm, Lp, Cn, K)
-        entry = "rave_conv1d_tc_wgrad"         # per-tap kernel: tap patterns / row lengths the haloed tiles do not cover
+    splits = _lib.load().rave_conv1d_tc_wgrad_splits(B, Cm, Lp, Cn, K)
     dwt = torch.empty(splits, K, Cm, Cn, dtype=torch.float32, device=P_cl.device)   # per-slice partial sums
-    call(entry, ptr(P_cl), ptr(Q_cl), ptr(dwt), dbias.data_ptr() if dbias is not None else None,
+    call("rave_conv1d_tc_wgrad", ptr(P_cl), ptr(Q_cl), ptr(dwt), dbias.data_ptr() if dbias is not None else None,
          B, Cm, Lp, p_pitch, Cn, Lq, q_pitch, K, stride, dil, pad_l, stream_ptr())
     return dwt
 
@@ -1009,13 +994,6 @@ class RfftFn(torch.autograd.Function):
             z = torch.complex(z.real, torch.cat([torch.zeros_like(z.imag[..., :1]), z.imag[..., 1:-1],
                                                  torch.zeros_like(z.imag[..., :1])], -1))
         return torch.fft.irfft(z, n=ctx.n), None
-
-
-def rfft_weights(n, device):
-    w = torch.full((n // 2 + 1,), 0.5 * n, dtype=torch.float32, device=device)
-    w[0] = n
-    w[-1] = n
-    return w
 
 
 def rfft(x, w):

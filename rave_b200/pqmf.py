@@ -135,10 +135,6 @@ class PQMF(nn.Module):
         return ops.PqmfSynthesisFn.apply(x, t["w"], t["w_bwd"], t["w_pad"], t["w_bwd_pad"])
 
 
-import os as _os
-USE_FAST = _os.environ.get("RAVE_PQMF_DENSE", "0") != "1"      # factorised kernels when the bank is cosine-modulated (always, for rave/pqmf.py designs)
-
-
 def _require_16(n_band):
     if n_band != 16:
         raise RaveB200Error(f"only the 16-band PQMF (every shipped config) has a device kernel, got {n_band}")
@@ -198,9 +194,10 @@ def _build_tables(taps, pad_l, pad_r, w, w_pad):
                taps_bwd_pad=P, w=w.contiguous(), w_pad=w_pad, w_bwd=w_bwd,
                w_bwd_pad=16 * (K - 1 - w_pad), dense=dict(taps=taps.contiguous(), taps_bwd=taps_bwd.contiguous(),
                                                           w=w.contiguous(), w_bwd=w_bwd))
-    if USE_FAST and K <= 33:
-        # factorised tables for the fast kernels (csrc/pqmf.cu): analysis-form tables are [16][n], synthesis-form
-        # weights w[m][c][j] are the band filters H[c][16 j + m]
+    if K <= 33:
+        # factorised tables for the fast kernels (csrc/pqmf.cu) when the bank is cosine-modulated (always, for
+        # rave/pqmf.py designs): analysis-form tables are [16][n], synthesis-form weights w[m][c][j] are the band
+        # filters H[c][16 j + m]
         def syn_as_bank(wt):
             return wt.permute(1, 2, 0).reshape(16, -1)
         fa, fs = _factorise(taps), _factorise(syn_as_bank(w))

@@ -99,10 +99,10 @@ def instance(lib, name, ints):
     if name == "rave_conv1d_tc_fwd":
         v = lib.rave_conv1d_tc_plan(ints[0], ints[1], ints[4], ints[5], ints[6])
         return f"conv<{v & 0xfff},{(v >> 12) & 0xfff}>"
-    if name in ("rave_conv1d_tc_wgrad", "rave_conv1d_tc_wgrad_mt"):
+    if name == "rave_conv1d_tc_wgrad":
         Bc, Cm, Lp, pp, Cn = ints[:5]
         s = lib.rave_conv1d_tc_wgrad_splits(Bc, Cm, Lp, Cn, ints[7])
-        return f"wgrad<{64 if Cn <= 64 else 128}> x{s}" + (" (mt)" if name.endswith("_mt") else "")
+        return f"wgrad<{64 if Cn <= 64 else 128}> x{s}"
     return name
 
 
@@ -155,7 +155,7 @@ def main():
     for (name, ints, ptrs), r in rows.items():
         if name == "rave_conv1d_tc_fwd":
             run, nb = fwd_runner(torch, ops, ints, ptrs)
-        elif name in ("rave_conv1d_tc_wgrad", "rave_conv1d_tc_wgrad_mt"):
+        elif name == "rave_conv1d_tc_wgrad":
             run, nb = wgrad_runner(torch, ops, ints, ptrs)
         else:
             print(f"# not re-timed: {name} {ints}", flush=True)

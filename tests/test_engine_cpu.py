@@ -478,6 +478,7 @@ def test_mrd_channel_last_engine_path_vs_oracle(emu, monkeypatch):
     """The MRD's engine path (channel-last end to end, one-layer chains, feature taps that also write the next conv's
     time-stacked operand) against the oracle's Conv2d form of rave/descript_discriminator.py:118-184: every feature and
     the input gradient; the fused tap + stack and the separate passes give the same numbers."""
+    from rave_b200 import descript_discriminator
     from rave_b200.descript_discriminator import MRD
     torch.manual_seed(21)
     mrd = MRD(256)
@@ -488,8 +489,8 @@ def test_mrd_channel_last_engine_path_vs_oracle(emu, monkeypatch):
     probes = [torch.randn_like(f) for f in want]
     (g_o,) = torch.autograd.grad(sum((f * p).sum() for f, p in zip(want, probes)), xo)
     res = {}
-    for fuse in ("1", "0"):
-        monkeypatch.setenv("RAVE_FUSE_TAP_STACK", fuse)
+    for fuse in (True, False):
+        monkeypatch.setattr(descript_discriminator, "FUSE_TAP_STACK", fuse)
         xe = x.clone().requires_grad_(True)
         got = mrd._forward_cl(xe)
         assert len(got) == len(want) == 26
@@ -503,6 +504,6 @@ def test_mrd_channel_last_engine_path_vs_oracle(emu, monkeypatch):
         (g_e,) = torch.autograd.grad(sum((f * p).sum() for f, p in zip(got, probes)), xe)
         assert rel_l2(g_e, g_o) < tol(emu, 5e-5, 0.1), (fuse, rel_l2(g_e, g_o))
         res[fuse] = ([f.detach().clone() for f in got], g_e)
-    for a, b in zip(res["1"][0], res["0"][0]):
+    for a, b in zip(res[True][0], res[False][0]):
         assert torch.equal(a, b)
-    assert rel_l2(res["1"][1], res["0"][1]) < 1e-6
+    assert rel_l2(res[True][1], res[False][1]) < 1e-6

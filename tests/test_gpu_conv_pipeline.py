@@ -191,9 +191,8 @@ def test_x3(case):
     (2, 96, 64, 1000, 5),     # 32 chunks split into slices of 8
     (3, 128, 128, 700, 7),    # 33 chunks: slices not a multiple of the stages
 ])
-def test_wgrad_chunk_counts(case, monkeypatch):
+def test_wgrad_chunk_counts(case):
     from rave_b200 import _lib, ops
-    monkeypatch.setenv("RAVE_WG_MT", "0")         # the per-tap kernel of csrc/conv_tc.cu
     B, Cm, Cn, L, K = case
     g = torch.Generator().manual_seed(L + K)
     pad_l = K // 2

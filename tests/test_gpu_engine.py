@@ -144,14 +144,14 @@ def test_fused_feature_matching_bf16_vs_oracle():
     assert rel_l2(fm, fm_o) < FWD_TOL and rel_l2(ld, ld_o) < FWD_TOL and rel_l2(la, la_o) < 5e-2
 
 
-@pytest.mark.parametrize("streams", ["1", "8"])
+@pytest.mark.parametrize("streams", [1, 8])
 def test_cuda_graph_training_matches_eager(streams, monkeypatch):
     """GraphedTrainer replays == eager training_step on the same data (same kernels, same order); with the
     discriminator nets captured on 8 side streams against a single-stream eager twin."""
     import copy
-    monkeypatch.setenv("RAVE_DISC_STREAMS", streams)
-    from rave_b200 import configs
+    from rave_b200 import configs, discriminator
     from rave_b200.graphs import GraphedTrainer
+    monkeypatch.setattr(discriminator, "DISC_STREAMS", streams)
     torch.manual_seed(0)
     m1 = configs.build_rave("v2", capacity=16, latent_size=16, disc_capacity=16).cuda().train()
     m1.warmed_up = True
@@ -166,7 +166,7 @@ def test_cuda_graph_training_matches_eager(streams, monkeypatch):
     # the trainer's eager warm-up is undone (parameters, buffers, optimiser state restored) and capture itself executes
     # nothing: the twin starts from the same state without any catching up
     assert torch.equal(w_before, m2.decoder.net[0].weight_v)
-    monkeypatch.setenv("RAVE_DISC_STREAMS", "1")
+    monkeypatch.setattr(discriminator, "DISC_STREAMS", 1)
     m1.optimizers(capturable=True)
     for i in range(4):
         la = tr.step(x, i)

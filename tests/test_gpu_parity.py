@@ -44,28 +44,36 @@ def test_pqmf_operators_golden(mode):
 
 
 def test_pqmf_backward_vs_oracle():
-    from rave_b200 import pqmf
+    """The module's factorised tables, and the dense tables of the kernels that serve banks which do not factorise."""
+    from rave_b200 import ops, pqmf
     p = pqmf.CachedPQMF(attenuation=100, n_band=16).cuda()
     hk = p.hk.cpu()
+    t = p._tables()
+    d = t["dense"]
+    assert isinstance(t["taps"], tuple) and isinstance(t["w"], tuple)
+    dense = (lambda v: ops.PqmfAnalysisFn.apply(v, d["taps"], d["taps_bwd"], t["pad_l"], t["pad_r"], t["taps_bwd_pad"]),
+             lambda v: ops.PqmfSynthesisFn.apply(v, d["w"], d["w_bwd"], t["w_pad"], t["w_bwd_pad"]))
     x = torch.randn(3, 1, 4096)
     xo = x.clone().requires_grad_(True)
     yo = O.pqmf_analysis(xo, hk)
     gy = torch.randn_like(yo)
     (gx_o,) = torch.autograd.grad(yo, xo, gy)
-    xg = x.cuda().requires_grad_(True)
-    yg = p(xg)
-    (gx,) = torch.autograd.grad(yg, xg, gy.cuda())
-    assert rel_l2(gx, gx_o) < 1e-5
     yb = torch.randn(3, 16, 256)
     ybo = yb.clone().requires_grad_(True)
     so = O.pqmf_synthesis(ybo, hk)
     gs = torch.randn_like(so)
     (gyb_o,) = torch.autograd.grad(so, ybo, gs)
-    ybg = yb.cuda().requires_grad_(True)
-    sg = p.inverse(ybg)
-    (gyb,) = torch.autograd.grad(sg, ybg, gs.cuda())
-    assert rel_l2(sg, so) < 2e-6
-    assert rel_l2(gyb, gyb_o) < 1e-5
+    for analysis, synthesis in [(p, p.inverse), dense]:
+        xg = x.cuda().requires_grad_(True)
+        yg = analysis(xg)
+        (gx,) = torch.autograd.grad(yg, xg, gy.cuda())
+        assert rel_l2(yg, yo) < 2e-6
+        assert rel_l2(gx, gx_o) < 1e-5
+        ybg = yb.cuda().requires_grad_(True)
+        sg = synthesis(ybg)
+        (gyb,) = torch.autograd.grad(sg, ybg, gs.cuda())
+        assert rel_l2(sg, so) < 2e-6
+        assert rel_l2(gyb, gyb_o) < 1e-5
 
 
 def test_pqmf_non_cached_variant_matches_polyphase_reference():

@@ -77,13 +77,9 @@ WG_CASES = [
 ]
 
 
-@pytest.mark.parametrize("multi_tap", [False, True])
 @pytest.mark.parametrize("case", WG_CASES)
-def test_conv1d_tc_wgrad_vs_oracle(case, multi_tap, monkeypatch):
-    """multi_tap: the opt-in kernel of csrc/wgrad_mt.cu (all taps of a group from one pass over P, haloed Q tiles); layers it
-    does not take (rows shorter than 16, tap patterns that do not fit) fall back to the per-tap kernel inside ops."""
+def test_conv1d_tc_wgrad_vs_oracle(case):
     from rave_b200 import ops
-    monkeypatch.setenv("RAVE_WG_MT", "1" if multi_tap else "0")
     B, Cm, Cn, L, K, stride, dil, pad_l, pad_r = case
     g = torch.Generator().manual_seed(hash(case) % (2 ** 31))
     x = torch.randn(B, Cn, L, generator=g).bfloat16().float()
@@ -138,7 +134,8 @@ def test_small_channel_kernels_vs_emulator():
         assert rel_l2(ops.gather_c1(Pm.cuda(), (R, L + 3), L, Lout, K, stride, pad),
                       E.gather_c1(Pm, (R, L + 3), L, Lout, K, stride, pad)) < 1e-6
         # the same rows read in place from a signal tensor: fold by a period / average pooling
-        for (period, pool) in [(3, 1), (7, 1), (1, 2), (1, 4)]:
+        # period 64: the staged tile exceeds 96 KB of shared memory and the per-thread im2col kernel runs
+        for (period, pool) in [(3, 1), (7, 1), (1, 2), (1, 4), (64, 1)]:
             Bs, T = 4, L * period * pool - (2 if period > 1 else 0) + (1 if pool > 1 else 0)
             src = torch.randn(Bs, T)
             Ls = (T + period - 1) // period if period > 1 else T // pool
@@ -169,7 +166,8 @@ def test_multi_tensor_weight_kernels_match_single():
     torch.manual_seed(1)
     items, singles = [], []
     for (C0, C1, K, wn, C0p, C1p) in [(96, 16, 7, True, 96, 16), (192, 96, 8, True, 192, 96), (96, 1, 15, True, 96, 16),
-                                      (1, 768, 1, False, 16, 768), (1536, 768, 4, True, 1536, 768), (48, 48, 3, True, 48, 48)]:
+                                      (1, 768, 1, False, 16, 768), (1536, 768, 4, True, 1536, 768), (48, 48, 3, True, 48, 48),
+                                      (8, 2048, 15, True, 16, 2048)]:
         v = torch.randn(C0, C1, K, device="cuda")
         g = (torch.rand(C0, 1, 1, device="cuda") + 0.5) if wn else None
         tapsA = list(range(K))
@@ -188,7 +186,9 @@ def test_multi_tensor_weight_kernels_match_single():
         dwt = torch.randn(3, K, C0p, C1p, device="cuda")
         jobs.append((dwt, v, g, norm))
         ref.append(ops.weight_norm_bwd_tapmajor(dwt, v, g, norm))
-    out = ops.weight_norm_bwd_multi(jobs)
+    # one launch takes the kernel its widest row allows: the last row (C1 K > 24 k weights) does not fit the shared-memory
+    # tile, so on its own it runs the global-memory kernel
+    out = ops.weight_norm_bwd_multi(jobs[:-1]) + ops.weight_norm_bwd_multi(jobs[-1:])
     for (dv1, dg1), (dv2, dg2) in zip(ref, out):
         assert torch.allclose(dv1, dv2, rtol=1e-5, atol=1e-6)
         assert (dg1 is None) == (dg2 is None)
