@@ -214,6 +214,12 @@ int rave_time_stack_nhwc(const float *x, void *out_bf16, int B, int C, int T, in
                          int pt, void *stream);
 int rave_time_stack_nhwc_bwd(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp, int kt, int pt,
                              void *stream);
+/* The same with time dilation dil (EncodecConvNet of the multi-scale spectral discriminator, rave/discriminator.py:54-74):
+ * out[(b,t)][f][dt*C + c] = x[b][t + dt*dil - pt][f][c]; dil = 1 is rave_time_stack_nhwc. */
+int rave_time_stack_nhwc_dil(const float *x, void *out_bf16, int B, int C, int T, int F, long sb, long st, int Fp, int Cp,
+                             int kt, int pt, int dil, void *stream);
+int rave_time_stack_nhwc_dil_bwd(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp, int kt, int pt,
+                                 int dil, void *stream);
 /* L1 feature matching on fp32 features (core.mean_difference, rave/core.py:236-252): stats[0] += sum|t - v|,
  * stats[1] += sum|t| (stats zeroed by the caller); gradient of d[0] * stats[0] + d[1] * stats[1]: gt = d0 sgn(t - v) +
  * d1 sgn(t), gv = -d0 sgn(t - v) (either may be null). */
@@ -234,6 +240,12 @@ int rave_leaky_fm_stack_fwd(const float *x, float *a, float *stats, void *xs_bf1
  * feature-matching terms d (nullable)) * LeakyReLU'(a) */
 int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx, long Rh, int T,
                             int F, int C, int Fp, float slope, void *stream);
+/* the same tap and backward for a next conv with time dilation dil (kt = 3, pt = dil):
+ * xs = rave_time_stack_nhwc_dil(a, kt = 3, pt = dil, dil); dil = 1 is rave_leaky_fm_stack_fwd / _bwd. */
+int rave_leaky_fm_stack_dil_fwd(const float *x, float *a, float *stats, void *xs_bf16, long Rh, int T, int F, int C, int Fp,
+                                int dil, float slope, void *stream);
+int rave_leaky_fm_stack_dil_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx, long Rh,
+                                int T, int F, int C, int Fp, int dil, float slope, void *stream);
 /* Snake (rave/blocks.py:852-860) on the engine's channel-last bf16 streams [rows][C] (v3 chains on the wgmma kernels):
  * a = h + sin^2(alpha h) / (alpha + 1e-9);  backward: gh = ga * da/dh + add (add may be null), dalpha[c] += sum_rows
  * ga * da/dalpha (dalpha zeroed by the caller). */
@@ -311,6 +323,13 @@ int rave_stft_frames(const float *x, const float *window, float *frames, int N, 
                      void *stream);
 int rave_stft_frames_bwd(const float *dframes, const float *window, float *dx, int N, int T, int n_fft, int hop,
                          void *stream);
+/* Uncentred framing of torchaudio Spectrogram(center=False, normalized=True) (rave/discriminator.py:12-20):
+ * frames[n][f][t] = scale * window[t] * x[n][f*hop + t], F = 1 + (T - n_fft)/hop frames, no padding (scale = 1/||w||_2
+ * for normalized=True); and its adjoint dx[n][j] (overlap-add as a gather, zero past the last frame). */
+int rave_stft_frames_valid(const float *x, const float *window, float *frames, int N, int T, int n_fft, int hop,
+                           float scale, void *stream);
+int rave_stft_frames_valid_bwd(const float *dframes, const float *window, float *dx, int N, int T, int n_fft, int hop,
+                               float scale, void *stream);
 /* gradient of rfft (last axis, n = 2*(bins-1)) prepared for ONE c2r transform: Z[k] = G[k]*n*(1 | 1/2 | ... | 1/2 | 1)
  * with the imaginary parts of the DC / Nyquist bins dropped; dx = irfft(Z, n).  G [N][F][bins] complex64 with element
  * strides (sN, sF, sB); Z contiguous. */

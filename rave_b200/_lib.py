@@ -53,11 +53,15 @@ SIGNATURES = {
     "rave_time_stack_cl_bwd": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_time_stack_nhwc": (c_int, [_P, _P, _I, _I, _I, _I, ctypes.c_long, ctypes.c_long, _I, _I, _I, _I, _P]),
     "rave_time_stack_nhwc_bwd": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "rave_time_stack_nhwc_dil": (c_int, [_P, _P, _I, _I, _I, _I, ctypes.c_long, ctypes.c_long, _I, _I, _I, _I, _I, _P]),
+    "rave_time_stack_nhwc_dil_bwd": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_l1_stats_f32": (c_int, [_P, _P, _P, ctypes.c_long, _P]),
     "rave_leaky_fm_fwd": (c_int, [_P, _P, _P, ctypes.c_long, ctypes.c_float, _P]),
     "rave_leaky_fm_bwd": (c_int, [_P, _P, _P, _P, ctypes.c_long, ctypes.c_float, _P]),
     "rave_leaky_fm_stack_fwd": (c_int, [_P, _P, _P, _P, ctypes.c_long, _I, _I, _I, _I, ctypes.c_float, _P]),
     "rave_leaky_fm_stack_bwd": (c_int, [_P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _I, _I, ctypes.c_float, _P]),
+    "rave_leaky_fm_stack_dil_fwd": (c_int, [_P, _P, _P, _P, ctypes.c_long, _I, _I, _I, _I, _I, ctypes.c_float, _P]),
+    "rave_leaky_fm_stack_dil_bwd": (c_int, [_P, _P, _P, _P, _P, ctypes.c_long, _I, _I, _I, _I, _I, ctypes.c_float, _P]),
     "rave_l1_grad_f32": (c_int, [_P, _P, _P, _P, _P, ctypes.c_long, _P]),
     "rave_snake_cl_fwd": (c_int, [_P, _P, _P, ctypes.c_long, _I, _P]),
     "rave_snake_cl_bwd": (c_int, [_P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _P]),
@@ -78,6 +82,8 @@ SIGNATURES = {
     "rave_spectral_grad": (c_int, [_P, _P, _P, _P, _P, _L, _F, _P]),
     "rave_stft_frames": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "rave_stft_frames_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    "rave_stft_frames_valid": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
+    "rave_stft_frames_valid_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_rfft_bwd_scale": (c_int, [_P, _P, _L, _I, _I, _L, _L, _L, _P]),
     "rave_noise_fir_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_noise_fir_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),

@@ -27,6 +27,9 @@ ARCH = {
     "discrete": dict(capacity=96, ratios=[4, 4, 2, 2], activation="leaky", adain=False, disc="v2",
                      update_discriminator_every=4, phase_1_duration=200000, discrete=True,
                      noise_augmentation=128, log_epsilon=1.0, num_skipped_features=0),
+    # `--config v2 --config spectral_discriminator`: v2 with the MPD replaced by the multi-scale spectral discriminator
+    "v2_spectral": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False,
+                        disc="v2_spectral", update_discriminator_every=4, phase_1_duration=1000000),
 }
 
 
@@ -75,9 +78,23 @@ def make_discriminator_v2(capacity=96, n_channels=1):
     ], n_channels=n_channels)
 
 
+def make_discriminator_v2_spectral(capacity=96, n_channels=1, spectral_capacity=32,
+                                   scales=(4096, 2048, 1024, 512, 256)):
+    """CombineDiscriminators[MSD(3), MultiScaleSpectralDiscriminator(EncodecConvNet)] (configs/spectral_discriminator.gin:
+    6-17 on top of configs/v2.gin)."""
+    scales_net = partial(discriminator.ConvNet, out_size=1, capacity=capacity, n_layers=4, stride=4,
+                         conv=nn.Conv1d, kernel_size=15)
+    return discriminator.CombineDiscriminators([
+        partial(discriminator.MultiScaleDiscriminator, n_discriminators=3, convnet=scales_net),
+        partial(discriminator.MultiScaleSpectralDiscriminator, scales=list(scales),
+                convnet=partial(discriminator.EncodecConvNet, capacity=spectral_capacity)),
+    ], n_channels=n_channels)
+
+
 def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n_channels=1,
-               padding_mode="centered", phase_1_duration=None, disc_capacity=None, ratios=None):
-    """The full `RAVE` model of a named configuration."""
+               padding_mode="centered", phase_1_duration=None, disc_capacity=None, ratios=None, spectral_capacity=32):
+    """The full `RAVE` model of a named configuration (`spectral_capacity`: EncodecConvNet capacity of "v2_spectral",
+    configs/spectral_discriminator.gin:11)."""
     a = ARCH[name]
     cap = capacity or a["capacity"]
     act = _activation_factory(a["activation"])
@@ -88,6 +105,8 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
     distance = partial(core.AudioDistanceV1, multiscale_stft=stft, log_epsilon=a.get("log_epsilon", 1e-7))
     if a["disc"] == "v2":
         disc = lambda n_channels=1: make_discriminator_v2(disc_capacity or cap, n_channels)
+    elif a["disc"] == "v2_spectral":
+        disc = lambda n_channels=1: make_discriminator_v2_spectral(disc_capacity or cap, n_channels, spectral_capacity)
     else:
         from .descript_discriminator import DescriptDiscriminator
         disc = lambda n_channels=1: DescriptDiscriminator(n_channels=n_channels)

@@ -938,11 +938,12 @@ time_stack_cl_bwd_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict_
 
 // Channel-last source (the MRD keeps its activations channel-last between layers: the conv output [(b, t)][f][c] IS the
 // next layer's [b][t][f][c]): x[b][t][f][c] fp32 with element strides (sb, st), f-stride C, channels contiguous.
-//   out[(b, t)][f][dt * C + c] = x[b][t + dt - pt][f][c]
+//   out[(b, t)][f][dt * C + c] = x[b][t + dt * dil - pt][f][c]
+// (dil > 1: the time dilation of the EncodecConvNet convs of the multi-scale spectral discriminator).
 // One thread = 8 output channels = one 16-byte store; with C % 8 == 0 its 8 sources are two 16-byte loads of one tap.
 __global__ void __launch_bounds__(256)
 time_stack_nhwc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ out, long sb, long st, int C, int T, int F,
-                       int Fp, int Cp, int kt, int pt, long total_vec, int vec) {
+                       int Fp, int Cp, int kt, int pt, int dil, long total_vec, int vec) {
   const int vpr = Cp >> 3;
   const int nch = kt * C;
   for (long i = blockIdx.x * 256L + threadIdx.x; i < total_vec; i += (long)gridDim.x * 256) {
@@ -959,7 +960,7 @@ time_stack_nhwc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ 
     if (f < F && ch0 < nch) {
       if (vec) {
         const int dt = ch0 / C, c = ch0 - dt * C;
-        const int ts = t + dt - pt;
+        const int ts = t + dt * dil - pt;
         if (ts >= 0 && ts < T) {
           const float4 *p = reinterpret_cast<const float4 *>(x + b * sb + ts * st + (long)f * C + c);
           const float4 a0 = __ldg(p), a1 = __ldg(p + 1);
@@ -972,7 +973,7 @@ time_stack_nhwc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ 
           const int ch = ch0 + j;
           if (ch < nch) {
             const int dt = ch / C, c = ch - dt * C;
-            const int ts = t + dt - pt;
+            const int ts = t + dt * dil - pt;
             if (ts >= 0 && ts < T) v[j] = __ldg(x + b * sb + ts * st + (long)f * C + c);
           }
         }
@@ -988,10 +989,10 @@ time_stack_nhwc_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ 
   }
 }
 
-// adjoint into a contiguous [B][T][F][C] fp32 gradient: gx[b][tp][f][c] = sum_dt g[(b, tp + pt - dt)][f][dt * C + c]
+// adjoint into a contiguous [B][T][F][C] fp32 gradient: gx[b][tp][f][c] = sum_dt g[(b, tp + pt - dt * dil)][f][dt * C + c]
 __global__ void __launch_bounds__(256)
 time_stack_nhwc_bwd_kernel(const __nv_bfloat16 *__restrict__ g, float *__restrict__ gx, int C, int T, int F, int Fp,
-                           int Cp, int kt, int pt, long total, int vec) {
+                           int Cp, int kt, int pt, int dil, long total, int vec) {
   if (vec) {           // one thread = 8 channels: kt 16-byte loads, two 16-byte stores
     const int cvn = C >> 3;
     for (long i = blockIdx.x * 256L + threadIdx.x; i < total; i += (long)gridDim.x * 256) {
@@ -1005,7 +1006,7 @@ time_stack_nhwc_bwd_kernel(const __nv_bfloat16 *__restrict__ g, float *__restric
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] = 0.f;
       for (int dt = 0; dt < kt; ++dt) {
-        const int t = tp + pt - dt;
+        const int t = tp + pt - dt * dil;
         if (t < 0 || t >= T) continue;
         const uint4 q = __ldg(reinterpret_cast<const uint4 *>(g + ((b * T + t) * Fp + f) * Cp + dt * C + cv * 8));
         const __nv_bfloat162 *h = reinterpret_cast<const __nv_bfloat162 *>(&q);
@@ -1031,7 +1032,7 @@ time_stack_nhwc_bwd_kernel(const __nv_bfloat16 *__restrict__ g, float *__restric
     const long b = bt / T;
     float acc = 0.f;
     for (int dt = 0; dt < kt; ++dt) {
-      const int t = tp + pt - dt;
+      const int t = tp + pt - dt * dil;
       if (t >= 0 && t < T) acc += __bfloat162float(g[((b * T + t) * Fp + f) * Cp + dt * C + c]);
     }
     gx[i] = acc;
@@ -1064,34 +1065,56 @@ extern "C" int rave_time_stack_cl_bwd(const void *g_bf16, float *gx, int B, int 
   return 0;
 }
 
-extern "C" int rave_time_stack_nhwc(const float *x, void *out_bf16, int B, int C, int T, int F, long sb, long st, int Fp,
-                                    int Cp, int kt, int pt, void *stream) {
-  using namespace rave;
+namespace rave {
+
+static int time_stack_nhwc_launch(const float *x, void *out_bf16, int B, int C, int T, int F, long sb, long st, int Fp,
+                                  int Cp, int kt, int pt, int dil, cudaStream_t stream) {
   RAVE_CHECK_ARG(x && out_bf16 && B > 0 && C > 0 && T > 0 && F > 0 && Fp >= F && kt >= 1 && Cp >= kt * C &&
-                     Cp % 8 == 0 && ((uintptr_t)out_bf16 & 15) == 0, "time_stack_nhwc: bad shape");
+                     Cp % 8 == 0 && dil >= 1 && ((uintptr_t)out_bf16 & 15) == 0, "time_stack_nhwc: bad shape");
   const int vec = (C % 8 == 0) && ((uintptr_t)x & 15) == 0 && sb % 4 == 0 && st % 4 == 0;
   const long total = (long)B * T * Fp * (Cp / 8);
   long blocks = (total + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
-  time_stack_nhwc_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)out_bf16, sb, st, C, T, F, Fp,
-                                                                        Cp, kt, pt, total, vec);
+  time_stack_nhwc_kernel<<<(int)blocks, 256, 0, stream>>>(x, (__nv_bfloat16 *)out_bf16, sb, st, C, T, F, Fp, Cp, kt, pt,
+                                                         dil, total, vec);
   RAVE_CHECK_LAUNCH("time_stack_nhwc");
   return 0;
 }
 
-extern "C" int rave_time_stack_nhwc_bwd(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp, int kt,
-                                        int pt, void *stream) {
-  using namespace rave;
+static int time_stack_nhwc_bwd_launch(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp, int kt,
+                                      int pt, int dil, cudaStream_t stream) {
   RAVE_CHECK_ARG(g_bf16 && gx && B > 0 && C > 0 && T > 0 && F > 0 && Fp >= F && kt >= 1 && Cp >= kt * C &&
-                     Cp % 8 == 0 && ((uintptr_t)g_bf16 & 15) == 0, "time_stack_nhwc_bwd: bad shape");
+                     Cp % 8 == 0 && dil >= 1 && ((uintptr_t)g_bf16 & 15) == 0, "time_stack_nhwc_bwd: bad shape");
   const int vec = (C % 8 == 0) && ((uintptr_t)gx & 15) == 0;
   const long total = vec ? (long)B * T * F * (C / 8) : (long)B * T * F * C;
   long blocks = (total + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
-  time_stack_nhwc_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>((const __nv_bfloat16 *)g_bf16, gx, C, T, F, Fp,
-                                                                            Cp, kt, pt, total, vec);
+  time_stack_nhwc_bwd_kernel<<<(int)blocks, 256, 0, stream>>>((const __nv_bfloat16 *)g_bf16, gx, C, T, F, Fp, Cp, kt, pt,
+                                                             dil, total, vec);
   RAVE_CHECK_LAUNCH("time_stack_nhwc_bwd");
   return 0;
+}
+
+}  // namespace rave
+
+extern "C" int rave_time_stack_nhwc(const float *x, void *out_bf16, int B, int C, int T, int F, long sb, long st, int Fp,
+                                    int Cp, int kt, int pt, void *stream) {
+  return rave::time_stack_nhwc_launch(x, out_bf16, B, C, T, F, sb, st, Fp, Cp, kt, pt, 1, (cudaStream_t)stream);
+}
+
+extern "C" int rave_time_stack_nhwc_bwd(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp, int kt,
+                                        int pt, void *stream) {
+  return rave::time_stack_nhwc_bwd_launch(g_bf16, gx, B, C, T, F, Fp, Cp, kt, pt, 1, (cudaStream_t)stream);
+}
+
+extern "C" int rave_time_stack_nhwc_dil(const float *x, void *out_bf16, int B, int C, int T, int F, long sb, long st,
+                                        int Fp, int Cp, int kt, int pt, int dil, void *stream) {
+  return rave::time_stack_nhwc_launch(x, out_bf16, B, C, T, F, sb, st, Fp, Cp, kt, pt, dil, (cudaStream_t)stream);
+}
+
+extern "C" int rave_time_stack_nhwc_dil_bwd(const void *g_bf16, float *gx, int B, int C, int T, int F, int Fp, int Cp,
+                                            int kt, int pt, int dil, void *stream) {
+  return rave::time_stack_nhwc_bwd_launch(g_bf16, gx, B, C, T, F, Fp, Cp, kt, pt, dil, (cudaStream_t)stream);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1148,11 +1171,11 @@ leaky_fm_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, float *_
   block_sum_finish(bs, stats);
 }
 
-// The same tap that ALSO writes the next MRD conv's operand (rave_time_stack_nhwc of its own output, kt = 3, pt = 1):
-// x rows are (b, t) pairs [2 Rh][F][C]; xs [2 Rh][Fp][3 C] bf16 with xs[(b, t)][f][dt C + c] = a[b][t + dt - 1][f][c], zero
-// outside the T time steps of a batch entry and in the pad columns f >= F.  The element at time t lands in slot 0 of row
-// t + 1, slot 1 of row t and slot 2 of row t - 1; the threads of the first / last time step and of the last column write
-// the zeros.  Saves the stand-alone time-stack pass (read 4 N, write 6 N bytes per layer, 78 launches per step).
+// The same tap that ALSO writes the next conv's operand (rave_time_stack_nhwc_dil of its own output, kt = 3, pt = dil):
+// x rows are (b, t) pairs [2 Rh][F][C]; xs [2 Rh][Fp][3 C] bf16 with xs[(b, t)][f][dt C + c] = a[b][t + (dt - 1) dil][f][c],
+// zero outside the T time steps of a batch entry and in the pad columns f >= F.  The element at time t lands in slot 0 of
+// row t + dil, slot 1 of row t and slot 2 of row t - dil; the threads of the first / last dil time steps and of the last
+// column write the zeros (dil = 1: the MRD's (3, 9) convs; 2, 4: the dilated EncodecConvNet convs).  Saves the stand-alone time-stack pass (read 4 N, write 6 N bytes per layer, 78 launches per step).
 __device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
   const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
   return make_uint2(*reinterpret_cast<const uint32_t *>(&lo), *reinterpret_cast<const uint32_t *>(&hi));
@@ -1160,7 +1183,7 @@ __device__ __forceinline__ uint2 pack_bf16x4(float4 v) {
 
 __global__ void __launch_bounds__(256)
 leaky_fm_stack_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, float *__restrict__ stats,
-                          __nv_bfloat16 *__restrict__ xs, long Rh, int T, int F, int C, int Fp, float slope,
+                          __nv_bfloat16 *__restrict__ xs, long Rh, int T, int F, int C, int Fp, int dil, float slope,
                           const BlockSum bs) {
   __shared__ float red0[8], red1[8];
   float s0 = 0.f, s1 = 0.f;
@@ -1188,12 +1211,12 @@ leaky_fm_stack_fwd_kernel(const float *__restrict__ x, float *__restrict__ a, fl
       const uint2 pk = pack_bf16x4(h ? fv : rv);
       const long row = r + (h ? Rh : 0);
       __nv_bfloat16 *base = xs + ((size_t)row * Fp + f) * Cp + 4 * c4;         // slot 0 of this (row, f)
-      const size_t row_stride = (size_t)Fp * Cp;
+      const size_t row_stride = (size_t)Fp * Cp * dil;
       *reinterpret_cast<uint2 *>(base + C) = pk;                                    // slot 1 of row t
-      if (t + 1 < T) *reinterpret_cast<uint2 *>(base + row_stride) = pk;            // slot 0 of row t + 1
-      else *reinterpret_cast<uint2 *>(base + 2 * C) = zero2;                        // last step: its slot 2 reads t + 1
-      if (t > 0) *reinterpret_cast<uint2 *>(base - row_stride + 2 * C) = pk;        // slot 2 of row t - 1
-      else *reinterpret_cast<uint2 *>(base) = zero2;                                // first step: its slot 0 reads t - 1
+      if (t + dil < T) *reinterpret_cast<uint2 *>(base + row_stride) = pk;          // slot 0 of row t + dil
+      else *reinterpret_cast<uint2 *>(base + 2 * C) = zero2;                        // last steps: slot 2 reads t + dil
+      if (t >= dil) *reinterpret_cast<uint2 *>(base - row_stride + 2 * C) = pk;     // slot 2 of row t - dil
+      else *reinterpret_cast<uint2 *>(base) = zero2;                                // first steps: slot 0 reads t - dil
       if (f == F - 1) {                                                             // pad columns of this row: zeros
         for (int fp = F; fp < Fp; ++fp) {
           __nv_bfloat16 *pz = base + (size_t)(fp - f) * Cp;
@@ -1257,8 +1280,8 @@ leaky_fm_bwd_kernel(const float *__restrict__ a, const float *__restrict__ g, co
 }
 
 // Backward of leaky_fm_stack_fwd in one pass: the gradient reaching a[(b, t)][f][c] through the stacked operand is
-//   gxs[(b, t + 1)][f][c] + gxs[(b, t)][f][C + c] + gxs[(b, t - 1)][f][2 C + c]      (rows inside the batch entry only)
-// (the adjoint rave_time_stack_nhwc_bwd computes, same summation order), plus `ga` (gradient arriving at the feature
+//   gxs[(b, t + dil)][f][c] + gxs[(b, t)][f][C + c] + gxs[(b, t - dil)][f][2 C + c]  (rows inside the batch entry only)
+// (the adjoint rave_time_stack_nhwc_dil_bwd computes, same summation order), plus `ga` (gradient arriving at the feature
 // itself, or null); the feature-matching terms and LeakyReLU' follow as in leaky_fm_bwd_kernel.
 __device__ __forceinline__ float4 bf16x4_to_f32(uint2 p) {
   return make_float4(__uint_as_float(p.x << 16), __uint_as_float(p.x & 0xFFFF0000u), __uint_as_float(p.y << 16),
@@ -1269,12 +1292,12 @@ __device__ __forceinline__ void add4(float4 &a, const float4 b) { a.x += b.x; a.
 __global__ void __launch_bounds__(256)
 leaky_fm_stack_bwd_kernel(const float *__restrict__ a, const __nv_bfloat16 *__restrict__ gxs, const float *__restrict__ ga,
                           const float *__restrict__ d, float *__restrict__ gx, long Rh, int T, int F, int C, int Fp,
-                          float slope) {
+                          int dil, float slope) {
   const float d0 = d ? d[0] : 0.f, d1 = d ? d[1] : 0.f;
   const int C4 = C >> 2;
   const int Cp = 3 * C;
   const long H4 = Rh * F * C4;
-  const size_t row_stride = (size_t)Fp * Cp;
+  const size_t row_stride = (size_t)Fp * Cp * dil;
   const float4 *ar4 = reinterpret_cast<const float4 *>(a), *af4 = ar4 + H4;
   const float4 *gr4 = reinterpret_cast<const float4 *>(ga), *gf4 = gr4 + H4;
   float4 *or4 = reinterpret_cast<float4 *>(gx), *of4 = or4 + H4;
@@ -1290,9 +1313,9 @@ leaky_fm_stack_bwd_kernel(const float *__restrict__ a, const __nv_bfloat16 *__re
       const long row = r + (h ? Rh : 0);
       const __nv_bfloat16 *base = gxs + ((size_t)row * Fp + f) * Cp + 4 * c4;
       float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (t + 1 < T) add4(acc, bf16x4_to_f32(__ldg(reinterpret_cast<const uint2 *>(base + row_stride))));
+      if (t + dil < T) add4(acc, bf16x4_to_f32(__ldg(reinterpret_cast<const uint2 *>(base + row_stride))));
       add4(acc, bf16x4_to_f32(__ldg(reinterpret_cast<const uint2 *>(base + C))));
-      if (t > 0) add4(acc, bf16x4_to_f32(__ldg(reinterpret_cast<const uint2 *>(base - row_stride + 2 * C))));
+      if (t >= dil) add4(acc, bf16x4_to_f32(__ldg(reinterpret_cast<const uint2 *>(base - row_stride + 2 * C))));
       if (ga) add4(acc, __ldg((h ? gf4 : gr4) + i));
       g2[h] = acc;
     }
@@ -1323,36 +1346,59 @@ extern "C" int rave_leaky_fm_fwd(const float *x, float *a, float *stats, long H,
   return 0;
 }
 
-extern "C" int rave_leaky_fm_stack_fwd(const float *x, float *a, float *stats, void *xs_bf16, long Rh, int T, int F, int C,
-                                       int Fp, float slope, void *stream) {
-  using namespace rave;
+namespace rave {
+
+static int leaky_fm_stack_fwd_launch(const float *x, float *a, float *stats, void *xs_bf16, long Rh, int T, int F, int C,
+                                     int Fp, int dil, float slope, cudaStream_t stream) {
   RAVE_CHECK_ARG(x && a && stats && xs_bf16 && Rh > 0 && T > 0 && Rh % T == 0 && F > 0 && Fp >= F && C > 0 && C % 4 == 0 &&
-                     slope > 0.f && (((uintptr_t)x | (uintptr_t)a) & 15) == 0 && ((uintptr_t)xs_bf16 & 7) == 0,
+                     dil >= 1 && slope > 0.f && (((uintptr_t)x | (uintptr_t)a) & 15) == 0 && ((uintptr_t)xs_bf16 & 7) == 0,
                  "leaky_fm_stack_fwd: bad argument (C %% 4 == 0, rows = whole batch entries of T steps, aligned buffers)");
   long blocks = (Rh * F * (C / 4) + 255) / 256;
   blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
   BlockSum bs;
-  if (int rc = block_sum_begin(&bs, blocks, 2, (cudaStream_t)stream)) return rc;
-  leaky_fm_stack_fwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, a, stats, (__nv_bfloat16 *)xs_bf16, Rh, T, F, C,
-                                                                          Fp, slope, bs);
-  block_sum_end(bs, (cudaStream_t)stream);
+  if (int rc = block_sum_begin(&bs, blocks, 2, stream)) return rc;
+  leaky_fm_stack_fwd_kernel<<<(int)blocks, 256, 0, stream>>>(x, a, stats, (__nv_bfloat16 *)xs_bf16, Rh, T, F, C, Fp, dil,
+                                                            slope, bs);
+  block_sum_end(bs, stream);
   RAVE_CHECK_LAUNCH("leaky_fm_stack_fwd");
   return 0;
 }
 
-extern "C" int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx,
-                                       long Rh, int T, int F, int C, int Fp, float slope, void *stream) {
-  using namespace rave;
+static int leaky_fm_stack_bwd_launch(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx,
+                                     long Rh, int T, int F, int C, int Fp, int dil, float slope, cudaStream_t stream) {
   RAVE_CHECK_ARG(a && gxs_bf16 && gx && Rh > 0 && T > 0 && Rh % T == 0 && F > 0 && Fp >= F && C > 0 && C % 4 == 0 &&
-                     slope > 0.f && (((uintptr_t)a | (uintptr_t)gx | (uintptr_t)ga) & 15) == 0 &&
+                     dil >= 1 && slope > 0.f && (((uintptr_t)a | (uintptr_t)gx | (uintptr_t)ga) & 15) == 0 &&
                      ((uintptr_t)gxs_bf16 & 7) == 0,
                  "leaky_fm_stack_bwd: bad argument (C %% 4 == 0, rows = whole batch entries of T steps, aligned buffers)");
   long blocks = (Rh * F * (C / 4) + 255) / 256;
   blocks = blocks < 1 ? 1 : (blocks > 132 * 8 ? 132 * 8 : blocks);
-  leaky_fm_stack_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(a, (const __nv_bfloat16 *)gxs_bf16, ga, d, gx, Rh,
-                                                                          T, F, C, Fp, slope);
+  leaky_fm_stack_bwd_kernel<<<(int)blocks, 256, 0, stream>>>(a, (const __nv_bfloat16 *)gxs_bf16, ga, d, gx, Rh, T, F, C,
+                                                            Fp, dil, slope);
   RAVE_CHECK_LAUNCH("leaky_fm_stack_bwd");
   return 0;
+}
+
+}  // namespace rave
+
+extern "C" int rave_leaky_fm_stack_fwd(const float *x, float *a, float *stats, void *xs_bf16, long Rh, int T, int F, int C,
+                                       int Fp, float slope, void *stream) {
+  return rave::leaky_fm_stack_fwd_launch(x, a, stats, xs_bf16, Rh, T, F, C, Fp, 1, slope, (cudaStream_t)stream);
+}
+
+extern "C" int rave_leaky_fm_stack_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d, float *gx,
+                                       long Rh, int T, int F, int C, int Fp, float slope, void *stream) {
+  return rave::leaky_fm_stack_bwd_launch(a, gxs_bf16, ga, d, gx, Rh, T, F, C, Fp, 1, slope, (cudaStream_t)stream);
+}
+
+extern "C" int rave_leaky_fm_stack_dil_fwd(const float *x, float *a, float *stats, void *xs_bf16, long Rh, int T, int F,
+                                           int C, int Fp, int dil, float slope, void *stream) {
+  return rave::leaky_fm_stack_fwd_launch(x, a, stats, xs_bf16, Rh, T, F, C, Fp, dil, slope, (cudaStream_t)stream);
+}
+
+extern "C" int rave_leaky_fm_stack_dil_bwd(const float *a, const void *gxs_bf16, const float *ga, const float *d,
+                                           float *gx, long Rh, int T, int F, int C, int Fp, int dil, float slope,
+                                           void *stream) {
+  return rave::leaky_fm_stack_bwd_launch(a, gxs_bf16, ga, d, gx, Rh, T, F, C, Fp, dil, slope, (cudaStream_t)stream);
 }
 
 extern "C" int rave_leaky_fm_bwd(const float *a, const float *g, const float *d, float *gx, long H, float slope,

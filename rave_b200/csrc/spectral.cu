@@ -130,6 +130,40 @@ stft_frames_bwd_kernel(const float *__restrict__ dframes, const float *__restric
   }
 }
 
+// Uncentred framing (torchaudio Spectrogram(center=False, normalized=True) of the multi-scale spectral discriminator,
+// rave/discriminator.py:12-20), F = 1 + (T - n_fft) / hop frames, no padding:
+//   frames[n][f][t] = s * w[t] * x[n][f*hop + t]           s = 1 / ||w||_2 for normalized=True
+// adjoint: dx[n][j] = s * sum over the frames f covering j of w[j - f*hop] * dframes[n][f][j - f*hop] (a gather: one
+// thread per output sample, no atomics); samples past the last frame get zero.
+__global__ void __launch_bounds__(256)
+stft_frames_valid_kernel(const float *__restrict__ x, const float *__restrict__ w, float *__restrict__ frames, long total4,
+                         int T, int n_fft, int hop, int F, float s, int vec_ok) {
+  const int q = n_fft >> 2;                   // float4 per frame
+  const int qs = 31 - __clz(q);
+  for (long i = blockIdx.x * 256L + threadIdx.x; i < total4; i += (long)gridDim.x * 256) {
+    const int t = (int)(i & (q - 1)) << 2;
+    const long nf = i >> qs;
+    const int f = (int)(nf % F);
+    const long n = nf / F;
+    const float *xn = x + n * T + (long)f * hop + t;
+    const float4 ww = __ldg(reinterpret_cast<const float4 *>(w + t));
+    const float4 xv = vec_ok ? __ldg(reinterpret_cast<const float4 *>(xn))
+                             : make_float4(__ldg(xn), __ldg(xn + 1), __ldg(xn + 2), __ldg(xn + 3));
+    reinterpret_cast<float4 *>(frames)[i] =
+        make_float4(s * ww.x * xv.x, s * ww.y * xv.y, s * ww.z * xv.z, s * ww.w * xv.w);
+  }
+}
+
+__global__ void __launch_bounds__(256)
+stft_frames_valid_bwd_kernel(const float *__restrict__ dframes, const float *__restrict__ w, float *__restrict__ dx,
+                             long total, int T, int n_fft, int hop, int F, float s) {
+  for (long i = blockIdx.x * 256L + threadIdx.x; i < total; i += (long)gridDim.x * 256) {
+    const int j = (int)(i % T);
+    const long n = i / T;
+    dx[i] = s * stft_ola_at(dframes + (size_t)n * F * n_fft, w, j, n_fft, hop, F);
+  }
+}
+
 // Gradient of y = rfft(x) (last axis, length n) as the input of ONE c2r transform: Z[k] = G[k] * n * (k == 0 || k == n/2
 // ? 1 : 1/2), imaginary parts of the DC and Nyquist bins dropped (cuFFT's C2R result is unspecified for a non-Hermitian
 // input; those parts carry no gradient).  dx = irfft(Z, n).  G: [N][F][bins] complex64 with arbitrary strides.
@@ -190,6 +224,37 @@ extern "C" int rave_stft_frames_bwd(const float *dframes, const float *window, f
   if (blocks > 132 * 16) blocks = 132 * 16;
   stft_frames_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(dframes, window, dx, total, T, n_fft, hop, F);
   RAVE_CHECK_LAUNCH("stft_frames_bwd");
+  return 0;
+}
+
+extern "C" int rave_stft_frames_valid(const float *x, const float *window, float *frames, int N, int T, int n_fft, int hop,
+                                      float scale, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(x && window && frames && N > 0 && T >= n_fft && n_fft >= 16 && (n_fft & (n_fft - 1)) == 0 && hop > 0,
+                 "stft_frames_valid: bad argument (T >= n_fft, n_fft a power of two >= 16)");
+  const int F = 1 + (T - n_fft) / hop;
+  const long total4 = (long)N * F * (n_fft / 4);
+  long blocks = (total4 + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  const int vec_ok = (T % 4 == 0) && (hop % 4 == 0) && (((uintptr_t)x & 15) == 0);
+  stft_frames_valid_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(x, window, frames, total4, T, n_fft, hop, F,
+                                                                          scale, vec_ok);
+  RAVE_CHECK_LAUNCH("stft_frames_valid");
+  return 0;
+}
+
+extern "C" int rave_stft_frames_valid_bwd(const float *dframes, const float *window, float *dx, int N, int T, int n_fft,
+                                          int hop, float scale, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(dframes && window && dx && N > 0 && T >= n_fft && n_fft >= 16 && hop > 0,
+                 "stft_frames_valid_bwd: bad argument");
+  const int F = 1 + (T - n_fft) / hop;
+  const long total = (long)N * T;
+  long blocks = (total + 255) / 256;
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  stft_frames_valid_bwd_kernel<<<(int)blocks, 256, 0, (cudaStream_t)stream>>>(dframes, window, dx, total, T, n_fft, hop,
+                                                                              F, scale);
+  RAVE_CHECK_LAUNCH("stft_frames_valid_bwd");
   return 0;
 }
 

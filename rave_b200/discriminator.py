@@ -287,3 +287,253 @@ class CombineDiscriminators(nn.Module):
                 if torch.is_tensor(t):
                     t.record_stream(cur)
         return out
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Multi-scale spectral discriminator (rave/discriminator.py:12-74, 139-153; configs/spectral_discriminator.gin): one
+# EncodecConvNet of weight-normed 2-D convs over the complex STFT [B, (re | im) x C, F, T] of each scale.  A (kf, kt)
+# conv with unit time stride is ONE library conv1d along frequency over rows (b, t) whose channels are the kt time-
+# shifted copies (by multiples of the time dilation) of the input channels (`SpectralConv2d`).  In bf16 mode each scale
+# runs channel-last from end to end on the wgmma engine, like the Descript MRD.
+# ---------------------------------------------------------------------------------------------------------------------
+
+class _Spectrogram(nn.Module):
+    """torchaudio.transforms.Spectrogram(n_fft, hop_length=n_fft // 4, power=None, normalized=True, center=False) of the
+    reference: its only state_dict entry is the hann `window`.  On CUDA tensors the framing is a library kernel
+    (no padding, scaled by 1 / ||window||_2) and cuFFT transforms; returns the complex [B, C, F, T]."""
+
+    def __init__(self, n_fft: int):
+        super().__init__()
+        self.n_fft, self.hop = n_fft, n_fft // 4
+        window = torch.hann_window(n_fft)
+        self.register_buffer("window", window)
+        self.scale = float(1.0 / window.pow(2.).sum().sqrt())
+        bw = torch.full((n_fft // 2 + 1,), 0.5 * n_fft)
+        bw[0] = n_fft
+        bw[-1] = n_fft
+        self.register_buffer("rfft_bw", bw, persistent=False)
+
+    def frames_spectrum(self, x):
+        """x [N, T] CUDA -> complex [N, frames, bins]: the channel-last (time, frequency) layout of the engine path."""
+        return ops.rfft(ops.stft_frames_valid(x, self.window, self.n_fft, self.hop, self.scale), self.rfft_bw)
+
+    def forward(self, x):
+        B, C, T = x.shape
+        if x.is_cuda:
+            z = self.frames_spectrum(x.reshape(B * C, T)).transpose(-1, -2)
+        else:
+            z = torch.stft(x.reshape(B * C, T), self.n_fft, hop_length=self.hop, win_length=self.n_fft,
+                           window=self.window, center=False, normalized=False, onesided=True,
+                           return_complex=True) * self.scale
+        return z.reshape(B, C, z.shape[-2], z.shape[-1])
+
+
+def spectrogram(n_fft: int):
+    """rave/discriminator.py:12-20."""
+    return _Spectrogram(n_fft)
+
+
+class SpectralConv2d(nn.Conv2d):
+    """nn.Conv2d with kernel (kf, kt), stride (sf, 1), dilation (1, dt), padding (pf, dt (kt - 1) / 2) on [B, C, F, T]
+    tensors, on the library's conv1d kernels: the kt time taps (time t + j dt - pt for tap j) become kt x Cin input
+    channels of a conv along frequency over rows (b, t).  Same parameters / state_dict keys as nn.Conv2d."""
+
+    def __init__(self, *args, **kwargs):
+        super().__init__(*args, **kwargs)
+        kt, dt = self.kernel_size[1], self.dilation[1]
+        if self.stride[1] != 1 or self.dilation[0] != 1 or self.groups != 1 or self.padding_mode != "zeros" \
+                or 2 * self.padding[1] != dt * (kt - 1):
+            raise RaveB200Error("SpectralConv2d: unit time stride, 'same' time padding, no groups / frequency dilation")
+
+    def forward(self, x):
+        B, C, Fq, T = x.shape
+        kf, kt = self.kernel_size
+        pf, pt = self.padding
+        dt = self.dilation[1]
+        if self.tc_ready(x):
+            out = self.forward_cl(x.permute(0, 3, 2, 1))
+            return out[..., :self.out_channels].reshape(B, T, out.shape[1], self.out_channels).permute(0, 3, 2, 1)
+        xp = nn.functional.pad(x, (pt, pt))
+        xi = torch.stack([xp[..., j * dt:j * dt + T] for j in range(kt)], 1)          # [B, kt, C, F, T]
+        xi = xi.permute(0, 4, 1, 2, 3).reshape(B * T, kt * C, Fq)                      # rows (b, t), channels (j, c)
+        w = self.weight.permute(0, 3, 1, 2).reshape(self.out_channels, kt * C, kf)
+        y = ops.conv1d(xi, w, self.bias, None, self.stride[0], 1, (pf, pf), ops.ACT_NONE, 0.0, None)
+        return y.view(B, T, self.out_channels, y.shape[-1]).permute(0, 2, 3, 1)
+
+    def tc_ready(self, x) -> bool:
+        from . import engine
+        return engine.precision() == "bf16" and x.is_cuda and engine.ACT_DTYPE == torch.bfloat16
+
+    def cout_ok(self) -> bool:
+        return self.out_channels % 16 == 0
+
+    def _tc_chain_spec(self, C):
+        """One-layer engine chain of this conv along frequency; the (j, c) channel order is a permuted VIEW of the
+        parameter, so the weight-norm backward of the chain reaches weight_v / weight_g through autograd."""
+        from . import engine
+        from .descript_discriminator import _ParamView
+        kf, kt = self.kernel_size
+        pf = self.padding[0]
+        cin = kt * C
+        proxy = self.__dict__.get("_tc_proxy")
+        if proxy is None:
+            proxy = self.__dict__["_tc_proxy"] = _ParamView()
+            if self.__dict__.get("_tc_proxy_static"):       # engine.enable_static_prep ran before the first forward
+                proxy.__dict__["_tc_static"] = {}
+            spec = engine.LayerSpec("conv", proxy, cin, self.out_channels, kf, self.stride[0], 1, (pf, pf),
+                                    ops.ACT_NONE, 0.0, None, True, True)
+            spec.cin_pad = (-cin) % 16
+            spec.cout_pad = (-self.out_channels) % 16
+            self.__dict__["_tc_spec"] = spec
+        spec = self.__dict__["_tc_spec"]
+        if spec.Cin != cin:
+            raise RaveB200Error(f"SpectralConv2d: planned for {spec.Cin // kt} input channels, called with {C}")
+        self._tc_refresh_proxy()
+        return spec
+
+    def _tc_refresh_proxy(self):
+        """(Re)build the proxy's (j, c)-ordered copies of the parameters (engine.refresh_static_prep calls this once the
+        parameters moved, before it rewrites the static layouts)."""
+        proxy = self.__dict__["_tc_proxy"]
+        kf = self.kernel_size[0]
+        co = self.out_channels
+        cin = self.__dict__["_tc_spec"].Cin
+        if hasattr(self, "weight_v"):
+            proxy.weight_v = self.weight_v.permute(0, 3, 1, 2).reshape(co, cin, kf)
+            proxy.weight_g = self.weight_g.reshape(co, 1, 1)
+        else:
+            proxy.weight = self.weight.permute(0, 3, 1, 2).reshape(co, cin, kf)
+        proxy.bias = self.bias
+
+    def stacked_geometry(self, Fq: int, C: int):
+        """(Fp, Cp) of this conv's time-stacked operand for an input of Fq positions and C channels."""
+        spec = self._tc_chain_spec(C)
+        return Fq + (-Fq) % spec.stride, self.kernel_size[1] * C + spec.cin_pad
+
+    def forward_cl(self, x_cl, xs=None):
+        """Channel-last in, channel-last out: x_cl [B, T, F, C] fp32 (dense (f, c) rows) -> the chain's own output buffer
+        [(b t), Fo, Cout(+pad to 16)] fp32, which IS [B, T, Fo, Cout] channel-last.  `xs`: the time-stacked bf16
+        operand when the producer already wrote it (ops.leaky_fm_stack of the previous layer's feature tap)."""
+        from . import engine
+        B, T, Fq, C = x_cl.shape
+        spec = self._tc_chain_spec(C)
+        kt, pt, dt = self.kernel_size[1], self.padding[1], self.dilation[1]
+        Fp, Cp = self.stacked_geometry(Fq, C)
+        if xs is None:
+            xs = ops.time_stack_nhwc(x_cl, kt, pt, Cp, Fp, dt)
+        elif tuple(xs.shape) != (B * T, Fp, Cp) or xs.dtype != engine.ACT_DTYPE:
+            raise RaveB200Error("SpectralConv2d.forward_cl: the pre-stacked operand does not match this conv's geometry")
+        (out,) = engine.run_chain(xs, [spec], Fq)
+        if out.shape[1] != engine.chain_lengths([spec], Fq)[0]:
+            raise RaveB200Error("SpectralConv2d: the one-layer chain's output pitch is its length")
+        return out
+
+
+def rectified_2d_conv_block(capacity, kernel_sizes, strides=None, dilations=None, in_size=None, out_size=None,
+                            activation: bool = True):
+    """rave/discriminator.py:23-51 (weight norm through blocks.normalization, configs/v1.gin:41)."""
+    if dilations is None:
+        paddings = kernel_sizes[0] // 2, kernel_sizes[1] // 2
+    else:
+        fks = (kernel_sizes[0] - 1) * dilations[0], (kernel_sizes[1] - 1) * dilations[1]
+        paddings = fks[0] // 2, fks[1] // 2
+    conv = normalization(SpectralConv2d(in_size or capacity, out_size or capacity, kernel_size=kernel_sizes,
+                                        stride=strides or (1, 1), dilation=dilations or (1, 1), padding=paddings))
+    if not activation:
+        return conv
+    return nn.Sequential(conv, nn.LeakyReLU(.2))
+
+
+def _tap_stack(out, slope, B, T, nxt):
+    """Post-activation feature tap of a chain output (descript_discriminator._feature_tap) that also writes the
+    time-stacked operand of the next conv `nxt` in the same pass when the geometry allows it (kt = 3, pt = its time
+    dilation, no channel padding on either side): returns (a, stats, xs | None)."""
+    from .descript_discriminator import _feature_tap
+    C = out.shape[2]
+    if (nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous()
+            and nxt.kernel_size[1] == 3 and nxt.padding[1] == nxt.dilation[1] and nxt.in_channels == C and C % 4 == 0
+            and out.shape[0] == B * T):
+        Fp, Cp = nxt.stacked_geometry(out.shape[1], C)
+        if Cp == 3 * C:
+            return ops.leaky_fm_stack(out, slope, T, Fp, nxt.dilation[1])
+    a, st = _feature_tap(out, slope, B)
+    return a, st, None
+
+
+class EncodecConvNet(nn.Module):
+    """rave/discriminator.py:54-74.  Features are the POST-activation output of every block, the last one (no
+    activation) is the score."""
+
+    def __init__(self, capacity: int, n_channels: int = 1) -> None:
+        super().__init__()
+        self.net = nn.Sequential(
+            rectified_2d_conv_block(capacity, (9, 3), in_size=2 * n_channels),
+            rectified_2d_conv_block(capacity, (9, 3), (2, 1), (1, 1)),
+            rectified_2d_conv_block(capacity, (9, 3), (2, 1), (1, 2)),
+            rectified_2d_conv_block(capacity, (9, 3), (2, 1), (1, 4)),
+            rectified_2d_conv_block(capacity, (3, 3)),
+            rectified_2d_conv_block(capacity, (3, 3), out_size=1, activation=False),
+        )
+
+    def convs(self):
+        return [layer[0] if isinstance(layer, nn.Sequential) else layer for layer in self.net]
+
+    def forward(self, x):
+        features = []
+        for layer in self.net:
+            if isinstance(layer, nn.Sequential):
+                h = layer[0](x)
+                x = ops.activation(h.contiguous(), ops.ACT_LEAKY, layer[1].negative_slope)
+            else:
+                x = layer(x)
+            features.append(x)
+        return features
+
+    def forward_cl(self, x0):
+        """bf16 engine mode: x0 = view_as_real(spectrum) [B, T, F, 2] is already the channel-last input of the first
+        conv; every conv's output buffer passes through the feature tap, which also writes the next conv's operand.
+        Features are NCHW views [B, C, F, T] of the tapped buffers, carrying `_cl_base` / `_fm_stats`."""
+        B, T = x0.shape[0], x0.shape[1]
+        convs = self.convs()
+        fmap = []
+        cur, xs = x0, None
+        for i, (layer, conv) in enumerate(zip(self.net, convs)):
+            out = conv.forward_cl(cur, xs)                                 # [(b t), Fo, Cout(+pad)]
+            Fo = out.shape[1]
+            if isinstance(layer, nn.Sequential):
+                nxt = convs[i + 1] if i + 1 < len(convs) else None
+                a, st, xs = _tap_stack(out, layer[1].negative_slope, B, T, nxt)
+                cur = a.view(B, T, Fo, out.shape[2])
+                feat = cur.permute(0, 3, 2, 1)
+                feat._cl_base = a
+                feat._fm_stats = st
+            else:
+                feat = out.view(B, T, Fo, out.shape[2])[..., :conv.out_channels].permute(0, 3, 2, 1)
+            fmap.append(feat)
+        return fmap
+
+
+class MultiScaleSpectralDiscriminator(nn.Module):
+    """rave/discriminator.py:139-153."""
+
+    def __init__(self, scales: Sequence[int], convnet: Callable[..., nn.Module], n_channels: int = 1) -> None:
+        super().__init__()
+        self.specs = nn.ModuleList([spectrogram(n) for n in scales])
+        self.nets = nn.ModuleList([convnet(n_channels=n_channels) for _ in scales])
+
+    def engine_ready(self, x) -> bool:
+        """bf16 engine path: mono CUDA input, 16-aligned widths, at least one frame at every scale."""
+        first = [net.convs()[0] for net in self.nets]
+        return (x.dim() == 3 and x.shape[1] == 1 and all(c.tc_ready(x) and c.cout_ok() for c in first)
+                and x.shape[-1] >= max(s.n_fft for s in self.specs))
+
+    def forward(self, x):
+        features = []
+        if self.engine_ready(x):
+            for spec, net in zip(self.specs, self.nets):
+                features.append(net.forward_cl(torch.view_as_real(spec.frames_spectrum(x[:, 0]))))
+            return features
+        for spec, net in zip(self.specs, self.nets):
+            spec_x = spec(x)
+            features.append(net(torch.cat([spec_x.real, spec_x.imag], 1)))
+        return features

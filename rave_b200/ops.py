@@ -506,10 +506,11 @@ def time_stack_cl(x, kt, pt, Cp, Fp):
 
 class TimeStackNhwcFn(torch.autograd.Function):
     """x [B, T, F, C] fp32 channel-last (any batch / time strides, channels and positions dense) -> the same
-    [(b t), Fp, Cp] bf16 operand (rave_time_stack_nhwc); backward = the adjoint into a contiguous [B, T, F, C]."""
+    [(b t), Fp, Cp] bf16 operand, tap dt reading time t + dt * dil - pt (rave_time_stack_nhwc_dil); backward = the
+    adjoint into a contiguous [B, T, F, C]."""
 
     @staticmethod
-    def forward(ctx, x, kt, pt, Cp, Fp):
+    def forward(ctx, x, kt, pt, Cp, Fp, dil):
         if x.dtype != torch.float32:
             x = x.float()
         B, T, F_, C = x.shape
@@ -518,22 +519,22 @@ class TimeStackNhwcFn(torch.autograd.Function):
         out = torch.empty(B * T, Fp, Cp, dtype=torch.bfloat16, device=x.device)
         if not x.is_cuda:
             raise _lib.RaveB200Error("rave_b200 ops need CUDA tensors (there is no CPU path)")
-        call("rave_time_stack_nhwc", x.data_ptr(), ptr(out), B, C, T, F_, x.stride(0), x.stride(1), Fp, Cp, kt, pt,
-             stream_ptr())          # x: a strided view (band slice of the spectrogram / rows of the previous output)
-        ctx.cfg = (B, C, T, F_, Fp, Cp, kt, pt)
+        call("rave_time_stack_nhwc_dil", x.data_ptr(), ptr(out), B, C, T, F_, x.stride(0), x.stride(1), Fp, Cp, kt, pt,
+             dil, stream_ptr())     # x: a strided view (band slice of the spectrogram / rows of the previous output)
+        ctx.cfg = (B, C, T, F_, Fp, Cp, kt, pt, dil)
         return out
 
     @staticmethod
     def backward(ctx, g):
-        B, C, T, F_, Fp, Cp, kt, pt = ctx.cfg
+        B, C, T, F_, Fp, Cp, kt, pt, dil = ctx.cfg
         g = g.contiguous()
         gx = torch.empty(B, T, F_, C, dtype=torch.float32, device=g.device)
-        call("rave_time_stack_nhwc_bwd", ptr(g), ptr(gx), B, C, T, F_, Fp, Cp, kt, pt, stream_ptr())
-        return gx, None, None, None, None
+        call("rave_time_stack_nhwc_dil_bwd", ptr(g), ptr(gx), B, C, T, F_, Fp, Cp, kt, pt, dil, stream_ptr())
+        return gx, None, None, None, None, None
 
 
-def time_stack_nhwc(x, kt, pt, Cp, Fp):
-    return TimeStackNhwcFn.apply(x, kt, pt, Cp, Fp)
+def time_stack_nhwc(x, kt, pt, Cp, Fp, dil=1):
+    return TimeStackNhwcFn.apply(x, kt, pt, Cp, Fp, dil)
 
 
 class L1HalvesFn(torch.autograd.Function):
@@ -603,14 +604,14 @@ def leaky_fm(x, slope):
 
 
 class LeakyFmStackFn(torch.autograd.Function):
-    """LeakyFmFn that also writes the NEXT MRD conv's operand in the same pass: x [(b t), F, C] fp32 with whole batch
+    """LeakyFmFn that also writes the NEXT conv's operand in the same pass: x [(b t), F, C] fp32 with whole batch
     entries of T steps (first half of the rows real) -> (a, stats, xs) with xs [(b t), Fp, 3 C] bf16 =
-    time_stack_nhwc(a.view(B, T, F, C), kt = 3, pt = 1) (rave_leaky_fm_stack_fwd).  The backward is the composition of the
-    two stand-alone backward kernels (adjoint of the time stack, then the tap's fused backward) in ONE kernel
-    (rave_leaky_fm_stack_bwd)."""
+    time_stack_nhwc(a.view(B, T, F, C), kt = 3, pt = dil, dil) (rave_leaky_fm_stack_dil_fwd; dil = 1 for the MRD, 1 / 2 / 4
+    along the EncodecConvNet).  The backward is the composition of the two stand-alone backward kernels (adjoint of the
+    time stack, then the tap's fused backward) in ONE kernel (rave_leaky_fm_stack_dil_bwd)."""
 
     @staticmethod
-    def forward(ctx, x, slope, T, Fp):
+    def forward(ctx, x, slope, T, Fp, dil):
         if x.dtype != torch.float32 or not x.is_contiguous() or x.dim() != 3 or x.shape[0] % (2 * T) or x.shape[2] % 4:
             raise _lib.RaveB200Error("leaky_fm_stack: contiguous fp32 [(b t), F, C] rows, even batch, C % 4 == 0 expected")
         R2, F_, C = x.shape
@@ -618,33 +619,33 @@ class LeakyFmStackFn(torch.autograd.Function):
         a = torch.empty_like(x)
         stats = torch.zeros(2, dtype=torch.float32, device=x.device)
         xs = torch.empty(R2, Fp, 3 * C, dtype=torch.bfloat16, device=x.device)
-        call("rave_leaky_fm_stack_fwd", ptr(x), ptr(a), ptr(stats), ptr(xs), R2 // 2, T, F_, C, Fp, float(slope),
-             stream_ptr())
+        call("rave_leaky_fm_stack_dil_fwd", ptr(x), ptr(a), ptr(stats), ptr(xs), R2 // 2, T, F_, C, Fp, dil,
+             float(slope), stream_ptr())
         ctx.save_for_backward(a)
         ctx.slope = float(slope)
-        ctx.cfg = (C, T, F_, Fp)
+        ctx.cfg = (C, T, F_, Fp, dil)
         return a, stats, xs
 
     @staticmethod
     def backward(ctx, ga, dstats, gxs):
         (a,) = ctx.saved_tensors
         if ga is None and dstats is None and gxs is None:
-            return None, None, None, None
-        C, T, F_, Fp = ctx.cfg
+            return None, None, None, None, None
+        C, T, F_, Fp, dil = ctx.cfg
         ga, dstats = _f32c(ga), _f32c(dstats)
         gx = torch.empty_like(a)
         if gxs is not None:
             # one pass: adjoint of the time stack + gradient at the feature + feature-matching terms + LeakyReLU'
             gxs = gxs.contiguous()
-            call("rave_leaky_fm_stack_bwd", ptr(a), ptr(gxs), ptr(ga), ptr(dstats), ptr(gx), a.shape[0] // 2, T, F_, C, Fp,
-                 ctx.slope, stream_ptr())
+            call("rave_leaky_fm_stack_dil_bwd", ptr(a), ptr(gxs), ptr(ga), ptr(dstats), ptr(gx), a.shape[0] // 2, T, F_, C,
+                 Fp, dil, ctx.slope, stream_ptr())
         else:
             call("rave_leaky_fm_bwd", ptr(a), ptr(ga), ptr(dstats), ptr(gx), a.numel() // 2, ctx.slope, stream_ptr())
-        return gx, None, None, None
+        return gx, None, None, None, None
 
 
-def leaky_fm_stack(x, slope, T, Fp):
-    return LeakyFmStackFn.apply(x, slope, T, Fp)
+def leaky_fm_stack(x, slope, T, Fp, dil=1):
+    return LeakyFmStackFn.apply(x, slope, T, Fp, dil)
 
 
 class L1StatsFn(torch.autograd.Function):
@@ -964,6 +965,35 @@ class StftFramesFn(torch.autograd.Function):
 
 def stft_frames(x, window, n_fft, hop):
     return StftFramesFn.apply(x, window, n_fft, hop)
+
+
+class StftFramesValidFn(torch.autograd.Function):
+    """Uncentred frames [N, F, n_fft] = scale * window * x[f*hop : f*hop + n_fft], F = 1 + (T - n_fft) // hop (torch.stft's
+    framing with center=False; scale = 1 / ||window||_2 gives torchaudio's normalized=True)."""
+
+    @staticmethod
+    def forward(ctx, x, window, n_fft, hop, scale):
+        x = _f32c(x)
+        N, T = x.shape
+        F = 1 + (T - n_fft) // hop
+        frames = torch.empty(N, F, n_fft, dtype=torch.float32, device=x.device)
+        call("rave_stft_frames_valid", ptr(x), ptr(window), ptr(frames), N, T, n_fft, hop, float(scale), stream_ptr())
+        ctx.save_for_backward(window)
+        ctx.dims = (N, T, n_fft, hop, float(scale))
+        return frames
+
+    @staticmethod
+    def backward(ctx, g):
+        (window,) = ctx.saved_tensors
+        N, T, n_fft, hop, scale = ctx.dims
+        g = _f32c(g)
+        dx = torch.empty(N, T, dtype=torch.float32, device=g.device)
+        call("rave_stft_frames_valid_bwd", ptr(g), ptr(window), ptr(dx), N, T, n_fft, hop, scale, stream_ptr())
+        return dx, None, None, None, None
+
+
+def stft_frames_valid(x, window, n_fft, hop, scale):
+    return StftFramesValidFn.apply(x, window, n_fft, hop, scale)
 
 
 class RfftFn(torch.autograd.Function):
