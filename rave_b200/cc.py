@@ -228,8 +228,10 @@ class CachedSequential(nn.Sequential):
             if specs is not None and (specs[0].kind != "conv" or x.shape[-1] % specs[0].stride == 0):
                 (out,) = engine.run_chain(engine.to_channel_last(x, x3=x3), specs, x3=x3)
                 Lout = engine.chain_lengths(specs, x.shape[-1])[-1]
-                if out.shape[1] != Lout:
-                    out = out[:, :Lout].contiguous()
+                Cout = specs[-1].Cout
+                if out.shape[1] != Lout or out.shape[2] != Cout:
+                    # slack rows / zero-padded output channels (their gradient is zero-extended by the slice)
+                    out = out[:, :Lout, :Cout].contiguous()
                 return engine.from_channel_last(out)
         mods = list(self)
         i = 0

@@ -30,6 +30,13 @@ ARCH = {
     # `--config v2 --config spectral_discriminator`: v2 with the MPD replaced by the multi-scale spectral discriminator
     "v2_spectral": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False,
                         disc="v2_spectral", update_discriminator_every=4, phase_1_duration=1000000),
+    # v2_nopqmf.gin on top of v1.gin: the generator writes the waveform itself (output_mode "raw", v2_nopqmf.gin:106;
+    # GeneratorV2.data_size unbound -> 64 -> 2 output conv with amplitude modulation, v2_nopqmf.gin:58-64) with its own
+    # ratios [8, 8, 8, 4] (v2_nopqmf.gin:60); the encoder keeps its PQMF input and ratios [4, 4, 4, 2] (v2_nopqmf.gin:45-52);
+    # CombineDiscriminators[MPD, MSD] at CAPACITY = 64 (v2_nopqmf.gin:22, 84-89; v1.gin:75-88)
+    "v2_nopqmf": dict(capacity=64, ratios=[4, 4, 4, 2], gen_ratios=[8, 8, 8, 4], raw_output=True,   # v2_nopqmf.gin:15-23
+                      activation="leaky", adain=False, disc="v2",
+                      update_discriminator_every=4, phase_1_duration=1000000),              # v2_nopqmf.gin:95-106
 }
 
 
@@ -40,11 +47,15 @@ def _activation_factory(kind):
 
 
 def make_autoencoder(name="v2", capacity=None, latent_size=128, n_band=16, n_channels=1,
-                     padding_mode="centered", ratios=None, activation=None, adain=None, with_noise=False):
-    """(pqmf, encoder, decoder) factories -> constructed modules for one architecture."""
+                     padding_mode="centered", ratios=None, activation=None, adain=None, with_noise=False,
+                     gen_ratios=None):
+    """(pqmf, encoder, decoder) factories -> constructed modules for one architecture.  `gen_ratios`: the generator's
+    own ratios (v2_nopqmf; defaults to the configuration's, else `ratios`)."""
     a = ARCH[name]
     capacity = capacity or a["capacity"]
     ratios = ratios or a["ratios"]
+    gen_ratios = gen_ratios or a.get("gen_ratios") or ratios
+    raw = a.get("raw_output", False)
     act = _activation_factory(activation or a["activation"])
     use_adain = a["adain"] if adain is None else adain
     adain_f = (lambda dim: blocks.AdaptiveInstanceNormalization(dim)) if use_adain else None
@@ -59,7 +70,7 @@ def make_autoencoder(name="v2", capacity=None, latent_size=128, n_band=16, n_cha
         if name == "v2_small" and with_noise:                                  # v2_small.gin:42-57
             noise = partial(blocks.NoiseGeneratorV2, hidden_size=64, data_size=n_band, ratios=[2, 2, 2],
                             noise_bands=32, activation=act)
-        dec = blocks.GeneratorV2(data_size=n_band, capacity=capacity, ratios=ratios,  # v2.gin:43-50
+        dec = blocks.GeneratorV2(data_size=None if raw else n_band, capacity=capacity, ratios=gen_ratios,  # v2.gin:43-50
                                  latent_size=latent_size, kernel_size=3, dilations=V2_DILATIONS,
                                  amplitude_modulation=True, activation=act, adain=adain_f,
                                  n_channels=n_channels, noise_module=noise)
@@ -100,6 +111,8 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
     act = _activation_factory(a["activation"])
     adain_f = (lambda dim: blocks.AdaptiveInstanceNormalization(dim)) if a["adain"] else None
     rat = ratios or a["ratios"]
+    gen_rat = a.get("gen_ratios") or rat
+    raw = a.get("raw_output", False)
     stft = partial(core.MultiScaleSTFT, scales=[2048, 1024, 512, 256, 128],        # v1.gin:21-28
                    sample_rate=sampling_rate, magnitude=True)
     distance = partial(core.AudioDistanceV1, multiscale_stft=stft, log_epsilon=a.get("log_epsilon", 1e-7))
@@ -133,7 +146,7 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
             latent_size=latent_size, sampling_rate=sampling_rate,
             pqmf=partial(pqmf.CachedPQMF, attenuation=100, n_band=16),
             encoder=encoder,
-            decoder=partial(blocks.GeneratorV2, data_size=16, capacity=cap, ratios=rat,
+            decoder=partial(blocks.GeneratorV2, data_size=None if raw else 16, capacity=cap, ratios=gen_rat,
                             latent_size=core.get_augmented_latent_size(latent_size, noise_aug), kernel_size=3,
                             dilations=V2_DILATIONS, amplitude_modulation=True, activation=act, adain=adain_f,
                             noise_module=noise),
@@ -144,5 +157,6 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
             num_skipped_features=a.get("num_skipped_features", 1),
             audio_distance=distance, multiband_audio_distance=distance,
             weights={"feature_matching": 20},                                 # v2.gin:87-89
-            update_discriminator_every=a["update_discriminator_every"], n_channels=n_channels)
+            update_discriminator_every=a["update_discriminator_every"], n_channels=n_channels,
+            output_mode="raw" if raw else "pqmf")
     return model

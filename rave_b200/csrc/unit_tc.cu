@@ -15,8 +15,9 @@
 //   epilogue2 acc + skip -> out (bf16 operand of the next layer and / or the fp32 stream); the skip h = x is
 //             recovered from the unit's own input operand a = LeakyReLU(x) (inverse LeakyReLU), as conv_tc.cu does
 //
-// The channels run in N chunks of NC = 96 (the accumulators of a 128 x NC chunk are NC registers per MMA thread); the
-// 128 x C bf16 A2 tile stays resident (96 KB at C = 384).  A finished chunk goes to a shared-memory buffer that the
+// The channels run in N chunks of NC columns (the accumulators of a 128 x NC chunk are NC registers per MMA thread):
+// NC = 96 at C = 96 / 192 / 384, NC = 64 at C = 64 / 128 / 256 (see unit_chunk); the 128 x C bf16 A2 tile stays
+// resident (96 KB at C = 384).  A finished chunk goes to a shared-memory buffer that the
 // epilogue reads while the warpgroup computes the next chunk -- except at the phase-1 -> phase-2 boundary of a tile,
 // where phase 2 needs the complete A2.
 // Algorithmic HBM bytes per unit: 2 B*L*C (operand in) + 2 B*L*C (operand out) [+ 2 B*L*C a1 when training] + 8 C^2
@@ -51,9 +52,9 @@ struct UnitParams {
   __nv_bfloat16 *out_act;      // [B][pitch][C] or null
 };
 
-template <int C, int BK>
+template <int C, int BK, int NCHUNK>
 struct UnitCfg {
-  static constexpr int NC = 96;                               // N chunk: NC accumulator registers per MMA thread
+  static constexpr int NC = NCHUNK;                           // N chunk: NC accumulator registers per MMA thread
   static constexpr int NCH = C / NC;
   static constexpr int KB = C / BK;                           // K blocks per tap
   static constexpr int SWZ = BK * 2;
@@ -63,7 +64,9 @@ struct UnitCfg {
   static constexpr int STAGE_BYTES = A_BYTES + B_PAD;
   static constexpr int A2_SLAB = 128 * BK * 2;
   static constexpr int A2_BYTES = KB * A2_SLAB;               // the whole [128 x C] bf16 tile
-  static constexpr int ACC_LD = acc_pitch(NC);
+  // one pitch for every instance (the 96-column one also for 64-column chunks: same banks, 100 = 4 mod 32): the
+  // translation unit then binds a single value to acc_bind's pitch, and the compiler folds it into the acc_ld addresses
+  static constexpr int ACC_LD = acc_pitch(96);
   static constexpr int ACC_BYTES = 128 * ACC_LD * 4;          // fp32 accumulator hand-over buffer
   static constexpr int MAX_STAGES = (U_SMEM_MAX - 256 - 1024 - A2_BYTES - ACC_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
@@ -72,17 +75,17 @@ struct UnitCfg {
   static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
   static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;
   static_assert(STAGES >= 2, "not enough shared memory for a 2-stage pipeline");
-  static_assert(NC % 32 == 0 && C % NC == 0, "chunk must be a multiple of 32 columns and tile C");
+  static_assert(NC % 32 == 0 && NC <= 96 && C % NC == 0, "chunk must be a multiple of 32 columns and tile C");
 };
 
 __device__ __forceinline__ float bfl(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bfh(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
 
-template <int C, int BK>
+template <int C, int BK, int NCHUNK>
 __global__ void __launch_bounds__(U_THREADS, 1)
 dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w3,
                        const __grid_constant__ CUtensorMap tmap_w1, const UnitParams p) {
-  using L = UnitCfg<C, BK>;
+  using L = UnitCfg<C, BK, NCHUNK>;
   constexpr int STAGES = L::STAGES, NC = L::NC, NCH = L::NCH, KB = L::KB, SWZ = L::SWZ;
 
   extern __shared__ uint8_t smem_raw[];
@@ -331,7 +334,8 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 }
 
 // =============================================================================================
-// Weight-stationary variant for the narrow units (C = 96: the six longest launches of the encoder / generator forward).
+// Weight-stationary variant for the narrow units (C = 96: the six longest launches of the encoder / generator forward of
+// v2; C = 64: the audio-rate stage of the raw-waveform generator, where W3 + W1 are 32 KB).
 // dilated_unit_tc_kernel re-streams, for EVERY 128-row tile, the three tap-shifted copies of the activation rows
 // (3 x 24 KB) and the whole weight set (W3 54 KB + W1 18 KB) from L2: 144 KB per tile.  Here the weights are loaded
 // ONCE per CTA and stay in shared memory (72 KB), and each tile brings ONE haloed activation tile (128 + 2 dil rows):
@@ -345,14 +349,19 @@ dilated_unit_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
 constexpr int UW_THREADS = 160;
 constexpr int UW_AROWS = 152;                       // 128 + 2 * dil rows, dil <= 12
 constexpr int UW_ASLAB = UW_AROWS * 64;             // one 32-channel K block of the haloed tile (64-byte rows)
-constexpr int UW_WSLAB = 96 * 64;                   // one (tap, K block) weight slab: 96 rows x 32 channels
 constexpr int UW_STAGES = 3;
-constexpr int UW_W3_OFF = 0, UW_W1_OFF = 9 * UW_WSLAB, UW_A_OFF = 12 * UW_WSLAB;
-constexpr int UW_A2_OFF = UW_A_OFF + UW_STAGES * 3 * UW_ASLAB;
-constexpr int UW_OUT_OFF = UW_A2_OFF + 3 * (128 * 64);      // staging tile of the bf16 output (TMA store source)
-constexpr int UW_BAR_OFF = UW_OUT_OFF + 3 * (128 * 64);
-constexpr int UW_TOTAL = UW_BAR_OFF + 256 + 1024;
-static_assert(UW_TOTAL <= U_SMEM_MAX, "weight-stationary unit: shared memory");
+
+template <int C>
+struct UwCfg {
+  static constexpr int KB = C / 32;                     // 32-channel K blocks
+  static constexpr int WSLAB = C * 64;                  // one (tap, K block) weight slab: C rows x 32 channels
+  static constexpr int W3_OFF = 0, W1_OFF = 3 * KB * WSLAB, A_OFF = 4 * KB * WSLAB;
+  static constexpr int A2_OFF = A_OFF + UW_STAGES * KB * UW_ASLAB;
+  static constexpr int OUT_OFF = A2_OFF + KB * (128 * 64);      // staging tile of the bf16 output (TMA store source)
+  static constexpr int BAR_OFF = OUT_OFF + KB * (128 * 64);
+  static constexpr int TOTAL = BAR_OFF + 256 + 1024;
+  static_assert(C % 32 == 0 && TOTAL <= U_SMEM_MAX, "weight-stationary unit: shared memory");
+};
 
 // byte offset of channel c (even) of row `row` in a [rows][32 ch] 64-byte-swizzled K-block sequence of `slab` bytes
 __device__ __forceinline__ uint32_t sw64_off(int row, int c, uint32_t slab) {
@@ -360,11 +369,15 @@ __device__ __forceinline__ uint32_t sw64_off(int row, int c, uint32_t slab) {
          (uint32_t)(c & 7) * 2u;
 }
 
+template <int C>
 __global__ void __launch_bounds__(UW_THREADS, 1)
-dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w3,
-                         const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_out,
-                         const __grid_constant__ CUtensorMap tmap_a1, const UnitParams p) {
-  constexpr int C = 96, BK = 32, KB = 3, SWZ = 64, A2_SLAB = 128 * 64;
+dilated_unit_ws_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_w3,
+                       const __grid_constant__ CUtensorMap tmap_w1, const __grid_constant__ CUtensorMap tmap_out,
+                       const __grid_constant__ CUtensorMap tmap_a1, const UnitParams p) {
+  using W = UwCfg<C>;
+  constexpr int BK = 32, KB = W::KB, SWZ = 64, A2_SLAB = 128 * 64;
+  constexpr int UW_WSLAB = W::WSLAB, UW_W3_OFF = W::W3_OFF, UW_W1_OFF = W::W1_OFF, UW_A_OFF = W::A_OFF;
+  constexpr int UW_A2_OFF = W::A2_OFF, UW_OUT_OFF = W::OUT_OFF, UW_BAR_OFF = W::BAR_OFF;
   constexpr uint64_t A_HALF = (64 * SWZ) >> 4;        // rows 64 .. 127 of a K-major operand tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -397,7 +410,7 @@ dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
   if (warp == 4) {
     // =========================== TMA producer ===========================
     if (elect_one()) {                                   // weights: once
-      mbar_arrive_expect_tx(w_bar, 12 * UW_WSLAB);
+      mbar_arrive_expect_tx(w_bar, 4 * KB * UW_WSLAB);
       for (int k = 0; k < 3; ++k)
         for (int kb = 0; kb < KB; ++kb)
           tma_load_2d(smem + UW_W3_OFF + (k * KB + kb) * UW_WSLAB, &tmap_w3, w_bar, kb * BK, k * C);
@@ -410,7 +423,7 @@ dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
       const int lt = tile % p.n_lt, b0 = tile / p.n_lt;          // BB == 1
       const int row0 = lt * 128 - p.pad_l;
       mbar_wait(&empty_bar[stage], phase ^ 1);
-      uint8_t *sa = smem + UW_A_OFF + stage * 3 * UW_ASLAB;
+      uint8_t *sa = smem + UW_A_OFF + stage * KB * UW_ASLAB;
       if (elect_one()) {
         mbar_arrive_expect_tx(&full_bar[stage], (uint32_t)(KB * arows * 64));
         for (int kb = 0; kb < KB; ++kb) tma_load_4d(sa + kb * UW_ASLAB, &tmap_a, &full_bar[stage], kb * BK, 0, row0, b0);
@@ -434,7 +447,7 @@ dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
     const int l0 = lt * 128;
     // ---- phase 1: conv3 over the haloed tile
     mbar_wait(&full_bar[stage], phase);
-    const uint32_t sa = smem_base + UW_A_OFF + stage * 3 * UW_ASLAB;
+    const uint32_t sa = smem_base + UW_A_OFF + stage * KB * UW_ASLAB;
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -501,7 +514,7 @@ dilated_unit_ws96_kernel(const __grid_constant__ CUtensorMap tmap_a, const __gri
       else bulk_wait_read<0>();
     }
     if (p.out_act) named_bar_sync(1, 128);
-    const uint8_t *sah = smem + UW_A_OFF + stage * 3 * UW_ASLAB;
+    const uint8_t *sah = smem + UW_A_OFF + stage * KB * UW_ASLAB;
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -559,13 +572,13 @@ static EncodeTiledFnU unit_encode_fn() {
   return fn;
 }
 
-template <int C, int BK>
+template <int C, int BK, int NC>
 static int launch_unit(const CUtensorMap &ta, const CUtensorMap &t3, const CUtensorMap &t1, const UnitParams &p,
                        cudaStream_t stream) {
-  using L = UnitCfg<C, BK>;
+  using L = UnitCfg<C, BK, NC>;
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dilated_unit_tc_kernel<C, BK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(dilated_unit_tc_kernel<C, BK, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          L::TOTAL);
     if (e != cudaSuccess) {
       set_error("dilated_unit_tc: cudaFuncSetAttribute(%d bytes): %s", L::TOTAL, cudaGetErrorString(e));
@@ -578,8 +591,37 @@ static int launch_unit(const CUtensorMap &ta, const CUtensorMap &t3, const CUten
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
-  launch_pdl(dilated_unit_tc_kernel<C, BK>, dim3(grid), dim3(U_THREADS), L::TOTAL, stream, ta, t3, t1, p);
+  launch_pdl(dilated_unit_tc_kernel<C, BK, NC>, dim3(grid), dim3(U_THREADS), L::TOTAL, stream, ta, t3, t1, p);
   RAVE_CHECK_LAUNCH("dilated_unit_tc");
+  return 0;
+}
+
+// N chunk of dilated_unit_tc_kernel per width.  NC = 128 would need 128 accumulator registers per MMA thread on top of
+// the ~26 the kernel keeps besides them (122 at NC = 96): over the 152 that 416 threads per SM leave, so the widths
+// that 96 does not divide run in 64-column chunks.
+static int unit_chunk(int C) { return C % 96 == 0 ? 96 : 64; }
+
+template <int C>
+static int launch_unit_ws(const CUtensorMap &ta, const CUtensorMap &t3, const CUtensorMap &t1, const CUtensorMap &tout,
+                          const CUtensorMap &ta1, const UnitParams &p, cudaStream_t stream) {
+  using W = UwCfg<C>;
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(dilated_unit_ws_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         W::TOTAL);
+    if (e != cudaSuccess) {
+      set_error("dilated_unit_tc(ws): cudaFuncSetAttribute(%d bytes): %s", W::TOTAL, cudaGetErrorString(e));
+      return 2;
+    }
+    attr = true;
+  }
+  const int tiles = p.n_lt * p.n_bg;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  launch_pdl(dilated_unit_ws_kernel<C>, dim3(tiles < sms ? tiles : sms), dim3(UW_THREADS), W::TOTAL, stream, ta, t3,
+             t1, tout, ta1, p);
+  RAVE_CHECK_LAUNCH("dilated_unit_tc(ws)");
   return 0;
 }
 
@@ -587,7 +629,7 @@ static int launch_unit(const CUtensorMap &ta, const CUtensorMap &t3, const CUten
 }  // namespace rave
 
 extern "C" int rave_dilated_unit_tc_supported(int C, int L) {
-  return (C == 96 || C == 192 || C == 384) && L >= 8;
+  return (C == 64 || C == 96 || C == 128 || C == 192 || C == 256 || C == 384) && L >= 8;
 }
 
 extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const void *w1t, void *a1_out, float *out_f32,
@@ -596,7 +638,8 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
   using namespace rave;
   using namespace rave::tc;
   RAVE_CHECK_ARG(xa && w3t && w1t && (out_f32 || out_act), "dilated_unit_tc: null pointer");
-  RAVE_CHECK_ARG(rave_dilated_unit_tc_supported(C, L), "dilated_unit_tc: unsupported width C=%d (96, 192, 384)", C);
+  RAVE_CHECK_ARG(rave_dilated_unit_tc_supported(C, L), "dilated_unit_tc: unsupported width C=%d (64, 96, 128, 192, 256, 384)",
+                 C);
   RAVE_CHECK_ARG(B > 0 && L > 0 && dil >= 1 && pad_l >= 0, "dilated_unit_tc: bad shape");
   if (pitch <= 0) pitch = L;
   RAVE_CHECK_ARG(pitch >= L, "dilated_unit_tc: pitch %d < L %d", pitch, L);
@@ -625,7 +668,7 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
   p.out_act = (__nv_bfloat16 *)out_act;
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  const int NC = 96;
+  const int NC = unit_chunk(C);
   CUtensorMap ta, t3, t1;
   {
     cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
@@ -647,7 +690,7 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc: weight tensor map encode failed (%d)", (int)r);
   }
   cudaStream_t s = (cudaStream_t)stream;
-  if (C == 96 && p.BB == 1 && dil <= 12) {
+  if ((C == 64 || C == 96) && p.BB == 1 && dil <= 12) {
     // weight-stationary kernel: its activation map carries the haloed box (128 + 2 dil rows), its weight maps one
     // (tap, K block) slab per box
     CUtensorMap tah, t3s, t1s;
@@ -664,27 +707,14 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
     for (int which = 0; which < 2; ++which) {
       cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
       cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-      cuuint32_t box[2] = {32, 96};
+      cuuint32_t box[2] = {32, (cuuint32_t)C};
       cuuint32_t estr[2] = {1, 1};
       CUresult r = enc(which == 0 ? &t3s : &t1s, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
                        const_cast<void *>(which == 0 ? w3t : w1t), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                        CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): weight tensor map encode failed (%d)", (int)r);
     }
-    static bool attr = false;
-    if (!attr) {
-      cudaError_t er = cudaFuncSetAttribute(dilated_unit_ws96_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, UW_TOTAL);
-      if (er != cudaSuccess) {
-        set_error("dilated_unit_tc(ws): cudaFuncSetAttribute(%d bytes): %s", UW_TOTAL, cudaGetErrorString(er));
-        return 2;
-      }
-      attr = true;
-    }
-    const int tiles = p.n_lt * p.n_bg;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // bf16 outputs leave through TMA: [B][pitch][96] viewed as (c, 1, row, b) boxes of one 32-channel K block x 128 rows
+    // bf16 outputs leave through TMA: [B][pitch][C] viewed as (c, 1, row, b) boxes of one 32-channel K block x 128 rows
     // (rows >= L and batches >= B are clipped by the TMA unit)
     CUtensorMap tout, ta1;
     memset(&tout, 0, sizeof(tout));
@@ -701,15 +731,15 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): output tensor map encode failed (%d)", (int)r);
     }
-    launch_pdl(dilated_unit_ws96_kernel, dim3(tiles < sms ? tiles : sms), dim3(UW_THREADS), UW_TOTAL, s, tah, t3s, t1s,
-               tout, ta1, p);
-    RAVE_CHECK_LAUNCH("dilated_unit_tc(ws)");
-    return 0;
+    return C == 64 ? launch_unit_ws<64>(tah, t3s, t1s, tout, ta1, p, s) : launch_unit_ws<96>(tah, t3s, t1s, tout, ta1, p, s);
   }
   switch (C) {
-    case 96: return launch_unit<96, 32>(ta, t3, t1, p, s);
-    case 192: return launch_unit<192, 64>(ta, t3, t1, p, s);
-    case 384: return launch_unit<384, 64>(ta, t3, t1, p, s);
+    case 64: return launch_unit<64, 64, 64>(ta, t3, t1, p, s);
+    case 96: return launch_unit<96, 32, 96>(ta, t3, t1, p, s);
+    case 128: return launch_unit<128, 64, 64>(ta, t3, t1, p, s);
+    case 192: return launch_unit<192, 64, 96>(ta, t3, t1, p, s);
+    case 256: return launch_unit<256, 64, 64>(ta, t3, t1, p, s);
+    case 384: return launch_unit<384, 64, 96>(ta, t3, t1, p, s);
   }
   set_error("dilated_unit_tc: no kernel for C=%d", C);
   return 1;

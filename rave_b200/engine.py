@@ -179,6 +179,10 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
         return None
     specs[-1].is_output = True
     specs[-1].want_f32 = True
+    if specs[-1].Cout % 16:
+        # narrow output conv (the raw-waveform generator's 64 -> 2): computed with zero weight rows up to a multiple of
+        # 16 output channels, as plan_convnet does for score layers; the caller keeps the first Cout channels
+        specs[-1].cout_pad = 16 - specs[-1].Cout % 16
     return specs
 
 
