@@ -293,6 +293,16 @@ int rave_im2col_c1(const float *src, void *X_bf16, int R, int src_pitch, int src
                    int out_pitch, int K, int stride, int pad_l, int period, int pool, void *stream);
 int rave_gather_c1(const float *P, float *dsrc, int R, int src_pitch, int src_len, int Lin, int Lout, int p_pitch,
                    int K, int stride, int pad_l, int period, int pool, void *stream);
+/* The same for a first layer with cin input channels (multichannel models): src [Bs][cin][src_pitch], the fold /
+ * pooling applied per channel (R = Bs*period rows, independent of cin), X rows of W = 16 or 32 bf16 columns
+ *   X[r][l][c*K + k] = bf16(row_{r,c}[l*stride + k - pad_l])   (cin*K <= W: the [c][k] order of
+ *                                                                weight.reshape(Cout, Cin*K); zero beyond cin*K)
+ * and the adjoint from P [R][p_pitch][W] fp32 into dsrc [Bs][cin][src_pitch].  rave_im2col_c1 / rave_gather_c1 are
+ * the cin = 1, W = 16 instances. */
+int rave_im2col_cin(const float *src, void *X_bf16, int R, int cin, int src_pitch, int src_len, int Lin, int Lout,
+                    int out_pitch, int W, int K, int stride, int pad_l, int period, int pool, void *stream);
+int rave_gather_cin(const float *P, float *dsrc, int R, int cin, int src_pitch, int src_len, int Lin, int Lout,
+                    int p_pitch, int W, int K, int stride, int pad_l, int period, int pool, void *stream);
 int rave_fm_stats(const void *a_bf16, float *stats, int Bh, int L, int pitch, int C, float slope, void *stream);
 int rave_fm_grad(const void *a_bf16, const float *dstats, void *gout_bf16, int Bh, int L, int pitch, int C,
                  float slope, void *stream);

@@ -74,6 +74,8 @@ SIGNATURES = {
     "rave_colsum_bf16": (c_int, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_im2col_c1": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_gather_c1": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "rave_im2col_cin": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "rave_gather_cin": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_fm_stats": (c_int, [_P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_fm_grad": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_score_stats": (c_int, [_P, _P, _I, _I, _I, _I, _P]),

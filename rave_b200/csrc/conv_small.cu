@@ -610,64 +610,89 @@ __device__ __forceinline__ float c1_src_value(const float *__restrict__ xb, int 
   return pool > 1 ? v / (float)pool : v;
 }
 
+// Writes one X row: column j = c*K + k (the [c][k] order of weight.reshape(Cout, Cin*K)), zero from cin*K to W (cin = 0:
+// an all-zero slack row).  The running (c, k) pair replaces a division per column; `val(c, k)` is the source value of
+// channel c at tap k.  Each 16-byte group is stored as soon as it is packed: only 4 words stay live (at W = 32 the
+// whole row held in registers cut the staged kernel's occupancy to a third).
+template <int W, typename F>
+__device__ __forceinline__ void write_cin_row(__nv_bfloat16 *dst_row, int cin, int K, F val) {
+  uint4 *dst = reinterpret_cast<uint4 *>(dst_row);
+  int c = 0, k = 0;
+#pragma unroll
+  for (int q = 0; q < W / 8; ++q) {
+    uint32_t wd[4];
+#pragma unroll
+    for (int j2 = 0; j2 < 4; ++j2) {
+      float v[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        v[h] = c < cin ? val(c, k) : 0.f;
+        if (++k == K) {
+          k = 0;
+          ++c;
+        }
+      }
+      wd[j2] = pack_bf16(v[0], v[1]);
+    }
+    dst[q] = make_uint4(wd[0], wd[1], wd[2], wd[3]);
+  }
+}
+
 // Per-thread variant, only for shapes whose staged tile (below) exceeds 96 KB of shared memory (large periods).
-// grid (ceil(pitch/256), R), block 256: one thread = one position = one 32-byte row of X (a single 256-bit store);
+// grid (ceil(pitch/256), R), block 256: one thread = one position = one 2W-byte row of X (W/8 16-byte stores);
 // the K source positions of neighbouring threads overlap (K > stride), so the strided reads hit in L1
+template <int W>
 __global__ void __launch_bounds__(256)
-im2col_c1_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ X, int src_pitch, int src_len, int Lin,
-                 int Lout, int out_pitch, int K, int stride, int pad_l, int period, int pool) {
+im2col_cin_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ X, int cin, int src_pitch, int src_len,
+                  int Lin, int Lout, int out_pitch, int K, int stride, int pad_l, int period, int pool) {
   const int r = blockIdx.y;
   const int l = blockIdx.x * 256 + threadIdx.x;
   if (l >= out_pitch) return;
-  uint32_t wds[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-  if (l < Lout) {
-    const int b = r / period, w = r - b * period;
-    const float *xb = x + (size_t)b * src_pitch;
-    const int p0 = l * stride - pad_l;
-#pragma unroll
-    for (int k2 = 0; k2 < 8; ++k2) {
-      float v0 = 0.f, v1 = 0.f;
-      const int pa = p0 + 2 * k2, pb = pa + 1;
-      if (2 * k2 < K && pa >= 0 && pa < Lin) v0 = c1_src_value(xb, pa, w, period, pool, src_len);
-      if (2 * k2 + 1 < K && pb >= 0 && pb < Lin) v1 = c1_src_value(xb, pb, w, period, pool, src_len);
-      wds[k2] = pack_bf16(v0, v1);
-    }
-  }
-  uint4 *dst = reinterpret_cast<uint4 *>(X + ((size_t)r * out_pitch + l) * 16);
-  dst[0] = make_uint4(wds[0], wds[1], wds[2], wds[3]);
-  dst[1] = make_uint4(wds[4], wds[5], wds[6], wds[7]);
+  const int b = r / period, w = r - b * period;
+  const float *xb = x + (size_t)b * cin * src_pitch;
+  const int p0 = l * stride - pad_l;
+  write_cin_row<W>(X + ((size_t)r * out_pitch + l) * W, l < Lout ? cin : 0, K, [&](int c, int k) {
+    const int p = p0 + k;
+    return (p >= 0 && p < Lin) ? c1_src_value(xb + (size_t)c * src_pitch, p, w, period, pool, src_len) : 0.f;
+  });
 }
 
-// Staged variant (every tile up to 96 KB): the per-thread gather above issues 16 strided loads per output row -- a warp access
-// touches 32 addresses (stride * period) floats apart, 8-44 sectors for 128 useful bytes, and the L1 wavefront queue,
-// not HBM, set its pace (40 us for a 33 MB operand).  Here one CTA serves IC_NL output positions of ALL `period` rows
-// of one source batch entry: the contiguous source span is read once, coalesced, and de-interleaved into shared memory
-// (one padded line per fold row w; the index skew i + i/32 makes the stride-`stride` tap reads conflict-free for
-// stride 1, 2, 4); every thread then assembles 32-byte rows from shared memory and stores them back to back.
+// Staged variant (every tile up to 96 KB): the per-thread gather above issues K strided loads per output row and
+// channel -- a warp access touches 32 addresses (stride * period) floats apart, 8-44 sectors for 128 useful bytes, and
+// the L1 wavefront queue, not HBM, set its pace (40 us for a 33 MB operand).  Here one CTA serves IC_NL output
+// positions of ALL `period` rows of one source batch entry: the contiguous source span of each channel is read once,
+// coalesced, and de-interleaved into shared memory (one padded line per channel and fold row (c, w); the index skew
+// i + i/32 makes the stride-`stride` tap reads conflict-free for stride 1, 2, 4); every thread then assembles 2W-byte
+// rows from shared memory and stores them back to back.
 constexpr int IC_NL = 128;
 __device__ __forceinline__ int ic_skew(int i) { return i + (i >> 5); }
 
-__global__ void __launch_bounds__(256)
-im2col_c1_staged_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ X, int src_pitch, int src_len, int Lin,
-                        int Lout, int out_pitch, int K, int stride, int pad_l, int period, int pool, int line) {
-  extern __shared__ float sm[];                      // [period][line]
+template <int W>
+__global__ void __launch_bounds__(256, 4)   // >= 32 warps per SM: the W = 32 instance otherwise takes 98 registers
+im2col_cin_staged_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__ X, int cin, int src_pitch,
+                         int src_len, int Lin, int Lout, int out_pitch, int K, int stride, int pad_l, int period,
+                         int pool, int line) {
+  extern __shared__ float sm[];                      // [cin][period][line]
   const int b = blockIdx.y;
   const int l0 = blockIdx.x * IC_NL;
   const int p_lo = l0 * stride - pad_l;
   const int n_p = (IC_NL - 1) * stride + K;
-  const float *xb = x + (size_t)b * src_pitch;
-  if (period > 1) {                                  // fold: element (p, w) lives at p * period + w
-    const long e_lo = (long)p_lo * period;
-    for (int q = threadIdx.x; q < n_p * period; q += blockDim.x) {
-      const int pp = q / period, w = q - pp * period;
-      const int pos = p_lo + pp;
-      const long e = e_lo + q;
-      sm[w * line + ic_skew(pp)] = (pos >= 0 && pos < Lin && e < src_len) ? __ldg(xb + e) : 0.f;
-    }
-  } else {                                           // average pooling: position p = mean of `pool` consecutive samples
-    for (int pp = threadIdx.x; pp < n_p; pp += blockDim.x) {
-      const int pos = p_lo + pp;
-      sm[ic_skew(pp)] = (pos >= 0 && pos < Lin) ? c1_src_value(xb, pos, 0, 1, pool, src_len) : 0.f;
+  for (int c = 0; c < cin; ++c) {
+    const float *xb = x + ((size_t)b * cin + c) * src_pitch;
+    float *smc = sm + (size_t)c * period * line;
+    if (period > 1) {                                // fold: element (p, w) lives at p * period + w
+      const long e_lo = (long)p_lo * period;
+      for (int q = threadIdx.x; q < n_p * period; q += blockDim.x) {
+        const int pp = q / period, w = q - pp * period;
+        const int pos = p_lo + pp;
+        const long e = e_lo + q;
+        smc[w * line + ic_skew(pp)] = (pos >= 0 && pos < Lin && e < src_len) ? __ldg(xb + e) : 0.f;
+      }
+    } else {                                         // average pooling: position p = mean of `pool` consecutive samples
+      for (int pp = threadIdx.x; pp < n_p; pp += blockDim.x) {
+        const int pos = p_lo + pp;
+        smc[ic_skew(pp)] = (pos >= 0 && pos < Lin) ? c1_src_value(xb, pos, 0, 1, pool, src_len) : 0.f;
+      }
     }
   }
   __syncthreads();
@@ -675,45 +700,39 @@ im2col_c1_staged_kernel(const float *__restrict__ x, __nv_bfloat16 *__restrict__
     const int w = idx / IC_NL, ll = idx - w * IC_NL;
     const int l = l0 + ll;
     if (l >= out_pitch) continue;
-    uint32_t wds[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
-    if (l < Lout) {
-      const float *row = sm + w * line;
-      const int q0 = ll * stride;
-#pragma unroll
-      for (int k2 = 0; k2 < 8; ++k2) {
-        const float v0 = (2 * k2 < K) ? row[ic_skew(q0 + 2 * k2)] : 0.f;
-        const float v1 = (2 * k2 + 1 < K) ? row[ic_skew(q0 + 2 * k2 + 1)] : 0.f;
-        wds[k2] = pack_bf16(v0, v1);
-      }
-    }
-    uint4 *dst = reinterpret_cast<uint4 *>(X + ((size_t)(b * period + w) * out_pitch + l) * 16);
-    dst[0] = make_uint4(wds[0], wds[1], wds[2], wds[3]);
-    dst[1] = make_uint4(wds[4], wds[5], wds[6], wds[7]);
+    const float *row = sm + w * line;
+    const int q0 = ll * stride, cs = period * line;
+    write_cin_row<W>(X + ((size_t)(b * period + w) * out_pitch + l) * W, l < Lout ? cin : 0, K,
+                     [&](int c, int k) { return row[c * cs + ic_skew(q0 + k)]; });
   }
 }
 
-// dsrc[b][(t*pool + j)*period + w] += (1/pool) * sum_k P[r][(t + pad - k)/stride][k]; P fp32 channel-last [R][p_pitch][16].
-// Every source element is touched by at most one (r, t, j): plain read-modify-write, launches are stream-ordered.
+// dsrc[b][c][(t*pool + j)*period + w] += (1/pool) * sum_k P[r][(t + pad - k)/stride][c*K + k]; P fp32 channel-last
+// [R][p_pitch][W].  Every source element is touched by at most one (r, t, j) thread: plain read-modify-write, launches
+// are stream-ordered.
+template <int W>
 __global__ void __launch_bounds__(256)
-gather_c1_kernel(const float *__restrict__ P, float *__restrict__ dx, int src_pitch, int src_len, int Lin, int Lout,
-                 int p_pitch, int K, int stride, int pad_l, int period, int pool) {
+gather_cin_kernel(const float *__restrict__ P, float *__restrict__ dx, int cin, int src_pitch, int src_len, int Lin,
+                  int Lout, int p_pitch, int K, int stride, int pad_l, int period, int pool) {
   const int r = blockIdx.y;
   const int t = blockIdx.x * 256 + threadIdx.x;
   if (t >= Lin) return;
-  float acc = 0.f;
-  const float *Pr = P + (size_t)r * p_pitch * 16;
+  const float *Pr = P + (size_t)r * p_pitch * W;
   // taps k = k0 + m stride hit output rows l0 - m: ONE integer division per thread (the loop used to divide twice per
   // tap by the run-time stride: ~125 of the thread's ~150 instructions)
   const int l0 = (t + pad_l) / stride;
   const int k0 = (t + pad_l) - l0 * stride;
-  for (int k = k0, l = l0; k < K && l >= 0; k += stride, --l)
-    if (l < Lout) acc += __ldg(Pr + (size_t)l * 16 + k);
   const int b = r / period, w = r - b * period;
-  float *db = dx + (size_t)b * src_pitch;
-  if (pool > 1) acc /= (float)pool;
-  for (int j = 0; j < pool; ++j) {
-    const long e = ((long)t * pool + j) * period + w;
-    if (e < src_len) db[e] += acc;
+  for (int c = 0; c < cin; ++c) {
+    float acc = 0.f;
+    for (int k = k0, l = l0; k < K && l >= 0; k += stride, --l)
+      if (l < Lout) acc += __ldg(Pr + (size_t)l * W + c * K + k);
+    float *db = dx + ((size_t)b * cin + c) * src_pitch;
+    if (pool > 1) acc /= (float)pool;
+    for (int j = 0; j < pool; ++j) {
+      const long e = ((long)t * pool + j) * period + w;
+      if (e < src_len) db[e] += acc;
+    }
   }
 }
 
@@ -721,45 +740,74 @@ gather_c1_kernel(const float *__restrict__ P, float *__restrict__ dx, int src_pi
 
 static inline int ic_skew_host(int i) { return i + (i >> 5); }
 
-extern "C" int rave_im2col_c1(const float *x, void *X_bf16, int R, int src_pitch, int src_len, int Lin, int Lout,
-                              int out_pitch, int K, int stride, int pad_l, int period, int pool, void *stream) {
+template <int W>
+static int im2col_cin_launch(const float *x, void *X_bf16, int R, int cin, int src_pitch, int src_len, int Lin,
+                             int Lout, int out_pitch, int K, int stride, int pad_l, int period, int pool,
+                             void *stream) {
   using namespace rave;
-  RAVE_CHECK_ARG(x && X_bf16 && R > 0 && R <= 65535 && K > 0 && K <= 16 && out_pitch >= Lout && period >= 1 &&
-                     pool >= 1 && (period == 1 || pool == 1) && R % period == 0,
-                 "im2col_c1: bad argument");
   const int n_p = (IC_NL - 1) * stride + K;
   const int line = (ic_skew_host(n_p - 1) + 1) | 1;    // odd pitch: the de-interleaving stores spread over the banks
-  const size_t smem = (size_t)period * line * sizeof(float);
+  const size_t smem = (size_t)cin * period * line * sizeof(float);
   if (stride >= 1 && smem <= 96 * 1024) {
     static bool attr = false;
     if (!attr) {
-      cudaFuncSetAttribute(im2col_c1_staged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
+      cudaFuncSetAttribute(im2col_cin_staged_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024);
       attr = true;
     }
     dim3 grid(ceil_div(out_pitch, IC_NL), R / period);
     // period 1: 128 rows per CTA -> 128 threads (one row each); folds: 128 * period rows over 256 threads
-    im2col_c1_staged_kernel<<<grid, period == 1 ? 128 : 256, smem, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)X_bf16, src_pitch, src_len, Lin,
-                                                                      Lout, out_pitch, K, stride, pad_l, period, pool, line);
-    RAVE_CHECK_LAUNCH("im2col_c1_staged");
+    im2col_cin_staged_kernel<W><<<grid, period == 1 ? 128 : 256, smem, (cudaStream_t)stream>>>(
+        x, (__nv_bfloat16 *)X_bf16, cin, src_pitch, src_len, Lin, Lout, out_pitch, K, stride, pad_l, period, pool, line);
+    RAVE_CHECK_LAUNCH("im2col_cin_staged");
     return 0;
   }
   dim3 grid(ceil_div(out_pitch, 256), R);
-  im2col_c1_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)X_bf16, src_pitch, src_len, Lin, Lout,
-                                                           out_pitch, K, stride, pad_l, period, pool);
-  RAVE_CHECK_LAUNCH("im2col_c1");
+  im2col_cin_kernel<W><<<grid, 256, 0, (cudaStream_t)stream>>>(x, (__nv_bfloat16 *)X_bf16, cin, src_pitch, src_len,
+                                                               Lin, Lout, out_pitch, K, stride, pad_l, period, pool);
+  RAVE_CHECK_LAUNCH("im2col_cin");
   return 0;
+}
+
+extern "C" int rave_im2col_cin(const float *x, void *X_bf16, int R, int cin, int src_pitch, int src_len, int Lin,
+                               int Lout, int out_pitch, int W, int K, int stride, int pad_l, int period, int pool,
+                               void *stream) {
+  RAVE_CHECK_ARG(x && X_bf16 && R > 0 && R <= 65535 && cin >= 1 && K > 0 && (W == 16 || W == 32) && cin * K <= W &&
+                     out_pitch >= Lout && period >= 1 && pool >= 1 && (period == 1 || pool == 1) && R % period == 0,
+                 "im2col_cin: bad argument");
+  if (W == 16)
+    return im2col_cin_launch<16>(x, X_bf16, R, cin, src_pitch, src_len, Lin, Lout, out_pitch, K, stride, pad_l, period,
+                                 pool, stream);
+  return im2col_cin_launch<32>(x, X_bf16, R, cin, src_pitch, src_len, Lin, Lout, out_pitch, K, stride, pad_l, period,
+                               pool, stream);
+}
+
+extern "C" int rave_gather_cin(const float *P, float *dsrc, int R, int cin, int src_pitch, int src_len, int Lin,
+                               int Lout, int p_pitch, int W, int K, int stride, int pad_l, int period, int pool,
+                               void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(P && dsrc && R > 0 && R <= 65535 && cin >= 1 && K > 0 && (W == 16 || W == 32) && cin * K <= W &&
+                     p_pitch >= Lout && period >= 1 && pool >= 1 && (period == 1 || pool == 1) && R % period == 0,
+                 "gather_cin: bad argument");
+  dim3 grid(ceil_div(Lin, 256), R);
+  if (W == 16)
+    gather_cin_kernel<16><<<grid, 256, 0, (cudaStream_t)stream>>>(P, dsrc, cin, src_pitch, src_len, Lin, Lout, p_pitch,
+                                                                  K, stride, pad_l, period, pool);
+  else
+    gather_cin_kernel<32><<<grid, 256, 0, (cudaStream_t)stream>>>(P, dsrc, cin, src_pitch, src_len, Lin, Lout, p_pitch,
+                                                                  K, stride, pad_l, period, pool);
+  RAVE_CHECK_LAUNCH("gather_cin");
+  return 0;
+}
+
+extern "C" int rave_im2col_c1(const float *x, void *X_bf16, int R, int src_pitch, int src_len, int Lin, int Lout,
+                              int out_pitch, int K, int stride, int pad_l, int period, int pool, void *stream) {
+  return rave_im2col_cin(x, X_bf16, R, 1, src_pitch, src_len, Lin, Lout, out_pitch, 16, K, stride, pad_l, period,
+                         pool, stream);
 }
 extern "C" int rave_gather_c1(const float *P, float *dsrc, int R, int src_pitch, int src_len, int Lin, int Lout,
                               int p_pitch, int K, int stride, int pad_l, int period, int pool, void *stream) {
-  using namespace rave;
-  RAVE_CHECK_ARG(P && dsrc && R > 0 && R <= 65535 && K > 0 && K <= 16 && p_pitch >= Lout && period >= 1 && pool >= 1 &&
-                     (period == 1 || pool == 1) && R % period == 0,
-                 "gather_c1: bad argument");
-  dim3 grid(ceil_div(Lin, 256), R);
-  gather_c1_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(P, dsrc, src_pitch, src_len, Lin, Lout, p_pitch, K, stride,
-                                                           pad_l, period, pool);
-  RAVE_CHECK_LAUNCH("gather_c1");
-  return 0;
+  return rave_gather_cin(P, dsrc, R, 1, src_pitch, src_len, Lin, Lout, p_pitch, 16, K, stride, pad_l, period, pool,
+                         stream);
 }
 
 // ---------------------------------------------------------------------------------------------

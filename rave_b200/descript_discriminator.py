@@ -200,7 +200,7 @@ class MPD(nn.Module):
 
     def _tc_specs(self):
         """Plan of the whole MPD as ONE tensor-core chain (bf16 mode): conv -> LeakyReLU(0.1) -> ... -> conv_post, every
-        conv's fp32 output kept (the features are its activation).  The period axis folds into the batch, the Cin = 1
+        conv's fp32 output kept (the features are its activation).  The period axis folds into the batch, the
         first layer reads the folded signal in place (engine.TcChainFn)."""
         from . import engine
         if "_tc_specs_cache" not in self.__dict__:
@@ -218,8 +218,8 @@ class MPD(nn.Module):
         from . import engine
         from .discriminator import ConvNet
         B, C, L, W = x.shape
-        xa, _, _, _ = ConvNet._chain_input(None, x, specs)
-        outs = engine.run_chain(xa, specs, L)
+        xa, src, _, _, _ = ConvNet._chain_input(None, x, specs)
+        outs = engine.run_chain(xa, specs, L, src=src)
         lens = engine.chain_lengths(specs, L)
         fmap = []
         for i, (s, o, Lo) in enumerate(zip(specs, outs, lens)):
@@ -238,9 +238,9 @@ class MPD(nn.Module):
         fmap = []
         x = self.pad_to_period(x)
         x = x.reshape(x.shape[0], x.shape[1], -1, self.period)
-        if engine.precision() == "bf16" and x.is_cuda and x.shape[1] == 1:
+        if engine.precision() == "bf16" and x.is_cuda:
             specs = self._tc_specs()
-            if specs is not None:
+            if specs is not None and engine.raw_input_ok(specs[0], x.shape[1]):
                 return self._forward_tc(x, specs)
         pre = None          # activation of the previous layer, fused into the next conv's operand load
         for layer in self.convs:
@@ -299,11 +299,14 @@ class MRD(nn.Module):
     def _forward_cl(self, x):
         """bf16 engine mode: the whole MRD channel-last.  The complex spectrogram [B, t, f, (re, im)] is already the
         channel-last input of the first conv; every conv's output buffer is the next conv's input and -- after the one
-        LeakyReLU pass -- the feature (an NCHW *view*, torch's channels_last layout)."""
+        LeakyReLU pass -- the feature (an NCHW *view*, torch's channels_last layout).  With C > 1 channels the B*C
+        spectrograms are interleaved into [B, t, f, (c, p)] ("b c f t p -> b (c p) t f"): one copy of the spectrogram."""
         B, C, T = x.shape
         st = self.stft
         z = ops.rfft(ops.stft_frames(x.reshape(B * C, T), st.window, st.n_fft, st.hop), st.rfft_bw)
-        x0 = torch.view_as_real(z)                                          # [B, t, f, 2]: "b (c p) t f" for c = 1
+        x0 = torch.view_as_real(z)                                          # [(b c), t, f, 2]
+        if C > 1:
+            x0 = x0.unflatten(0, (B, C)).permute(0, 2, 3, 1, 4).reshape(B, x0.shape[1], x0.shape[2], 2 * C)
         t = x0.shape[1]
         fmap, outs = [], []
         for (lo, hi), stack in zip(self.bands, self.band_convs):
@@ -326,7 +329,7 @@ class MRD(nn.Module):
         return fmap
 
     def forward(self, x):
-        if (x.is_cuda and x.shape[1] == 1 and x.shape[-1] > self.stft.n_fft // 2
+        if (x.is_cuda and x.shape[-1] > self.stft.n_fft // 2
                 and self.conv_post.tc_ready(x, 32) and self.band_convs[0][0][0].cout_ok()):
             return self._forward_cl(x)
         fmap = []

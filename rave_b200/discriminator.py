@@ -94,26 +94,29 @@ class ConvNet(nn.Module):
         return self.__dict__["_tc_specs_cache"]
 
     def _chain_input(self, x, specs):
-        """Channel-last operand of the chain.  Cin = 1 (every shipped config): the raw fp32 rows
-        [B(*W), pitch] for the small-channel first-layer kernel; otherwise the zero-padded bf16 stream."""
+        """Operand of the chain and the `src` argument of engine.run_chain.  A first layer that reads the signal in
+        place (engine.raw_input_ok: every shipped config, mono or stereo) gets the raw fp32 rows, [B(*W), pitch] for
+        mono and [B(*W), C, pitch] otherwise; any other first layer the zero-padded channel-last bf16 stream."""
         from . import engine
         first = specs[0]
         if x.dim() == 3:
             B, C, L = x.shape
             W = 1
-            rows = x.transpose(1, 2)
         else:
             B, C, L, W = x.shape
-            rows = x.permute(0, 3, 2, 1).reshape(B * W, L, C)
         rpad = (-L) % first.stride              # row pitch: a multiple of the first layer's stride
-        if C == 1 and first.dil == 1:
-            xa = nn.functional.pad(rows.reshape(B * W, L), (0, rpad)).contiguous()
-        else:
-            xa = nn.functional.pad(rows, (0, first.cin_pad, 0, rpad)).to(engine.ACT_DTYPE).contiguous()
-        return xa, B, W, L
+        if engine.raw_input_ok(first, C):
+            rows = x.unsqueeze(-1) if x.dim() == 3 else x          # [B, C, L, W]
+            rows = rows.permute(0, 3, 1, 2).reshape(B * W, C, L)
+            if C == 1:
+                return nn.functional.pad(rows.reshape(B * W, L), (0, rpad)).contiguous(), None, B, W, L
+            return nn.functional.pad(rows, (0, rpad)).contiguous(), (1, 1), B, W, L
+        rows = x.transpose(1, 2) if x.dim() == 3 else x.permute(0, 3, 2, 1).reshape(B * W, L, C)
+        xa = nn.functional.pad(rows, (0, first.cin_pad, 0, rpad)).to(engine.ACT_DTYPE).contiguous()
+        return xa, None, B, W, L
 
     def forward_fm(self, x, period: int = 1, pool: int = 1, fake_grad_only: bool = False):
-        """Fused feature-matching path (bf16 engine): x = cat([real, fake]) RAW signal [B, 1, T] -> (stats [n-1, 2],
+        """Fused feature-matching path (bf16 engine): x = cat([real, fake]) RAW signal [B, C, T] -> (stats [n-1, 2],
         counts, score, score_stats [3, 2], n_score) with stats[i] = (sum|h_r - h_f|, sum|h_r|) of hidden feature i,
         counts[i] = its number of elements per half, score = the last conv's output in the reference's shape,
         score_stats = the six sums of the score tail (engine.TcChainFn), n_score = score elements per half.
@@ -122,12 +125,14 @@ class ConvNet(nn.Module):
         from . import engine
         specs = self._tc_specs()
         first = specs[0]
-        if x.dim() != 3 or x.shape[1] != 1 or first.Cin != 1 or first.dil != 1:
-            raise RuntimeError("forward_fm expects a mono signal [B, 1, T] and a Cin = 1 first layer")
-        B, _, T = x.shape
+        if x.dim() != 3 or not engine.raw_input_ok(first, x.shape[1]):
+            raise RuntimeError("forward_fm expects a signal [B, C, T] and a first layer that reads its C channels in "
+                               "place (engine.raw_input_ok)")
+        B, C, T = x.shape
         W = period
         L = (T + period - 1) // period if period > 1 else T // pool
-        stats, score_stats, last = engine.run_chain(x.reshape(B, T), specs, L, fm=True, src=(period, pool),
+        xr = x.reshape(B, T) if C == 1 else x.contiguous()
+        stats, score_stats, last = engine.run_chain(xr, specs, L, fm=True, src=(period, pool),
                                                     fake_grad_only=fake_grad_only)
         lens = engine.chain_lengths(specs, L)
         counts = [(B // 2) * W * Lo * s.Cout for s, Lo in zip(specs[:-1], lens[:-1])]
@@ -145,8 +150,8 @@ class ConvNet(nn.Module):
         """bf16 tensor-core path: the whole ConvNet as one chain in channel-last layout; features come
         back as permuted views with the reference's shapes."""
         from . import engine
-        xa, B, W, L = self._chain_input(x, specs)
-        outs = engine.run_chain(xa, specs, L)
+        xa, src, B, W, L = self._chain_input(x, specs)
+        outs = engine.run_chain(xa, specs, L, src=src)
         lens = engine.chain_lengths(specs, L)
         features = []
         for s, o, Lo in zip(specs, outs, lens):
@@ -239,7 +244,7 @@ class CombineDiscriminators(nn.Module):
     def supports_fused_fm(self, x) -> bool:
         """True when every sub-discriminator can run the fused feature-matching path on `x`."""
         from . import engine
-        if engine.precision() != "bf16" or not x.is_cuda or x.dim() != 3 or x.shape[1] != 1:
+        if engine.precision() != "bf16" or not x.is_cuda or x.dim() != 3:
             return False
         for disc in self.discriminators:
             if not hasattr(disc, "forward_fm"):
@@ -248,8 +253,7 @@ class CombineDiscriminators(nn.Module):
                 if not isinstance(layer, ConvNet) or layer._tc_specs() is None:
                     return False
                 specs = layer._tc_specs()
-                first = specs[0]
-                if first.Cin != 1 or first.dil != 1:
+                if not engine.raw_input_ok(specs[0], x.shape[1]):
                     return False
                 # the statistics are read from the bf16 operand a = LeakyReLU(h) of the NEXT layer: every hidden feature
                 # needs a LeakyReLU consumer and un-padded channels (tiny test capacities have Cout % 16 != 0)

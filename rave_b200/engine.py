@@ -29,8 +29,9 @@ from . import _lib, ops
 _state = {"precision": "fp32", "prep_epoch": 0}
 ACT_DTYPE = torch.bfloat16   # storage type of operand / gradient streams (tests may widen it)
 
-# output positions per tensor-core row of a Cin = 1 first layer (see TcChainFn.forward); pitches that are not a
-# multiple of it run with one position (plain 16-channel rows)
+# output positions per tensor-core row of a raw first layer with 16-column operand rows (see TcChainFn.forward); rows
+# of 32 columns (multichannel, Cin*K > 16) take half as many; pitches that are not a multiple of it run with one
+# position (plain W-channel rows)
 C1_GROUP = 4
 # Residual(DilatedUnit) blocks as ONE launch (csrc/unit_tc.cu) where the width allows it, else two launches per unit
 FUSE_UNITS = True
@@ -79,6 +80,12 @@ class LayerSpec:
                                    # residual stream: the skip is recovered from it (no fp32 copy of h_src)
     pre_mod: Optional[nn.Module] = None   # the Snake module (owner of alpha) when pre_act == ACT_SNAKE
     res_raw: Optional[int] = None  # Snake units: index of the layer whose raw (pre-Snake) bf16 input IS the skip stream
+
+
+def raw_input_ok(spec: LayerSpec, cin: int) -> bool:
+    """True when a chain whose first layer is `spec` can read a raw fp32 signal of `cin` channels in place (TcChainFn:
+    the Cin*K taps of a position fit one operand row of 16 columns for mono, 32 for more channels)."""
+    return spec.kind == "conv" and spec.Cin == cin and spec.dil == 1 and spec.K * cin <= (16 if cin == 1 else 32)
 
 
 def chain_supported(specs: List[LayerSpec]) -> bool:
@@ -443,10 +450,11 @@ def _out_len(spec: LayerSpec, Lin: int) -> int:
 class TcChainFn(torch.autograd.Function):
     """forward(x, specs, L0, fm, *flat_params).
 
-    x   : [B, pitch, Cin(+pad)] operand stream (ACT_DTYPE), or -- when the first layer has Cin == 1 --
-          a raw fp32 signal tensor [Bs, T] from which the chain rows are read in place: `src = (period, pool)`
-          (L0 = positions per row; B = Bs*period rows; MPD fold / MSD pooling, ops.im2col_c1); no padding to 16
-          channels, no bf16 rounding of the audio, no folded / pooled copy.
+    x   : [B, pitch, Cin(+pad)] operand stream (ACT_DTYPE), or -- when the first layer passes raw_input_ok --
+          a raw fp32 signal tensor, [Bs, T] (mono) or [Bs, Cin, T] with `src` given, from which the chain rows are
+          read in place: `src = (period, pool)` (L0 = positions per row; B = Bs*period rows; MPD fold / MSD pooling,
+          ops.im2col_c1 / ops.im2col_cin); no padding to 16 channels, no bf16 rounding of the audio, no folded /
+          pooled copy.
     fm  : False -> returns one fp32 channel-last tensor per `is_output` layer;
           True  -> discriminator feature-matching mode: the batch is [real; fake]; returns
                    (stats [n-1, 2] = per hidden layer (sum|h_r-h_f|, sum|h_r|),
@@ -476,8 +484,9 @@ class TcChainFn(torch.autograd.Function):
         if alpha_idx and (x3 or fm):
             raise _lib.RaveB200Error("Snake chains run in the plain bf16 mode only (no split operands, no fused fm)")
         hraw: Dict[int, torch.Tensor] = {}     # raw (pre-Snake) bf16 input stream of layer i
-        c1 = x_in.dim() == 2
+        c1 = x_in.dim() == 2 or src is not None
         period, pool = src if (c1 and src is not None) else (1, 1)
+        cin = x_in.shape[1] if (c1 and x_in.dim() == 3) else 1
         B = x_in.shape[0] * period
         ctx.c1_src = (period, pool, tuple(x_in.shape))
         ctx.B = B
@@ -486,8 +495,9 @@ class TcChainFn(torch.autograd.Function):
         plain = all(s.kind == "conv" and s.res_src is None and s.res_opnd is None and s.res_raw is None
                     and s.pre_act != ops.ACT_SNAKE for s in specs)
         ctx.fake_grad_only = bool(fake_grad_only) and (fm or (plain and B % 2 == 0 and not x3))
-        if c1 and not (specs[0].kind == "conv" and specs[0].Cin == 1 and specs[0].dil == 1):
-            raise _lib.RaveB200Error("raw fp32 rows are only accepted by a Cin = 1 first conv")
+        if c1 and not raw_input_ok(specs[0], cin):
+            raise _lib.RaveB200Error("raw fp32 rows are only accepted by a first conv with Cin = the signal's channels, "
+                                     "Cin * K <= 32 and no dilation")
         dev = x_in.device
         a = x_in
         f32: Dict[int, torch.Tensor] = {}
@@ -577,23 +587,31 @@ class TcChainFn(torch.autograd.Function):
                         t[:, Lout:].zero_()
             acts.append(a)
             if use_c1:
-                # Cin = 1: the K taps become the 16 "channels" of a tiny im2col X[r][l][k].  Four consecutive
-                # positions are then read as ONE 64-channel row (X viewed as [R][L/4][64], 128-byte TMA rows
-                # instead of 32-byte ones) against the block-diagonal weight kron(I4, w): the output row holds
-                # the 4 x Cout results of those positions, i.e. the same bytes as out[r][4*l4 + p][co].
-                G = C1_GROUP if (pitch % C1_GROUP == 0) else 1
+                # raw first layer: the Cin*K taps become the W (16 or 32) "channels" of a tiny im2col X[r][l][c*K + k].
+                # G = 64 / W consecutive positions are then read as ONE 64-channel row (X viewed as [R][L/G][64],
+                # 128-byte TMA rows instead of 2W-byte ones) against the block-diagonal weight kron(I_G, w): the output
+                # row holds the G x Cout results of those positions, i.e. the same bytes as out[r][G*lg + p][co].
+                Wc = ops.cin_width(cin, s.K)
+                G = max(1, C1_GROUP * 16 // Wc)
+                if pitch % G:
+                    G = 1
                 Xp = (Lout + G - 1) // G * G
-                X = ops.im2col_c1(a, Lin, Lout, Xp, s.K, s.stride, s.pad[0], period, pool)
+                if a.dim() == 2:         # mono rows [Bs, T]
+                    X = ops.im2col_c1(a, Lin, Lout, Xp, s.K, s.stride, s.pad[0], period, pool)
+                else:
+                    X = ops.im2col_cin(a, Lin, Lout, Xp, s.K, s.stride, s.pad[0], period, pool)
                 ctx.c1_X = X
                 ctx.c1_group = G
+                ctx.c1_width = Wc
 
-                def c1_weights(s=s, G=G, cout_p=cout_p):
+                def c1_weights(s=s, G=G, cout_p=cout_p, Wc=Wc):
                     v_, g_, b_ = _layer_params(s)
                     w_eff = ops.weight_norm_raw(v_.detach(), g_.detach())[0] if g_ is not None else v_.detach()
-                    w_ck = nn.functional.pad(w_eff.reshape(s.Cout, s.K), (0, 16 - s.K, 0, s.cout_pad))   # [Cout_p, 16]
+                    w_ck = nn.functional.pad(w_eff.reshape(s.Cout, s.Cin * s.K),
+                                             (0, Wc - s.Cin * s.K, 0, s.cout_pad))                 # [Cout_p, W]
                     if G > 1:
                         eye = torch.eye(G, dtype=w_ck.dtype, device=w_ck.device)
-                        w_blk = (eye[:, None, :, None] * w_ck[None, :, None, :]).reshape(G * cout_p, G * 16)
+                        w_blk = (eye[:, None, :, None] * w_ck[None, :, None, :]).reshape(G * cout_p, G * Wc)
                     else:
                         w_blk = w_ck
                     bp = b_
@@ -601,11 +619,12 @@ class TcChainFn(torch.autograd.Function):
                         bp = nn.functional.pad(b_.detach(), (0, s.cout_pad))
                     bias_g_ = bp.detach().repeat(G) if (bp is not None and G > 1) else (bp.detach() if bp is not None
                                                                                          else None)
-                    return (w_blk.to(ACT_DTYPE).unsqueeze(0).contiguous(),                     # [1][G*Cout_p][G*16]
-                            w_blk.t().contiguous().to(ACT_DTYPE).unsqueeze(0), bias_g_)        # [1][G*16][G*Cout_p]
+                    return (w_blk.to(ACT_DTYPE).unsqueeze(0).contiguous(),                     # [1][G*Cout_p][G*W]
+                            w_blk.t().contiguous().to(ACT_DTYPE).unsqueeze(0), bias_g_)        # [1][G*W][G*Cout_p]
 
                 static = s.module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
-                rec = static.get(("c1", G, cout_p)) if static is not None else None
+                skey = ("c1", G, Wc, cout_p)
+                rec = static.get(skey) if static is not None else None
                 if rec is None:
                     w_fwd, w_dg, bias_g = c1_weights()
                     if static is not None and not torch.cuda.is_current_stream_capturing():
@@ -615,11 +634,11 @@ class TcChainFn(torch.autograd.Function):
                             w_dg.copy_(b_)
                             if bias_g is not None:
                                 bias_g.copy_(c_)
-                        static[("c1", G, cout_p)] = {"t": (w_fwd, w_dg, bias_g), "refresh": _refresh}
+                        static[skey] = {"t": (w_fwd, w_dg, bias_g), "refresh": _refresh}
                 else:
                     w_fwd, w_dg, bias_g = rec["t"]
                 ctx.c1_wt_dgrad = w_dg
-                ops.conv1d_tc(X.view(B, Xp // G, G * 16), w_fwd, bias_g,
+                ops.conv1d_tc(X.view(B, Xp // G, G * Wc), w_fwd, bias_g,
                               None, 1, 1, (0, 0), act_code, act_slope, want_f32=False, want_act=False,
                               out_f32=out_f32.view(B, pitch // G, G * cout_p) if out_f32 is not None else None,
                               out_act=out_act.view(B, pitch // G, G * cout_p) if out_act is not None else None,
@@ -754,22 +773,22 @@ class TcChainFn(torch.autograd.Function):
                 if i in db_off:
                     db = db_all[db_off[i]:db_off[i] + cout_p]
                 if use_c1:
-                    G = ctx.c1_group
+                    G, Wc = ctx.c1_group, ctx.c1_width
                     X = ctx.c1_X
                     if G > 1 and g.shape[1] % G == 0 and X.shape[1] % G == 0:
                         # same G-positions-per-row view as the forward: 64-channel rows for the TMA loads; the wanted
-                        # [Cout][16] gradient is the sum of the G diagonal blocks of the [G*Cout][G*16] result
+                        # [Cout][W] gradient is the sum of the G diagonal blocks of the [G*Cout][G*W] result
                         dbw = torch.zeros(G * cout_p, dtype=torch.float32, device=g.device) if db is not None else None
-                        d = ops.conv1d_tc_wgrad(g.view(B, g.shape[1] // G, G * cout_p), X.view(B, X.shape[1] // G, G * 16),
+                        d = ops.conv1d_tc_wgrad(g.view(B, g.shape[1] // G, G * cout_p), X.view(B, X.shape[1] // G, G * Wc),
                                                 1, 1, 1, 0, Lp=(Lout + G - 1) // G, Lq=(Lout + G - 1) // G, dbias=dbw)
-                        blk = d.sum(0)[0].view(G, cout_p, G, 16)
-                        dw_full = torch.diagonal(blk, dim1=0, dim2=2).sum(-1)                  # [Cout_p][16]
+                        blk = d.sum(0)[0].view(G, cout_p, G, Wc)
+                        dw_full = torch.diagonal(blk, dim1=0, dim2=2).sum(-1)                  # [Cout_p][W]
                         if db is not None:
                             db.copy_(dbw.view(G, cout_p).sum(0))
                     else:
                         dw_full = ops.conv1d_tc_wgrad(g, X, 1, 1, 1, 0, Lp=Lout, Lq=Lout, dbias=db).sum(0)[0]
-                    dw_ck = dw_full[:s.Cout, :s.K]                                             # [Cout][K]
-                    dwt = dw_ck.t().reshape(1, s.K, s.Cout, 1).contiguous()                    # [1][K][C0][C1=1]
+                    dw_ck = dw_full[:s.Cout, :s.Cin * s.K].reshape(s.Cout, s.Cin, s.K)         # [Cout][Cin][K]
+                    dwt = dw_ck.permute(2, 0, 1).reshape(1, s.K, s.Cout, s.Cin).contiguous()   # [1][K][C0][C1]
                 else:
                     P_op, Q_op = (g, a_in) if s.kind == "conv" else (a_in, g)
                     Lp_, Lq_ = (Lout, Lin) if s.kind == "conv" else (Lin, Lout)
@@ -812,22 +831,23 @@ class TcChainFn(torch.autograd.Function):
             add_conv = None if snake_here else add       # Snake: the skip / external gradient joins after dSnake
             fm_partner = a_full[:Bh] if (fo and fm_d is not None) else None
             in_pitch = a_in.shape[1]
-            if use_c1:                  # P[r][l][k] = <g[r][l][:], w[:][k]> on the tensor cores, then a gather
-                G = ctx.c1_group
+            if use_c1:                  # P[r][l][c*K + k] = <g[r][l][:], w[:][c][k]> on the tensor cores, then a gather
+                G, Wc = ctx.c1_group, ctx.c1_width
                 gpitch = g.shape[1]
                 if G > 1 and gpitch % G == 0:
-                    # same 4-positions-per-row view as the forward (slack rows of g are zero)
+                    # same G-positions-per-row view as the forward (slack rows of g are zero)
                     P, _ = ops.conv1d_tc(g.view(B, gpitch // G, G * cout_p), ctx.c1_wt_dgrad, None, None, 1, 1, (0, 0),
                                          ops.ACT_NONE, 0.0, want_f32=True, want_act=False, Lout=gpitch // G,
                                          Lin=gpitch // G)
-                    P = P.view(B, gpitch, 16)
+                    P = P.view(B, gpitch, Wc)
                 else:
-                    wt_d = ctx.c1_wt_dgrad if G == 1 else ctx.c1_wt_dgrad[:, :16, :cout_p].contiguous()
+                    wt_d = ctx.c1_wt_dgrad if G == 1 else ctx.c1_wt_dgrad[:, :Wc, :cout_p].contiguous()
                     P, _ = ops.conv1d_tc(g, wt_d, None, None, 1, 1, (0, 0), ops.ACT_NONE, 0.0, want_f32=True,
                                          want_act=False, Lout=Lout, Lin=Lout)
                 period, pool, src_shape = ctx.c1_src
-                gx = ops.gather_c1(P, src_shape, Lin, Lout, s.K, s.stride, s.pad[0], period, pool,
-                                   batch0=src_shape[0] // 2 if fo else 0)
+                gather = ops.gather_c1 if len(src_shape) == 2 else ops.gather_cin
+                gx = gather(P, src_shape, Lin, Lout, s.K, s.stride, s.pad[0], period, pool,
+                            batch0=src_shape[0] // 2 if fo else 0)
                 break
             if fo and i == 0:
                 # fake-rows-only backward: the chain's input gradient is [zeros; gx_fake] -- the last dgrad writes its
@@ -915,7 +935,7 @@ class fake_rows_only:
 def run_chain(x_cl_bf16: torch.Tensor, specs: List[LayerSpec], L0: Optional[int] = None, fm: bool = False,
               src: Optional[Tuple[int, int]] = None, fake_grad_only: bool = False, x3: bool = False):
     """x_cl_bf16: [B, pitch, Cin(+pad)] (rows beyond the true length L0 must be zero), or raw fp32 rows
-    [B, pitch] for a Cin = 1 first layer.  Returns one fp32 channel-last tensor [B, pitch_i, Cout_i(+pad)]
+    [B, pitch] for a Cin = 1 first layer, or [B, Cin, pitch] with `src` given (engine.raw_input_ok).  Returns one fp32 channel-last tensor [B, pitch_i, Cout_i(+pad)]
     per output layer (slice [:, :L_i, :Cout_i]); with fm=True: (stats [n-1, 2], score_stats [3, 2], last layer
     output)."""
     flat = []

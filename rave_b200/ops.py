@@ -893,6 +893,39 @@ def gather_c1(P_cl, src_shape, Lin, Lout, K, stride, pad_l, period=1, pool=1, ba
     return dsrc
 
 
+def cin_width(cin, K):
+    """Row width W (bf16 columns) of the multichannel first-layer operand: 16 or 32 >= cin*K."""
+    return 16 if cin * K <= 16 else 32
+
+
+def im2col_cin(src, Lin, Lout, out_pitch, K, stride, pad_l, period=1, pool=1):
+    """im2col_c1 for a first layer with Cin = src.shape[1] channels: X [R, out_pitch, W] bf16 (W = cin_width(cin, K))
+    with X[r, l, c*K + k] = row_{r,c}[l*stride + k - pad_l], the rows read from src [Bs, cin, T] through the fold /
+    pooling of each channel (R = Bs*period)."""
+    src = _f32c(src)
+    Bs, cin, T = src.shape
+    W = cin_width(cin, K)
+    R = Bs * period
+    X = torch.empty(R, out_pitch, W, dtype=torch.bfloat16, device=src.device)
+    call("rave_im2col_cin", ptr(src), ptr(X), R, cin, T, T, Lin, Lout, out_pitch, W, K, stride, pad_l, period, pool,
+         stream_ptr())
+    return X
+
+
+def gather_cin(P_cl, src_shape, Lin, Lout, K, stride, pad_l, period=1, pool=1, batch0=0):
+    """dsrc [Bs, cin, T] fp32: the adjoint of im2col_cin applied to P [R, p_pitch, W] fp32.  With batch0 > 0, P holds
+    only the rows of source batches batch0 .. Bs-1 (the other gradients stay zero)."""
+    P_cl = _f32c(P_cl)
+    R, p_pitch, W = P_cl.shape
+    Bs, cin, T = src_shape
+    dsrc = torch.zeros(Bs, cin, T, dtype=torch.float32, device=P_cl.device)
+    if R != (Bs - batch0) * period or W != cin_width(cin, K):
+        raise _lib.RaveB200Error("gather_cin: P does not match the source batches or the row width")
+    call("rave_gather_cin", ptr(P_cl), dsrc.data_ptr() + batch0 * cin * T * 4, R, cin, T, T, Lin, Lout, p_pitch, W, K,
+         stride, pad_l, period, pool, stream_ptr())
+    return dsrc
+
+
 # ----------------------------------------------------------------------------------------------
 # fused spectral distance of one STFT scale (csrc/spectral.cu)
 # ----------------------------------------------------------------------------------------------
