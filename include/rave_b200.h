@@ -403,6 +403,31 @@ int rave_noise_fir_bwd(const float *h, const float *M, const float *noise, const
                        int NB, int T, int TS, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Mel front end of the hybrid encoder (rave/model.py:238-242, torchaudio MelSpectrogram(normalized=True)):
+ *   out[n][m][f] = log1p(scale * sum_{k in [lo_m, hi_m)} w[off_m + k - lo_m] |X[n][f][k]|^2),  f < F - 1
+ * X: [N][F][bins] complex64 (rfft of centred frames), band: [M][3] ints (lo, hi, off), weights: the nnz packed
+ * nonzero filter-bank entries, out: [N][M][F-1] (= [B][C*M][F-1] for n = b*C + c), scale = 1 / sum(window^2).
+ * ------------------------------------------------------------------------------------------- */
+int rave_mel_log1p_fwd(const void *X_c64, const int *band, const float *weights, float *out, int N, int F, int bins,
+                       int M, int nnz, float scale, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
+ * GRU layer (rave/blocks.py:295-319: nn.GRU, gate order r, z, n), fp32, H = 128, one persistent launch per layer:
+ *   fwd: gi [B][T][3H] = W_ih x_t + b_ih (precomputed), w_hh [3H][H], b_hh [3H] -> h_out [B][T][H] (h0 = 0);
+ *        save [B][T][5][H] = (r, z, n, W_hn h + b_hn, h_prev) for the backward (NULL: not written)
+ *   bwd: dy [B][T][H] (gradient of h_out) -> gate gradients dgi [B][T][3H] (of gi) and dgh [B][T][3H] (of W_hh h + b_hh)
+ * ------------------------------------------------------------------------------------------- */
+int rave_gru_fwd(const float *gi, const float *w_hh, const float *b_hh, float *h_out, float *save, int B, int T, int H,
+                 void *stream);
+int rave_gru_bwd(const float *dy, const float *save, const float *w_hh, float *dgi, float *dgh, int B, int T, int H,
+                 void *stream);
+/* C[m][n] = sum_k A[m*sam + k*sak] B[k*sbk + n*sbn] (+ bias[n]), row pitch ldc; rowsum[m] = sum_k A(m, k) if non-NULL.
+ * Fixed-order split-K over `splits` (rave_gemm_f32_splits) with workspace ws of splits*(M*N + M) floats. */
+int rave_gemm_f32_splits(int M, int N, int K);
+int rave_gemm_f32(const float *A, long sam, long sak, const float *B, long sbk, long sbn, const float *bias, float *C,
+                  long ldc, float *rowsum, int M, int N, int K, float *ws, int splits, void *stream);
+
+/* ---------------------------------------------------------------------------------------------
  * Multi-tensor Adam, torch.optim.Adam arithmetic without weight decay / amsgrad (rave/model.py:226-236):
  *   step += 1;  m = lerp(m, g, 1-b1);  v = b2 v + (1-b2) g^2;  p -= lr/(1-b1^step) * m / (sqrt(v)/sqrt(1-b2^step) + eps)
  * n fp32 tensors given by host arrays of device pointers; lr and step are single device floats (graph-replayable).

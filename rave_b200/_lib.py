@@ -87,6 +87,11 @@ SIGNATURES = {
     "rave_stft_frames_valid": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_stft_frames_valid_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_rfft_bwd_scale": (c_int, [_P, _P, _L, _I, _I, _L, _L, _L, _P]),
+    "rave_mel_log1p_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_gru_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_gru_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_gemm_f32_splits": (c_int, [_I, _I, _I]),
+    "rave_gemm_f32": (c_int, [_P, _L, _L, _P, _L, _L, _P, _P, _L, _P, _I, _I, _I, _P, _I, _P]),
     "rave_noise_fir_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_noise_fir_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_adam_multi": (c_int, [_I, _P, _P, _P, _P, _P, _P, _P, _F, _F, _F, _P]),

@@ -433,6 +433,29 @@ class NoiseGeneratorV2(nn.Module):
         return out.reshape(out.shape[0], out.shape[1], -1)
 
 
+class GRU(nn.Module):
+    """rave/blocks.py:295-319 (configs/hybrid.gin: GeneratorV2.recurrent_layer, num_layers 2): nn.GRU over the time
+    axis of [B, C, T], on rave_gru_fwd / rave_gru_bwd and GEMMs (ops.gru).  `gru_state` is the reference's (unused)
+    buffer; `disable()` makes the module an identity."""
+
+    def __init__(self, latent_size: int, num_layers: int) -> None:
+        super().__init__()
+        self.gru = nn.GRU(input_size=latent_size, hidden_size=latent_size, num_layers=num_layers, batch_first=True)
+        self.register_buffer("gru_state", torch.tensor(0))
+        self.enabled = True
+
+    def forward(self, x: torch.Tensor) -> torch.Tensor:
+        if not self.enabled:
+            return x
+        return ops.gru(x, self.gru)
+
+    def disable(self):
+        self.enabled = False
+
+    def enable(self):
+        self.enabled = True
+
+
 def normalize_dilations(dilations, ratios):
     if isinstance(dilations[0], int):
         dilations = [dilations for _ in ratios]

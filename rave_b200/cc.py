@@ -226,6 +226,9 @@ class CachedSequential(nn.Sequential):
         if res is None and mode in ("bf16", "bf16x3") and x.is_cuda and x.dim() == 3 and not self._cached:
             specs = self._tc_plan()
             if specs is not None and (specs[0].kind != "conv" or x.shape[-1] % specs[0].stride == 0):
+                lead = engine.split_recurrent(list(self))[0]
+                if lead is not None:
+                    x = lead(x)
                 (out,) = engine.run_chain(engine.to_channel_last(x, x3=x3), specs, x3=x3)
                 Lout = engine.chain_lengths(specs, x.shape[-1])[-1]
                 Cout = specs[-1].Cout

@@ -37,7 +37,30 @@ ARCH = {
     "v2_nopqmf": dict(capacity=64, ratios=[4, 4, 4, 2], gen_ratios=[8, 8, 8, 4], raw_output=True,   # v2_nopqmf.gin:15-23
                       activation="leaky", adain=False, disc="v2",
                       update_discriminator_every=4, phase_1_duration=1000000),              # v2_nopqmf.gin:95-106
+    # `--config v2 --config hybrid`: mel-spectrogram encoder input and a GRU generator head (HYBRID below)
+    "v2_hybrid": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False, disc="v2",
+                      update_discriminator_every=4, phase_1_duration=1000000, hybrid=True),
 }
+
+# configs/hybrid.gin on top of any v2-style configuration: EncoderV2(data_size=N_MELS, ratios=[2, 2, 2], dilations=[1])
+# fed log1p(MelSpectrogram(n_fft=2048, hop=256, normalized=True, n_mels=128)) (input_mode "mel"), and
+# GeneratorV2.recurrent_layer = GRU(LATENT_SIZE, num_layers=2)
+HYBRID = dict(n_mels=128, n_fft=2048, hop_length=256, encoder_ratios=[2, 2, 2], encoder_dilations=[1],
+              num_gru_layers=2)
+
+
+def _hybrid_parts(hybrid):
+    """(encoder overrides, generator recurrent_layer) of the hybrid switch."""
+    if not hybrid:
+        return None, None
+    enc = dict(data_size=HYBRID["n_mels"], ratios=HYBRID["encoder_ratios"], dilations=HYBRID["encoder_dilations"])
+    return enc, partial(blocks.GRU, num_layers=HYBRID["num_gru_layers"])
+
+
+def mel_spectrogram(sampling_rate):
+    """The hybrid configuration's transforms.MelSpectrogram binding (configs/hybrid.gin:19-25)."""
+    return core.MelSpectrogram(sampling_rate, n_fft=HYBRID["n_fft"], win_length=HYBRID["n_fft"],
+                               hop_length=HYBRID["hop_length"], normalized=True, n_mels=HYBRID["n_mels"])
 
 
 def _activation_factory(kind):
@@ -48,13 +71,16 @@ def _activation_factory(kind):
 
 def make_autoencoder(name="v2", capacity=None, latent_size=128, n_band=16, n_channels=1,
                      padding_mode="centered", ratios=None, activation=None, adain=None, with_noise=False,
-                     gen_ratios=None):
+                     gen_ratios=None, hybrid=None):
     """(pqmf, encoder, decoder) factories -> constructed modules for one architecture.  `gen_ratios`: the generator's
-    own ratios (v2_nopqmf; defaults to the configuration's, else `ratios`)."""
+    own ratios (v2_nopqmf; defaults to the configuration's, else `ratios`).  `hybrid` (default: the configuration's):
+    mel-input encoder (its input is core.MelSpectrogram.encode_log1p of the waveform) and GRU generator head."""
     a = ARCH[name]
+    hyb_enc, recurrent = _hybrid_parts(a.get("hybrid", False) if hybrid is None else hybrid)
     capacity = capacity or a["capacity"]
     ratios = ratios or a["ratios"]
     gen_ratios = gen_ratios or a.get("gen_ratios") or ratios
+    enc_kw = {**dict(data_size=n_band, ratios=ratios, dilations=V2_DILATIONS), **(hyb_enc or {})}
     raw = a.get("raw_output", False)
     act = _activation_factory(activation or a["activation"])
     use_adain = a["adain"] if adain is None else adain
@@ -62,9 +88,8 @@ def make_autoencoder(name="v2", capacity=None, latent_size=128, n_band=16, n_cha
     with cc.configure(conv_bias=False, padding_mode=padding_mode):       # v1.gin:33-34, causal.gin:5
         pq = pqmf.CachedPQMF(attenuation=100, n_band=n_band, n_channels=n_channels)  # v1.gin:37-39
         enc = blocks.VariationalEncoder(                                  # v2.gin:30-40
-            partial(blocks.EncoderV2, data_size=n_band, capacity=capacity, ratios=ratios,
-                    latent_size=latent_size, n_out=2, kernel_size=3, dilations=V2_DILATIONS,
-                    activation=act, adain=adain_f),
+            partial(blocks.EncoderV2, capacity=capacity, latent_size=latent_size, n_out=2, kernel_size=3,
+                    activation=act, adain=adain_f, **enc_kw),
             n_channels=n_channels)
         noise = None
         if name == "v2_small" and with_noise:                                  # v2_small.gin:42-57
@@ -73,7 +98,7 @@ def make_autoencoder(name="v2", capacity=None, latent_size=128, n_band=16, n_cha
         dec = blocks.GeneratorV2(data_size=None if raw else n_band, capacity=capacity, ratios=gen_ratios,  # v2.gin:43-50
                                  latent_size=latent_size, kernel_size=3, dilations=V2_DILATIONS,
                                  amplitude_modulation=True, activation=act, adain=adain_f,
-                                 n_channels=n_channels, noise_module=noise)
+                                 n_channels=n_channels, noise_module=noise, recurrent_layer=recurrent)
     return pq, enc, dec
 
 
@@ -103,10 +128,15 @@ def make_discriminator_v2_spectral(capacity=96, n_channels=1, spectral_capacity=
 
 
 def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n_channels=1,
-               padding_mode="centered", phase_1_duration=None, disc_capacity=None, ratios=None, spectral_capacity=32):
+               padding_mode="centered", phase_1_duration=None, disc_capacity=None, ratios=None, spectral_capacity=32,
+               hybrid=None):
     """The full `RAVE` model of a named configuration (`spectral_capacity`: EncodecConvNet capacity of "v2_spectral",
-    configs/spectral_discriminator.gin:11)."""
+    configs/spectral_discriminator.gin:11).  `hybrid=True` adds `--config hybrid` to any configuration with a
+    VariationalEncoder (default: the configuration's own, True for "v2_hybrid")."""
     a = ARCH[name]
+    hyb_enc, recurrent = _hybrid_parts(a.get("hybrid", False) if hybrid is None else hybrid)
+    if hyb_enc is not None and a.get("discrete"):
+        raise NotImplementedError("hybrid: the mel-input encoder is built for VariationalEncoder configurations")
     cap = capacity or a["capacity"]
     act = _activation_factory(a["activation"])
     adain_f = (lambda dim: blocks.AdaptiveInstanceNormalization(dim)) if a["adain"] else None
@@ -133,10 +163,10 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
                                          dim=latent_size, codebook_size=1024),
                           num_quantizers=16, noise_augmentation=noise_aug)
     else:
+        enc_kw = {**dict(data_size=16, ratios=rat, dilations=V2_DILATIONS), **(hyb_enc or {})}
         encoder = partial(blocks.VariationalEncoder,
-                          partial(blocks.EncoderV2, data_size=16, capacity=cap, ratios=rat,
-                                  latent_size=latent_size, n_out=2, kernel_size=3,
-                                  dilations=V2_DILATIONS, activation=act, adain=adain_f))
+                          partial(blocks.EncoderV2, capacity=cap, latent_size=latent_size, n_out=2, kernel_size=3,
+                                  activation=act, adain=adain_f, **enc_kw))
     noise = None
     if name == "v2_small":                                                       # v2_small.gin:42-57
         noise = partial(blocks.NoiseGeneratorV2, hidden_size=64, data_size=16, ratios=[2, 2, 2],
@@ -149,7 +179,7 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
             decoder=partial(blocks.GeneratorV2, data_size=None if raw else 16, capacity=cap, ratios=gen_rat,
                             latent_size=core.get_augmented_latent_size(latent_size, noise_aug), kernel_size=3,
                             dilations=V2_DILATIONS, amplitude_modulation=True, activation=act, adain=adain_f,
-                            noise_module=noise),
+                            noise_module=noise, recurrent_layer=recurrent),
             discriminator=disc,
             phase_1_duration=phase_1_duration if phase_1_duration is not None else a["phase_1_duration"],
             gan_loss=core.hinge_gan, valid_signal_crop=True,                  # v2.gin:81-83
@@ -158,5 +188,7 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
             audio_distance=distance, multiband_audio_distance=distance,
             weights={"feature_matching": 20},                                 # v2.gin:87-89
             update_discriminator_every=a["update_discriminator_every"], n_channels=n_channels,
-            output_mode="raw" if raw else "pqmf")
+            output_mode="raw" if raw else "pqmf",
+            spectrogram=mel_spectrogram(sampling_rate) if hyb_enc is not None else None,
+            input_mode="mel" if hyb_enc is not None else "pqmf")
     return model

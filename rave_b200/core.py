@@ -4,6 +4,7 @@ PyTorch for now; the conv / PQMF hot path they consume is native).
 """
 from typing import Callable, Optional, Sequence
 
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -148,6 +149,95 @@ class MultiScaleSTFT(nn.Module):
 
     def forward(self, x):
         return [y.abs() if self.magnitude else torch.stack([y.real, y.imag], -1) for y in self.complex_stfts(x)]
+
+
+def htk_mel_filterbank(sample_rate: int, n_fft: int, n_mels: int) -> torch.Tensor:
+    """[n_fft // 2 + 1, n_mels] triangular HTK filter bank, norm=None, f_min = 0, f_max = sample_rate // 2: the `fb`
+    buffer of torchaudio.transforms.MelScale (torchaudio.functional.melscale_fbanks), computed in numpy."""
+    # float32 throughout, as torchaudio computes it: the zero pattern (which bins feed which band) is then the same
+    f32 = np.float32
+    n_freqs = n_fft // 2 + 1
+    all_freqs = np.linspace(0.0, float(sample_rate // 2), n_freqs).astype(f32)
+    m_max = 2595.0 * np.log10(1.0 + (sample_rate // 2) / 700.0)
+    m_pts = np.linspace(0.0, m_max, n_mels + 2).astype(f32)
+    f_pts = f32(700.0) * (f32(10.0) ** (m_pts / f32(2595.0)) - f32(1.0))
+    f_diff = f_pts[1:] - f_pts[:-1]
+    slopes = f_pts[None, :] - all_freqs[:, None]
+    down = -slopes[:, :-2] / f_diff[:-1]
+    up = slopes[:, 2:] / f_diff[1:]
+    return torch.from_numpy(np.maximum(f32(0.0), np.minimum(down, up)).astype(f32))
+
+
+class _MelStft(nn.Module):
+    """Holder of the periodic hann window (`spectrogram.window` of torchaudio.transforms.Spectrogram)."""
+
+    def __init__(self, n_fft: int) -> None:
+        super().__init__()
+        self.register_buffer("window", torch.hann_window(n_fft))
+
+
+class _MelScale(nn.Module):
+    """Holder of the filter bank (`mel_scale.fb` of torchaudio.transforms.MelScale)."""
+
+    def __init__(self, fb: torch.Tensor) -> None:
+        super().__init__()
+        self.register_buffer("fb", fb)
+
+
+class MelSpectrogram(nn.Module):
+    """torchaudio.transforms.MelSpectrogram(sr, n_fft, win_length=n_fft, hop_length, normalized=True, n_mels) as the
+    hybrid configuration binds it (configs/hybrid.gin), fused with what RAVE._mel_encode does next
+    (rave/model.py:238-242): `encode_log1p(x)` = log1p(mel(x)[..., :-1]) reshaped to [B, C * n_mels, frames - 1].
+    Periodic hann window, centred reflect-padded frames, |X|^2 / sum(w^2), HTK bands.  Forward only: the encoder's
+    input needs no gradient.  Same sub-modules / buffers as torchaudio's, so reference checkpoints load."""
+
+    def __init__(self, sample_rate: int, n_fft: int = 2048, win_length: Optional[int] = None,
+                 hop_length: Optional[int] = None, normalized: bool = True, n_mels: int = 128) -> None:
+        super().__init__()
+        if (win_length or n_fft) != n_fft or not normalized:
+            raise NotImplementedError("MelSpectrogram: only win_length = n_fft and normalized=True are on the hot path")
+        self.n_fft, self.hop_length, self.n_mels = n_fft, hop_length or n_fft // 2, n_mels
+        self.spectrogram = _MelStft(n_fft)
+        self.mel_scale = _MelScale(htk_mel_filterbank(sample_rate, n_fft, n_mels))
+
+    def band_table(self):
+        """(band [n_mels, 3] int32 = lo, hi, offset; packed weights) of the current `fb`, on its device; rebuilt only
+        when the buffer changes (load_state_dict), so a captured step reads the same tensors."""
+        fb = self.mel_scale.fb
+        hit = self.__dict__.get("_bands")
+        if hit is not None and hit[0] is fb and hit[1] == fb._version:
+            return hit[2]
+        if fb.is_cuda and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError("MelSpectrogram: run one eager step before capturing a CUDA graph")
+        f = fb.detach().cpu()
+        rows, wts, off = [], [], 0
+        for m in range(f.shape[1]):
+            nz = torch.nonzero(f[:, m]).reshape(-1)
+            lo, hi = (int(nz[0]), int(nz[-1]) + 1) if nz.numel() else (0, 0)
+            rows.append((lo, hi, off))
+            wts.append(f[lo:hi, m])
+            off += hi - lo
+        w = torch.cat(wts) if off else torch.zeros(1)
+        table = (torch.tensor(rows, dtype=torch.int32).to(fb.device), w.contiguous().to(fb.device))
+        self.__dict__["_bands"] = (fb, fb._version, table)
+        return table
+
+    def encode_log1p(self, x: torch.Tensor) -> torch.Tensor:
+        from . import ops
+        batch, channels, T = x.shape
+        w = self.spectrogram.window
+        with torch.no_grad():
+            frames = ops.stft_frames(x.detach().reshape(-1, T), w, self.n_fft, self.hop_length)
+            X = torch.fft.rfft(frames)
+            band, wts = self.band_table()
+            return ops.mel_log1p(X, band, wts, self.n_mels, 1.0 / float(self._win_energy()), batch, channels)
+
+    def _win_energy(self):
+        w = self.spectrogram.window
+        hit = self.__dict__.get("_energy")
+        if hit is None or hit[0] is not w or hit[1] != w._version:
+            hit = self.__dict__["_energy"] = (w, w._version, float(w.detach().double().square().sum().cpu()))
+        return hit[2]
 
 
 class AudioDistanceV1(nn.Module):

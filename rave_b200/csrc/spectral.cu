@@ -285,6 +285,64 @@ extern "C" int rave_spectral_grad(const void *X, const void *Y, void *dY, const 
 }
 
 // ---------------------------------------------------------------------------------------------
+// Mel front end of the hybrid encoder (rave/model.py:238-242 with torchaudio.transforms.MelSpectrogram(normalized=True),
+// configs/hybrid.gin): from the complex STFT X[n][f][k] (n = b*C + c, centred frames, cuFFT),
+//     out[b][c*M + m][f] = log1p( scale * sum_{k in [lo_m, hi_m)} fb_m[k - lo_m] |X[n][f][k]|^2 ),   f < F - 1
+// scale = 1 / sum(w^2).  The HTK filter bank is banded (each band spans a contiguous bin range), so the host passes
+// per-band [lo, hi) and the packed nonzero weights.  One CTA = one signal n and MEL_FT frames: |X|^2 of those frames
+// goes through shared memory, one thread per (band, frame) output.
+// ---------------------------------------------------------------------------------------------
+namespace rave {
+
+constexpr int MEL_FT = 8;
+
+__global__ void __launch_bounds__(256)
+mel_log1p_kernel(const float2 *__restrict__ X, const int *__restrict__ band, const float *__restrict__ wts,
+                 float *__restrict__ out, int F, int bins, int M, int nnz, float scale) {
+  extern __shared__ float sm[];
+  float *P = sm;                          // [MEL_FT][bins]
+  float *W = P + MEL_FT * bins;           // [nnz]
+  int *bd = reinterpret_cast<int *>(W + nnz);   // [M][3]: lo, hi, offset into W
+  const int n = blockIdx.y, f0 = blockIdx.x * MEL_FT;
+  const int Fo = F - 1;                   // the last frame is dropped
+  const int nf = min(MEL_FT, Fo - f0);
+  const float2 *Xn = X + ((size_t)n * F + f0) * bins;
+  for (int i = threadIdx.x; i < nf * bins; i += blockDim.x) {
+    const float2 v = Xn[i];
+    P[i] = fmaf(v.x, v.x, v.y * v.y);
+  }
+  for (int i = threadIdx.x; i < nnz; i += blockDim.x) W[i] = wts[i];
+  for (int i = threadIdx.x; i < 3 * M; i += blockDim.x) bd[i] = band[i];
+  __syncthreads();
+  for (int o = threadIdx.x; o < M * MEL_FT; o += blockDim.x) {
+    const int m = o / MEL_FT, f = o % MEL_FT;
+    if (f >= nf) continue;
+    const int lo = bd[3 * m], hi = bd[3 * m + 1], off = bd[3 * m + 2];
+    const float *p = P + f * bins;
+    float acc = 0.f;
+    for (int k = lo; k < hi; ++k) acc = fmaf(W[off + k - lo], p[k], acc);
+    out[((size_t)n * M + m) * Fo + f0 + f] = log1pf(scale * acc);
+  }
+}
+
+}  // namespace rave
+
+extern "C" int rave_mel_log1p_fwd(const void *X_c64, const int *band, const float *weights, float *out, int N, int F,
+                                  int bins, int M, int nnz, float scale, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(X_c64 && band && weights && out && N > 0 && F > 1 && bins > 0 && M > 0 && nnz > 0 && N <= 65535,
+                 "mel_log1p_fwd: bad argument");
+  const size_t smem = ((size_t)MEL_FT * bins + nnz + 3 * M) * 4;
+  RAVE_CHECK_ARG(smem <= 48 * 1024, "mel_log1p_fwd: %d bins / %d filter weights / %d bands need %zu bytes of shared memory "
+                 "(at most 48 KB)", bins, nnz, M, smem);
+  dim3 grid(ceil_div(F - 1, MEL_FT), N);
+  mel_log1p_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>((const float2 *)X_c64, band, weights, out, F, bins, M, nnz,
+                                                             scale);
+  RAVE_CHECK_LAUNCH("mel_log1p_fwd");
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // NoiseGeneratorV2 tail (rave/blocks.py:284-292, rave/core.py:20-21,48-81): band amplitudes -> FIR -> filtered
 // uniform noise, in ONE kernel.  The reference goes mod_sigmoid -> irfft -> roll -> hann -> pad/crop -> roll
 // (amp_to_impulse_response) and then a zero-padded rfft * rfft -> irfft (fft_convolve): 4 FFT launches and ~15

@@ -103,12 +103,23 @@ def chain_supported(specs: List[LayerSpec]) -> bool:
 # planning: walk a module list into LayerSpecs
 # ----------------------------------------------------------------------------------------------
 
+def split_recurrent(mods: List[nn.Module]):
+    """(leading blocks.GRU or None, the modules after it): GeneratorV2's `recurrent_layer` (configs/hybrid.gin) opens
+    its sequence; it runs on its own kernels (ops.gru) and the rest of the sequence is planned as a chain."""
+    from . import blocks
+    if mods and isinstance(mods[0], blocks.GRU):
+        return mods[0], mods[1:]
+    return None, mods
+
+
 def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
     """EncoderV2.net / GeneratorV2.net style sequences: activations (LeakyReLU or Snake), cc.Conv1d, cc.ConvTranspose1d,
     Residual(DilatedUnit), AdaIN (identity in training).  Returns None if something is unsupported.
     Snake (v3): the producer writes its pre-activation as bf16, a channel-last Snake kernel turns it into the next conv's
-    operand (and keeps the raw stream for the backward and for the unit's skip)."""
+    operand (and keeps the raw stream for the backward and for the unit's skip).
+    A leading GRU is not part of the plan (split_recurrent): the caller runs it first."""
     from . import blocks, cc
+    mods = split_recurrent(list(mods))[1]
     specs: List[LayerSpec] = []
     NONE = (ops.ACT_NONE, 0.0, None)
     pending = NONE

@@ -215,12 +215,14 @@ class RAVE(nn.Module):
         if self.input_mode == "pqmf":
             x_enc = _pqmf_encode(self.pqmf, x_enc)
         elif self.input_mode == "mel":
-            raise NotImplementedError("mel input is not on the hot path")
+            x_enc = self.spectrogram.encode_log1p(x)          # rave/model.py:238-242
         z = self.encoder(x_enc)
         if return_mb:
             if self.input_mode == "pqmf":
                 return z, x_enc
-            return z, _pqmf_encode(self.pqmf, x_enc)
+            # quirk D9 (SURVEY.md): the reference analyses x_enc, i.e. the mel spectrogram in mel mode, which its own
+            # multiband distance cannot take; the multiband target is the PQMF analysis of the waveform
+            return z, _pqmf_encode(self.pqmf, x if self.input_mode == "mel" else x_enc)
         return z
 
     def decode(self, z):

@@ -1164,3 +1164,87 @@ def weight_norm_bwd_multi(items):
                     L.tapsA[k] = sl
         call("rave_weight_norm_bwd_multi", len(chunk), arr, stream_ptr())
     return outs
+
+
+# ----------------------------------------------------------------------------------------------
+# hybrid configuration: mel front end, GRU
+# ----------------------------------------------------------------------------------------------
+
+def mel_log1p(X, band, weights, n_mels, scale, batch, channels):
+    """log1p(scale * |X|^2 @ fb) of the complex STFT X [B*C, F, bins], last frame dropped -> [B, C*n_mels, F-1]
+    (rave_mel_log1p_fwd; forward only).  `band` [n_mels, 3] int32 (lo, hi, offset into `weights`)."""
+    N, F, bins = X.shape
+    X = X.contiguous()
+    out = torch.empty(batch, channels * n_mels, F - 1, dtype=torch.float32, device=X.device)
+    call("rave_mel_log1p_fwd", ptr(torch.view_as_real(X)), ptr(band), ptr(weights), ptr(out), N, F, bins, n_mels,
+         weights.numel(), float(scale), stream_ptr())
+    return out
+
+
+def _dptr(t, offset=0):
+    """Device pointer of contiguous fp32 `t` plus `offset` elements."""
+    return ptr(t) + 4 * offset
+
+
+def gemm_f32(A, sam, sak, Bm, sbk, sbn, M, N, K, out, ldc, bias=None, rowsum=None, a_off=0, b_off=0):
+    """out[m][n] = sum_k A(m, k) B(k, n) (+ bias[n]) over element strides (rave_gemm_f32); rowsum[m] = sum_k A(m, k)."""
+    S = int(_lib.load().rave_gemm_f32_splits(M, N, K))
+    ws = torch.empty(S * (M * N + M), dtype=torch.float32, device=out.device) if S > 1 else None
+    call("rave_gemm_f32", _dptr(A, a_off), sam, sak, _dptr(Bm, b_off), sbk, sbn, ptr(bias), ptr(out), ldc, ptr(rowsum),
+         M, N, K, ptr(ws), S, stream_ptr())
+
+
+class GruLayerFn(torch.autograd.Function):
+    """One nn.GRU layer (batch_first, h0 = 0) on x [B, T, I]: the input projection for all t as one GEMM, the recurrence
+    as one persistent launch (rave_gru_fwd); backward = the reverse-time recurrence (rave_gru_bwd) producing the gate
+    gradients, then dx, dW_ih, dW_hh and both bias gradients as GEMMs over the B*T rows."""
+
+    @staticmethod
+    def forward(ctx, x, w_ih, w_hh, b_ih, b_hh):
+        x, w_ih, w_hh, b_ih, b_hh = (_f32c(t) for t in (x, w_ih, w_hh, b_ih, b_hh))
+        B, T, I = x.shape
+        G, H = w_hh.shape
+        gi = torch.empty(B, T, G, dtype=torch.float32, device=x.device)
+        gemm_f32(x, I, 1, w_ih, 1, I, B * T, G, I, gi, G, bias=b_ih)
+        h = torch.empty(B, T, H, dtype=torch.float32, device=x.device)
+        need = any(ctx.needs_input_grad)
+        save = torch.empty(B, T, 5, H, dtype=torch.float32, device=x.device) if need else None
+        call("rave_gru_fwd", ptr(gi), ptr(w_hh), ptr(b_hh), ptr(h), ptr(save), B, T, H, stream_ptr())
+        if need:
+            ctx.save_for_backward(x, w_ih, w_hh, save)
+        return h
+
+    @staticmethod
+    def backward(ctx, dh):
+        x, w_ih, w_hh, save = ctx.saved_tensors
+        B, T, I = x.shape
+        G, H = w_hh.shape
+        dh = _f32c(dh)
+        dgi = torch.empty(B, T, G, dtype=torch.float32, device=x.device)
+        dgh = torch.empty(B, T, G, dtype=torch.float32, device=x.device)
+        call("rave_gru_bwd", ptr(dh), ptr(save), ptr(w_hh), ptr(dgi), ptr(dgh), B, T, H, stream_ptr())
+        dx = dw_ih = dw_hh = db_ih = db_hh = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty(B, T, I, dtype=torch.float32, device=x.device)
+            gemm_f32(dgi, G, 1, w_ih, I, 1, B * T, I, G, dx, I)
+        if any(ctx.needs_input_grad[1:]):
+            dw_ih = torch.empty(G, I, dtype=torch.float32, device=x.device)
+            dw_hh = torch.empty(G, H, dtype=torch.float32, device=x.device)
+            db_ih = torch.empty(G, dtype=torch.float32, device=x.device)
+            db_hh = torch.empty(G, dtype=torch.float32, device=x.device)
+            gemm_f32(dgi, 1, G, x, I, 1, G, I, B * T, dw_ih, I, rowsum=db_ih)
+            gemm_f32(dgh, 1, G, save, 5 * H, 1, G, H, B * T, dw_hh, H, rowsum=db_hh, b_off=4 * H)   # h_prev slot
+        return dx, dw_ih, dw_hh, db_ih, db_hh
+
+
+def gru(x, rnn):
+    """nn.GRU(batch_first=True) `rnn` applied to channel-first x [B, C, T] -> [B, H, T] (rave/blocks.py:308-313), one
+    GruLayerFn per layer.  fp32 in every precision mode: the recurrence compounds rounding."""
+    if (not rnn.batch_first or rnn.bidirectional or not rnn.bias or rnn.proj_size or
+            (rnn.dropout and rnn.training and rnn.num_layers > 1)):
+        raise _lib.RaveB200Error("gru: only unidirectional, biased, batch-first nn.GRU without dropout is on the hot path")
+    h = x.transpose(1, 2).contiguous()
+    for l in range(rnn.num_layers):
+        h = GruLayerFn.apply(h, getattr(rnn, f"weight_ih_l{l}"), getattr(rnn, f"weight_hh_l{l}"),
+                             getattr(rnn, f"bias_ih_l{l}"), getattr(rnn, f"bias_hh_l{l}"))
+    return h.transpose(1, 2)
