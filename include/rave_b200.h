@@ -173,8 +173,9 @@ int rave_dilated_unit_tc_supported(int C, int L);
 int rave_dilated_unit_tc_fwd(const void *xa_bf16, const void *w3t_bf16, const void *w1t_bf16, void *a1_out,
                              float *out_f32, void *out_act, int B, int C, int L, int pitch, int dil, int pad_l,
                              float slope_in, float slope_mid, int act_out, float slope_out, void *stream);
-/* kernel instance rave_conv1d_tc_fwd selects for a shape: BLOCK_N | BLOCK_K << 12, 0 = none
- * (bench.py names the dominant kernel with it) */
+/* kernel instance rave_conv1d_tc_fwd selects for a shape (a launch that writes out_act): BLOCK_N | BLOCK_K << 12 |
+ * (accumulator buffers - 1) << 24 | (bf16 output staged in shared memory, written by TMA) << 25 | ring stages << 26;
+ * 0 = none (bench.py names the dominant kernel with it) */
 int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K);
 int rave_conv1d_tc_fwd(const void *xa_bf16, const void *wt_bf16, const float *bias, const float *res,
                        const void *res_bf16, const void *dact_src_bf16, const void *res_act_bf16, float res_slope,

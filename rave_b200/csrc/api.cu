@@ -18,7 +18,7 @@ void set_error(const char *fmt, ...) {
 void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memory_order_relaxed); }
 }  // namespace rave
 
-extern "C" int rave_b200_version(void) { return 104; }
+extern "C" int rave_b200_version(void) { return 105; }
 extern "C" const char *rave_b200_last_error(void) { return rave::g_err; }
 extern "C" unsigned long long rave_b200_launch_count(void) {
   return rave::g_launches.load(std::memory_order_relaxed);

@@ -10,7 +10,9 @@
 // the canonical K-major swizzled layout (row = one swizzle span = BLOCK_K*2 bytes).  One warpgroup issues the
 // wgmma of a 128-row tile (two m64 halves) and keeps the accumulators in registers; a finished tile goes to a
 // shared-memory buffer from which the epilogue (bias, residual, dual write of the pre-activation fp32 stream and the
-// bf16 activated operand of the NEXT conv) reads it row by row while the warpgroup already runs the next tile.
+// bf16 activated operand of the NEXT conv) reads it row by row while the warpgroup already runs the next tile.  Where
+// shared memory allows (plan_smem) there are two such buffers, and the bf16 rows go to a swizzled staging tile that one
+// epilogue thread writes out with TMA tensor stores.
 // Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
@@ -53,6 +55,10 @@ struct TcParams {
                            // Cout, or 2*Cout in x3 mode
   int act_cs;              // x3: channels per POSITION of an output row (Cout; Cout/stride when the row holds the phases
                            // of a transposed conv side by side): column n = q*cs + c lives at q*2cs + c (hi), +cs (lo)
+  // shared-memory split of this launch (plan_smem): ring stages, accumulator buffers, bf16 output staging tile
+  int stages, nacc;
+  int stg;                 // 1: out_act rows go through the staging tile and leave by TMA tensor stores
+  int acc_off, stg_off, bar_off;
 };
 
 template <int BLOCK_N, int BLOCK_K, bool X3 = false>
@@ -66,13 +72,48 @@ struct SmemLayout {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES_PAD;
   static constexpr int ACC_LD = acc_pitch(BLOCK_N);
   static constexpr int ACC_BYTES = BLOCK_M * ACC_LD * 4;                 // fp32 accumulator hand-over buffer
-  static constexpr int MAX_STAGES = (SMEM_MAX - ACC_BYTES - 256 - 1024) / STAGE_BYTES;
-  static constexpr int STAGES = MAX_STAGES > 8 ? 8 : MAX_STAGES;
-  static constexpr int ACC_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFFSET = ACC_OFFSET + ACC_BYTES;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;  // + barriers + alignment slack
-  static_assert(STAGES >= 2, "not enough shared memory for a 2-stage pipeline");
+  // bf16 output staging tile: BLOCK_N / OUT_BOXC boxes of [128 rows][OUT_BOXC channels], each row one swizzle span
+  static constexpr int OUT_BOXC = BLOCK_N % 64 == 0 ? 64 : BLOCK_N % 32 == 0 ? 32 : 16;
+  static constexpr int OUT_SPAN = OUT_BOXC * 2;
+  static constexpr int STG_BYTES = X3 ? 0 : BLOCK_M * BLOCK_N * 2;      // x3 rows ([hi | lo] pairs) keep direct stores
+  static constexpr int FIXED = 256 + 1024;                              // barriers + alignment slack
+  static constexpr int stages_for(int nacc, int stg) {
+    const int s = (SMEM_MAX - FIXED - nacc * ACC_BYTES - stg * STG_BYTES) / STAGE_BYTES;
+    return s > 8 ? 8 : s;
+  }
 };
+
+// Shared-memory split of one launch.  The ring depth the single-buffer layout gives (at most 8) is what the main loop
+// needs when a tile has many k-blocks; a tile of kblocks k-blocks cannot use more than kblocks + 1 stages.  The first
+// layout that keeps min(that depth, kblocks + 1) stages wins, in this order: two accumulator buffers + the output
+// staging tile (the MMA warpgroup hands over a tile without waiting for the epilogue of the previous one; bf16 rows leave
+// by TMA), one buffer + staging, one buffer alone (the direct-store epilogue).
+template <int BLOCK_N, int BLOCK_K, bool X3>
+static void plan_smem(int kblocks, TcParams &p) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
+  const int base = L::stages_for(1, 0);
+  const int need = kblocks + 1 < base ? kblocks + 1 : base;
+  p.nacc = 1;
+  p.stg = 0;
+  if (L::stages_for(2, 1) >= need) { p.nacc = 2; p.stg = 1; }
+  else if (L::stages_for(1, 1) >= need) p.stg = 1;
+  if (X3) p.stg = 0;
+  p.stages = L::stages_for(p.nacc, p.stg);
+  p.acc_off = p.stages * L::STAGE_BYTES;
+  p.stg_off = p.acc_off + p.nacc * L::ACC_BYTES;
+  p.bar_off = p.stg_off + p.stg * L::STG_BYTES;
+}
+
+// Byte offset of the 16-byte piece holding channels c .. c + 7 of tile row `row` in the output staging tile: the
+// canonical swizzle TMA applies to a box whose rows are one SPAN-byte swizzle span (16-byte piece index XOR address
+// bits 7..): the 8 rows one quarter-warp writes land in 8 different bank groups.
+template <int BOXC>
+__device__ __forceinline__ uint32_t stg_offset(int row, int c) {
+  constexpr int SPAN = BOXC * 2;
+  const uint32_t line = (uint32_t)row * SPAN;
+  const uint32_t piece = (uint32_t)((c % BOXC) >> 3) ^ ((line >> 7) & (SPAN / 16 - 1));
+  return (uint32_t)(c / BOXC) * (BLOCK_M * SPAN) + line + (piece << 4);
+}
 
 // Epilogue of one 128 x BLOCK_N accumulator tile: this thread owns row (taddr >> 16) + lane of the accumulator buffer.
 // One chunk = CW (16 or 32) consecutive channels.  All global loads of the chunk (residual, gradient skip,
@@ -93,9 +134,10 @@ __device__ __forceinline__ void st_words(void *ptr, const uint32_t *w) {
 __device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
 
-template <int CW, bool X3>
+// stg (or null): the output staging tile; out_act then goes there (tile row `row`, channel co - n0) instead of to HBM
+template <int CW, bool X3, int BOXC>
 __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, int co, bool valid, size_t orow,
-                                             int fm_side = 0) {
+                                             int fm_side, uint8_t *stg, int row, int cl) {
   constexpr int NW = CW / 2;      // 32-bit words of a bf16 row segment
   float v[CW];
   uint32_t rf[CW], rb[NW], dm[NW], ra[NW], ra2[X3 ? NW : 1], pm[NW];
@@ -195,44 +237,50 @@ __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, 
         pl[w] = *reinterpret_cast<uint32_t *>(&l);
       }
     }
-    st_words<NW>(p.out_act + offa, pk);
-    if (X3) st_words<NW>(p.out_act + offa + cs, pl);
+    if (!X3 && stg) {
+#pragma unroll
+      for (int j = 0; j < NW / 4; ++j) sts128(stg + stg_offset<BOXC>(row, cl + 8 * j), pk + 4 * j);
+    } else {
+      st_words<NW>(p.out_act + offa, pk);
+      if (X3) st_words<NW>(p.out_act + offa + cs, pl);
+    }
   }
 }
 
-template <int BLOCK_N, bool X3>
+template <int BLOCK_N, bool X3, int BOXC>
 __device__ __forceinline__ void tc_epilogue(const TcParams &p, uint32_t taddr, int n0, bool valid, size_t orow,
-                                            int fm_side) {
+                                            int fm_side, uint8_t *stg, int row) {
   constexpr int MAIN = BLOCK_N / 32 * 32;
   if (X3 && (p.act_cs & 31)) {
     // split-operand rows whose positions are 16 (mod 32) channels wide (capacity-48 transposed convs: 48 channels per
     // position): a 32-column chunk would straddle a [hi | lo] boundary -> 16-column chunks
 #pragma unroll 1
     for (int c0 = 0; c0 < BLOCK_N; c0 += 16)
-      tc_epi_chunk<16, X3>(p, taddr + c0, n0 + c0, valid, orow, fm_side);
+      tc_epi_chunk<16, X3, BOXC>(p, taddr + c0, n0 + c0, valid, orow, fm_side, stg, row, c0);
     return;
   }
 #pragma unroll 1
   for (int c0 = 0; c0 < MAIN; c0 += 32)
-    tc_epi_chunk<32, X3>(p, taddr + c0, n0 + c0, valid, orow, fm_side);
-  if (MAIN < BLOCK_N) tc_epi_chunk<16, X3>(p, taddr + MAIN, n0 + MAIN, valid, orow, fm_side);
+    tc_epi_chunk<32, X3, BOXC>(p, taddr + c0, n0 + c0, valid, orow, fm_side, stg, row, c0);
+  if (MAIN < BLOCK_N) tc_epi_chunk<16, X3, BOXC>(p, taddr + MAIN, n0 + MAIN, valid, orow, fm_side, stg, row, MAIN);
 }
 
 template <int BLOCK_N, int BLOCK_K, bool X3>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-               const TcParams p) {
+               const __grid_constant__ CUtensorMap tmap_o, const TcParams p) {
   using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
-  constexpr int STAGES = L::STAGES;
+  const int STAGES = p.stages;
   constexpr int SWZ = BLOCK_K * 2;
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + L::BAR_OFFSET);
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + p.bar_off);
   uint64_t *empty_bar = full_bar + STAGES;
-  uint64_t *tfull_bar = empty_bar + STAGES;      // MMA warpgroup -> epilogue: the accumulator buffer holds a tile
-  uint64_t *tempty_bar = tfull_bar + 1;          // epilogue -> MMA warpgroup: the buffer has been read
+  uint64_t *tfull_bar = empty_bar + STAGES;      // MMA warpgroup -> epilogue: accumulator buffer b holds a tile
+  uint64_t *tempty_bar = tfull_bar + 2;          // epilogue -> MMA warpgroup: buffer b has been read
+  uint8_t *stg = (!X3 && p.stg) ? smem + p.stg_off : nullptr;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -242,14 +290,17 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_a);
     tma_prefetch_desc(&tmap_b);
+    if (stg) tma_prefetch_desc(&tmap_o);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 4);               // one arrival per MMA warp
     }
-    mbar_init(tfull_bar, 128);
-    mbar_init(tempty_bar, 4);
+    for (int b = 0; b < 2; ++b) {
+      mbar_init(&tfull_bar[b], 128);
+      mbar_init(&tempty_bar[b], 4);
+    }
     fence_barrier_init();
-    acc_bind(smem + L::ACC_OFFSET, L::ACC_LD);
+    acc_bind(smem + p.acc_off, L::ACC_LD);       // nacc buffers back to back: buffer b = rows 128 b ..
   }
   __syncthreads();
   griddep_launch_dependents();      // dependents may begin their prologue ...
@@ -343,14 +394,18 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       wgmma_fence_regs<BLOCK_N / 2>(d[1]);
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[prev]);              // the last k-block's slot
-      mbar_wait(tempty_bar, (it & 1) ^ 1);                       // the epilogue has read the previous tile
-      acc_store<BLOCK_N>(d, threadIdx.x);
-      mbar_arrive(tfull_bar);
+      const int buf = p.nacc == 2 ? (it & 1) : 0;
+      const uint32_t use = p.nacc == 2 ? (it >> 1) : it;         // earlier tiles handed over through this buffer
+      mbar_wait(&tempty_bar[buf], (use & 1) ^ 1);                // the epilogue has read the buffer's previous tile
+      acc_store<BLOCK_N>(d, threadIdx.x, 0, 128 * buf);
+      mbar_arrive(&tfull_bar[buf]);
     }
   } else {
     // =========================== epilogue (4 warps) ===========================
+    constexpr int BOXC = L::OUT_BOXC;
     const int quad = warp & 3;           // rows quad * 32 .. quad * 32 + 31 of the tile
     const int row = quad * 32 + lane;    // row of the 128-row tile
+    const bool issuer = threadIdx.x == 160;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int nt = tile % p.n_nt;
@@ -363,12 +418,30 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
       const bool valid = (b < p.B) && (l < p.Lout);
       const size_t orow = (size_t)b * p.out_rows + (size_t)l * p.out_row_stride + p.out_row_offset;
 
-      mbar_wait(tfull_bar, it & 1);
-      const uint32_t taddr = (uint32_t)(quad * 32) << 16;
-      tc_epilogue<BLOCK_N, X3>(p, taddr, n0, valid, orow, p.fm_d ? (b < p.fm_bh ? 1 : -1) : 0);
+      const int buf = p.nacc == 2 ? (it & 1) : 0;
+      const uint32_t use = p.nacc == 2 ? (it >> 1) : it;
+      if (stg) {                         // the previous tile's tensor stores have read the staging tile
+        if (issuer) bulk_wait_read<0>();
+        named_bar_sync(1, 128);
+      }
+      mbar_wait(&tfull_bar[buf], use & 1);
+      const uint32_t taddr = (uint32_t)(128 * buf + quad * 32) << 16;
+      tc_epilogue<BLOCK_N, X3, BOXC>(p, taddr, n0, valid, orow, p.fm_d ? (b < p.fm_bh ? 1 : -1) : 0, stg, row);
       __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar);
+      if (lane == 0) mbar_arrive(&tempty_bar[buf]);
+      if (stg) {
+        // rows past Lout and batches past B fall outside the tensor map and are not written
+        fence_proxy_async();             // generic-proxy shared-memory writes -> TMA
+        named_bar_sync(1, 128);
+        if (issuer) {
+#pragma unroll
+          for (int c = 0; c < BLOCK_N; c += BOXC)
+            tma_store_3d(&tmap_o, stg + (c / BOXC) * (BLOCK_M * L::OUT_SPAN), n0 + c, lt * p.BL, bg * p.BB);
+          bulk_commit();
+        }
+      }
     }
+    if (stg && issuer) bulk_wait_all();
   }
 }
 
@@ -422,24 +495,44 @@ static int pick_block_n(int Cout, long m_tiles) {
 }
 
 template <int BN, int BK, bool X3>
-static int launch(const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t stream) {
+static int launch(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cudaStream_t stream) {
   using L = SmemLayout<BN, BK, X3>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, BK, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::TOTAL);
+  plan_smem<BN, BK, X3>(p.K * p.num_kb, p);
+  if (!p.out_act) p.stg = 0;
+  const int smem = p.bar_off + L::FIXED;
+  static int attr = 0;              // dynamic shared memory this instance has been allowed so far
+  if (smem > attr) {
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, BK, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) {
-      set_error("conv1d_tc: cudaFuncSetAttribute(%d bytes): %s", L::TOTAL, cudaGetErrorString(e));
+      set_error("conv1d_tc: cudaFuncSetAttribute(%d bytes): %s", smem, cudaGetErrorString(e));
       return 2;
     }
-    attr = true;
+    attr = smem;
+  }
+  CUtensorMap to;
+  memset(&to, 0, sizeof(to));
+  if (p.stg) {
+    // bf16 output rows (c, l, b) over [B][out_rows][Cout] from row out_row_offset on: row l of batch b is
+    // b * out_rows + l * out_row_stride + out_row_offset; the extents Lout and B clip the rows of a ragged tile
+    EncodeTiledFn enc = get_encode_fn();
+    cuuint64_t dims[3] = {(cuuint64_t)p.Cout, (cuuint64_t)p.Lout, (cuuint64_t)p.B};
+    cuuint64_t strides[2] = {(cuuint64_t)p.Cout * 2 * p.out_row_stride, (cuuint64_t)p.Cout * 2 * p.out_rows};
+    cuuint32_t box[3] = {(cuuint32_t)L::OUT_BOXC, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(&to, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.out_act + (size_t)p.out_row_offset * p.Cout, dims,
+                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(L::OUT_SPAN),
+                     CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+      set_error("conv1d_tc: output tensor map encode failed (%d)", (int)r);
+      return 1;
+    }
   }
   const int tiles = p.n_lt * p.n_bg * p.n_nt;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int grid = tiles < sms ? tiles : sms;
-  launch_pdl(conv_tc_kernel<BN, BK, X3>, dim3(grid), dim3(NUM_THREADS), L::TOTAL, stream, ta, tb, p);
+  launch_pdl(conv_tc_kernel<BN, BK, X3>, dim3(grid), dim3(NUM_THREADS), smem, stream, ta, tb, to, p);
   RAVE_CHECK_LAUNCH("conv1d_tc");
   return 0;
 }
@@ -457,6 +550,22 @@ static int dispatch_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, cons
   }
   set_error("conv1d_tc: no kernel for BLOCK_N=%d", bn);
   return 1;
+}
+
+// shared-memory split rave_conv1d_tc_plan reports (a launch that writes out_act)
+template <int BK>
+static int smem_plan_bits(int BN, int kblocks) {
+  TcParams q;
+  switch (BN) {
+    case 128: plan_smem<128, BK, false>(kblocks, q); break;
+    case 96: plan_smem<96, BK, false>(kblocks, q); break;
+    case 64: plan_smem<64, BK, false>(kblocks, q); break;
+    case 48: plan_smem<48, BK, false>(kblocks, q); break;
+    case 32: plan_smem<32, BK, false>(kblocks, q); break;
+    case 16: plan_smem<16, BK, false>(kblocks, q); break;
+    default: return 0;
+  }
+  return (q.nacc - 1) << 24 | q.stg << 25 | q.stages << 26;
 }
 
 template <bool X3>
@@ -490,7 +599,8 @@ extern "C" int rave_conv1d_tc_supported(int Cin, int Cout, int K, int stride, in
   return 1;
 }
 
-// Which kernel instance rave_conv1d_tc_fwd runs for a shape: BLOCK_N | BLOCK_K << 12; 0 = none.
+// Which kernel instance rave_conv1d_tc_fwd runs for a shape (writing out_act): BLOCK_N | BLOCK_K << 12 |
+// (accumulator buffers - 1) << 24 | staged output << 25 | ring stages << 26; 0 = none.
 extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
   using namespace rave;
   using namespace rave::tc;
@@ -501,7 +611,10 @@ extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
   const long m_tiles = (long)ceil_div(Lout, BL) * ceil_div(B, 128 / BL);
   const int BN = pick_block_n(Cout, m_tiles);
   if (!BN) return 0;
-  return BN | (BK << 12);
+  const int kblocks = K * ceil_div(Cin, BK);
+  const int smem = BK == 64 ? smem_plan_bits<64>(BN, kblocks)
+                 : BK == 32 ? smem_plan_bits<32>(BN, kblocks) : smem_plan_bits<16>(BN, kblocks);
+  return BN | (BK << 12) | smem;
 }
 
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,

@@ -178,14 +178,15 @@ __device__ __forceinline__ void acc_bind(const void *buf, int ld) {    // one th
   s_acc_ld = (uint32_t)ld;
 }
 // store the warpgroup's accumulators of a 128 x N tile (wgmma fragment: d[4j + {0,1}] at row 16 warp + lane / 4,
-// columns 8 j + 2 (lane % 4) + {0,1}; d[4j + {2,3}] eight rows further down) at column `col0` of the buffer
+// columns 8 j + 2 (lane % 4) + {0,1}; d[4j + {2,3}] eight rows further down) at column `col0` and row `row0` of the
+// buffer (row0 = 128: the second of two accumulator buffers bound back to back)
 template <int N>
-__device__ __forceinline__ void acc_store(const float (*d)[N / 2], int wg_thread, int col0 = 0) {
+__device__ __forceinline__ void acc_store(const float (*d)[N / 2], int wg_thread, int col0 = 0, int row0 = 0) {
   const int w = wg_thread >> 5, l = wg_thread & 31;
   const uint32_t ld = s_acc_ld;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    const uint32_t r0 = (uint32_t)(64 * h + 16 * w + (l >> 2));
+    const uint32_t r0 = (uint32_t)(row0 + 64 * h + 16 * w + (l >> 2));
 #pragma unroll
     for (int j = 0; j < N / 8; ++j) {
       const uint32_t c = (uint32_t)(col0 + 8 * j + 2 * (l & 3));
