@@ -13,7 +13,8 @@
 // bf16 activated operand of the NEXT conv) reads it row by row while the warpgroup already runs the next tile.  Where
 // shared memory allows (plan_smem) there are two such buffers, and the bf16 rows go to a swizzled staging tile that one
 // epilogue thread writes out with TMA tensor stores.
-// Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.
+// Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.  The input-gradient launches (LeakyReLU' mask,
+// bf16 out only) run conv_tc_pp_kernel instead: two MMA warpgroups in ping-pong, epilogue from registers.
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
@@ -59,6 +60,7 @@ struct TcParams {
   int stages, nacc;
   int stg;                 // 1: out_act rows go through the staging tile and leave by TMA tensor stores
   int acc_off, stg_off, bar_off;
+  int ops_off, ops_bytes;  // ping-pong dgrad kernel: the two epilogue operand slots (plan_smem_pp)
 };
 
 template <int BLOCK_N, int BLOCK_K, bool X3 = false>
@@ -445,6 +447,258 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   }
 }
 
+// =============================================================================================
+// Ping-pong dgrad kernel.  The launches whose epilogue applies the LeakyReLU' mask (dact_src), optionally with the fused
+// feature-matching term and the bf16 gradient skip, and writes bf16 only (the input gradients of every chain) read up
+// to three operand tiles per output tile; in conv_tc_kernel that epilogue is as long as the main loop and the MMAs wait
+// for it.  Here two MMA warpgroups take alternate tiles of the persistent loop: each runs a whole 128 x BLOCK_N tile
+// (the same wgmma sequence as conv_tc_kernel) and then its epilogue straight from its accumulator registers while the
+// other one runs its main loop; an ordering barrier pair hands the tensor pipe from one warpgroup to the other.  When
+// the producer starts a tile it also loads the tile's epilogue operands with TMA into that warpgroup's operand slot,
+// on a barrier of their own, so they land during the main loop; the bf16 result replaces the mask in the slot (same
+// swizzled position) and leaves by TMA tensor stores.
+// Warp roles: warpgroup 0 = TMA producer (warp 0; warps 1-3 leave after giving their registers back), warpgroups 1
+// and 2 = MMA + epilogue.
+// =============================================================================================
+constexpr int PP_THREADS = 384;
+
+// Epilogue of one tile from the accumulator registers of warpgroup thread (w, lane).  slot = [mask | partner (FM) |
+// gradient skip (RS)] tiles, each BLOCK_N / BOXC boxes of [128 rows][BOXC channels] in the canonical swizzle.  Per
+// element the same fp32 sequence as tc_epi_chunk: mask, feature-matching term, skip, one rounding to bf16.
+template <int BLOCK_N, int BOXC, bool FM, bool RS>
+__device__ __forceinline__ void pp_epilogue(float (*d)[BLOCK_N / 2], uint8_t *slot, const TcParams &p, int w, int lane,
+                                            int b0) {
+  constexpr int TILE_BYTES = BLOCK_M * BLOCK_N * 2;
+  uint8_t *part = slot + TILE_BYTES;
+  uint8_t *skip = slot + (FM ? 2 : 1) * TILE_BYTES;
+  constexpr int SPAN = BOXC * 2, JB = BOXC / 8;          // 16-byte pieces per box row
+  const float d0 = FM ? __ldg(p.fm_d) : 0.f, d1 = FM ? __ldg(p.fm_d + 1) : 0.f;
+  // wgmma fragment: d[h][4 j + 2 r + {0, 1}] = row 64 h + 16 w + lane / 4 + 8 r, columns 8 j + 2 (lane % 4) + {0, 1}.
+  // The four rows of a thread are 8 apart, so they share the swizzle (piece index XOR row bits that a multiple of 8
+  // rows does not change): the word of column 8 j + 2 (lane % 4) sits at base ^ (j % JB) << 4, plus a whole box per
+  // JB pieces and a constant per row -- JB registers of addresses instead of one per element.
+  const uint32_t base = stg_offset<BOXC>(16 * w + (lane >> 2), 0) + 4 * (lane & 3);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = 64 * h + 16 * w + (lane >> 2) + 8 * r;
+      const float d1r = (FM && b0 + row / p.BL < p.fm_bh) ? d1 : 0.f;     // d1 sgn(a_r) on real rows only
+#pragma unroll
+      for (int j = 0; j < BLOCK_N / 8; ++j) {
+        const uint32_t off = (base ^ (uint32_t)((j % JB) << 4)) + (j / JB) * (BLOCK_M * SPAN) + (64 * h + 8 * r) * SPAN;
+        float v0 = d[h][4 * j + 2 * r], v1 = d[h][4 * j + 2 * r + 1];
+        const uint32_t dm = *reinterpret_cast<const uint32_t *>(slot + off);
+        if (dm & 0x00008000u) v0 *= p.slope;
+        if (dm & 0x80000000u) v1 *= p.slope;
+        if (FM) {
+          const uint32_t pm = *reinterpret_cast<const uint32_t *>(part + off);
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const float as = e ? bf_hi(dm) : bf_lo(dm);
+            const float ap = e ? bf_hi(pm) : bf_lo(pm);
+            const float t = (as > ap ? 1.f : 0.f) - (as < ap ? 1.f : 0.f);
+            const float sr = (as > 0.f ? 1.f : 0.f) - (as < 0.f ? 1.f : 0.f);
+            float &v = e ? v1 : v0;
+            v = fmaf(d1r, sr, fmaf(d0, t, v));
+          }
+        }
+        if (RS) {
+          const uint32_t rb = *reinterpret_cast<const uint32_t *>(skip + off);
+          v0 += bf_lo(rb);
+          v1 += bf_hi(rb);
+        }
+        __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        *reinterpret_cast<uint32_t *>(slot + off) = *reinterpret_cast<uint32_t *>(&o);
+      }
+    }
+  }
+}
+
+// FM, RS: fm_d, res_bf16 set.  One instance per operand set: the epilogue compiled once for run-time flags made the
+// v2 step slower (DESIGN section 5.3).
+template <int BLOCK_N, int BLOCK_K, bool FM, bool RS>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_m, const __grid_constant__ CUtensorMap tmap_p,
+                  const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o,
+                  const TcParams p) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, false>;
+  constexpr int BOXC = L::OUT_BOXC;
+  constexpr int BOX_BYTES = BLOCK_M * L::OUT_SPAN;          // one [128 rows][BOXC channels] box
+  constexpr int TILE_BYTES = BLOCK_M * BLOCK_N * 2;         // one operand tile
+  constexpr int SWZ = BLOCK_K * 2;
+  const int STAGES = p.stages;
+  static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + p.bar_off);
+  uint64_t *empty_bar = full_bar + STAGES;
+  uint64_t *ofull_bar = empty_bar + STAGES;      // producer -> warpgroup c: its operand slot holds the tile's operands
+  uint64_t *oempty_bar = ofull_bar + 2;          // warpgroup c -> producer: the tensor stores have read the slot
+  uint64_t *order_bar = oempty_bar + 2;          // warpgroup 1 - c -> c: c may issue its main loop
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_tiles = p.n_lt * p.n_bg * p.n_nt;
+  const int kblocks = p.K * p.num_kb;
+  constexpr bool fm = FM, rs = RS;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_m);
+    tma_prefetch_desc(&tmap_o);
+    if (fm) tma_prefetch_desc(&tmap_p);
+    if (rs) tma_prefetch_desc(&tmap_r);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);               // one arrival per MMA warp of the consuming warpgroup
+    }
+    for (int c = 0; c < 2; ++c) {
+      mbar_init(&ofull_bar[c], 1);
+      mbar_init(&oempty_bar[c], 1);
+      mbar_init(&order_bar[c], 4);
+    }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch_dependents();
+  griddep_wait();
+
+  if (wg == 0) {
+    // =========================== TMA producer (warp-uniform loop, elected lane issues) ===========================
+    warpgroup_reg_dealloc<56>();
+    if (warp != 0) return;
+    int stage = 0;
+    uint32_t phase = 0;
+    int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
+      const int nt = tile % p.n_nt;
+      const int mt = tile / p.n_nt;
+      const int lt = mt % p.n_lt;
+      const int bg = mt / p.n_lt;
+      const int l0 = lt * p.BL;
+      const int b0 = bg * p.BB;
+      const int n0 = nt * BLOCK_N;
+      const int c = it & 1;                        // consumer warpgroup of this tile
+      for (int k = 0; k < p.K; ++k) {
+        const int off = k * p.dil - p.pad_l;
+        int j = off / p.stride;
+        int ph = off - j * p.stride;
+        if (ph < 0) { ph += p.stride; j -= 1; }
+        for (int kb = 0; kb < p.num_kb; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t *sa = smem + stage * L::STAGE_BYTES;
+          uint8_t *sb = sa + L::A_BYTES;
+          if (elect_one()) {
+            mbar_arrive_expect_tx(&full_bar[stage], L::A_BYTES + L::B_BYTES);
+            tma_load_4d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, ph, l0 + j, b0);
+            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, k * p.Cout + n0);
+          }
+          __syncwarp();
+          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          if (k == 0 && kb == 0) {
+            // The tile's epilogue operands, behind its first k-block, into warpgroup c's slot once the tensor stores of
+            // that warpgroup's previous tile have read it.  A box past Lout / B is zero-filled and still counts in full.
+            mbar_wait(&oempty_bar[c], ((it >> 1) & 1) ^ 1);
+            uint8_t *slot = smem + p.ops_off + c * p.ops_bytes;
+            if (elect_one()) {
+              mbar_arrive_expect_tx(&ofull_bar[c], p.ops_bytes);
+              for (int cb = 0; cb < BLOCK_N / BOXC; ++cb) {
+                tma_load_3d(slot + cb * BOX_BYTES, &tmap_m, &ofull_bar[c], n0 + cb * BOXC, l0, b0);
+                if (fm) {
+                  // partner rows one batch at a time: a batch group may straddle the [real; fake] boundary
+                  for (int i = 0; i < p.BB; ++i) {
+                    const int b = b0 + i;
+                    const int pb = p.fm_bh > 0 ? (b < p.fm_bh ? b + p.fm_bh : b - p.fm_bh) : b;
+                    tma_load_3d(slot + TILE_BYTES + cb * BOX_BYTES + i * p.BL * L::OUT_SPAN, &tmap_p, &ofull_bar[c],
+                                n0 + cb * BOXC, l0, pb);
+                  }
+                }
+                if (rs)
+                  tma_load_3d(slot + (fm ? 2 : 1) * TILE_BYTES + cb * BOX_BYTES, &tmap_r, &ofull_bar[c], n0 + cb * BOXC,
+                              l0, b0);
+              }
+            }
+            __syncwarp();
+          }
+        }
+      }
+    }
+  } else {
+    // =========================== MMA + epilogue warpgroups 1, 2 ===========================
+    warpgroup_reg_alloc<224>();
+    const int c = wg - 1;
+    const int w = warp & 3;
+    const bool issuer = (threadIdx.x & 127) == 0;
+    constexpr uint64_t A_HALF = (64 * SWZ) >> 4;
+    const uint32_t smem_base = smem_u32(smem);
+    uint8_t *slot = smem + p.ops_off + c * p.ops_bytes;
+    float d[2][BLOCK_N / 2];
+    int u = 0;                                     // tiles this warpgroup has run
+    for (int tile = blockIdx.x + c * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, ++u) {
+      const int it = 2 * u + c;                    // position of the tile in the CTA's sequence
+      const uint32_t g0 = (uint32_t)it * (uint32_t)kblocks;      // ring position of its first k-block
+      int stage = (int)(g0 % (uint32_t)STAGES);
+      uint32_t phase = (g0 / (uint32_t)STAGES) & 1;
+      if (it > 0) mbar_wait(&order_bar[c], ((it - 1) >> 1) & 1);  // the other warpgroup has issued tile it - 1
+      int prev = 0;
+      for (int kb = 0; kb < kblocks; ++kb) {
+        mbar_wait(&full_bar[stage], phase);
+        const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
+        const uint64_t adesc = make_kmajor_desc(sa, SWZ);
+        const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+            Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (kb > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty_bar[prev]);
+        }
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&order_bar[c ^ 1]);             // every MMA of this tile is issued
+      wgmma_wait<0>();
+      wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+      wgmma_fence_regs<BLOCK_N / 2>(d[1]);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+      const int nt = tile % p.n_nt;
+      const int mt = tile / p.n_nt;
+      const int lt = mt % p.n_lt;
+      const int bg = mt / p.n_lt;
+      const int b0 = bg * p.BB;
+      const int n0 = nt * BLOCK_N;
+      mbar_wait(&ofull_bar[c], u & 1);
+      pp_epilogue<BLOCK_N, BOXC, FM, RS>(d, slot, p, w, lane, b0);
+      // rows past Lout and batches past B fall outside the tensor map and are not written
+      fence_proxy_async();
+      named_bar_sync(1 + c, 128);
+      if (issuer) {
+#pragma unroll
+        for (int cb = 0; cb < BLOCK_N / BOXC; ++cb)
+          tma_store_3d(&tmap_o, slot + cb * BOX_BYTES, n0 + cb * BOXC, lt * p.BL, b0);
+        bulk_commit();
+        bulk_wait_read<0>();
+        mbar_arrive(&oempty_bar[c]);
+      }
+    }
+    if (issuer) bulk_wait_all();
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -494,6 +748,122 @@ static int pick_block_n(int Cout, long m_tiles) {
   return best;
 }
 
+// bf16 rows (c, l, b) over [B][out_rows][Cout] from row out_row_offset on: row l of batch b is
+// b * out_rows + l * out_row_stride + out_row_offset; the extents Lout and B clip the rows of a ragged tile.  Boxes of
+// [box_b batches][BL rows][OUT_BOXC channels], each row one swizzle span.
+template <int BN>
+static int encode_rows_map(CUtensorMap *m, const __nv_bfloat16 *base, const TcParams &p, int box_b) {
+  using L = SmemLayout<BN, 64, false>;
+  EncodeTiledFn enc = get_encode_fn();
+  cuuint64_t dims[3] = {(cuuint64_t)p.Cout, (cuuint64_t)p.Lout, (cuuint64_t)p.B};
+  cuuint64_t strides[2] = {(cuuint64_t)p.Cout * 2 * p.out_row_stride, (cuuint64_t)p.Cout * 2 * p.out_rows};
+  cuuint32_t box[3] = {(cuuint32_t)L::OUT_BOXC, (cuuint32_t)p.BL, (cuuint32_t)box_b};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<__nv_bfloat16 *>(base) + (size_t)p.out_row_offset * p.Cout,
+                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(L::OUT_SPAN),
+                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    set_error("conv1d_tc: bf16 row tensor map encode failed (%d)", (int)r);
+    return 1;
+  }
+  return 0;
+}
+
+// Shared-memory split of a ping-pong launch: two operand slots (mask, + partner rows with fm_d, + gradient skip with
+// res_bf16: [128][BLOCK_N] bf16 each), the ring in what is left (at most 8 stages).  False when fewer than 2 stages fit
+// (mask + partner + skip at BLOCK_N = 128, BLOCK_K = 64); such a launch runs conv_tc_kernel.
+template <int BLOCK_N, int BLOCK_K>
+static bool plan_smem_pp(int nops, TcParams &p) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, false>;
+  p.ops_bytes = nops * BLOCK_M * BLOCK_N * 2;
+  const int s = (SMEM_MAX - L::FIXED - 2 * p.ops_bytes) / L::STAGE_BYTES;
+  p.stages = s > 8 ? 8 : s;
+  p.ops_off = p.stages * L::STAGE_BYTES;
+  p.bar_off = p.ops_off + 2 * p.ops_bytes;
+  return p.stages >= 2;
+}
+
+// 0: launched, 1: error, -1: the operand slots leave no room for the ring (run conv_tc_kernel instead)
+template <int BN, int BK>
+static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cudaStream_t stream) {
+  using L = SmemLayout<BN, BK, false>;
+  if (!plan_smem_pp<BN, BK>(1 + (p.fm_d ? 1 : 0) + (p.res_bf16 ? 1 : 0), p)) return -1;
+  const int smem = p.bar_off + L::FIXED;
+  const int v = (p.fm_d ? 2 : 0) + (p.res_bf16 ? 1 : 0);
+  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TcParams) =
+      v == 3 ? conv_tc_pp_kernel<BN, BK, true, true> : v == 2 ? conv_tc_pp_kernel<BN, BK, true, false>
+      : v == 1 ? conv_tc_pp_kernel<BN, BK, false, true> : conv_tc_pp_kernel<BN, BK, false, false>;
+  static int attr[4] = {0, 0, 0, 0};   // dynamic shared memory each instance has been allowed so far
+  if (smem > attr[v]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) {
+      set_error("conv1d_tc: cudaFuncSetAttribute(%d bytes): %s", smem, cudaGetErrorString(e));
+      return 1;
+    }
+    attr[v] = smem;
+  }
+  // mask, skip and output boxes cover the tile's batch group; partner rows go one batch per box.  With fm_bh < 0
+  // (the launch covers the fake half) the partner of batch b is batch b of the half stored right before dact_src.
+  CUtensorMap tm, tp, tr, to;
+  memset(&tp, 0, sizeof(tp));
+  memset(&tr, 0, sizeof(tr));
+  if (encode_rows_map<BN>(&tm, p.dact_src, p, p.BB) || encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
+  if (p.fm_d && encode_rows_map<BN>(&tp, p.fm_bh > 0 ? p.dact_src : p.dact_src - p.fm_half, p, 1)) return 1;
+  if (p.res_bf16 && encode_rows_map<BN>(&tr, p.res_bf16, p, p.BB)) return 1;
+  const int tiles = p.n_lt * p.n_bg * p.n_nt;
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  const int grid = tiles < sms ? tiles : sms;
+  launch_pdl(kern, dim3(grid), dim3(PP_THREADS), smem, stream, ta, tb, tm, tp, tr, to, p);
+  RAVE_CHECK_LAUNCH("conv1d_tc");
+  return 0;
+}
+
+#ifndef RAVE_TC_X3_UNIT
+template <int BK>
+static int dispatch_pp_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
+  switch (bn) {
+    case 128: return launch_pp<128, BK>(ta, tb, p, s);
+    case 96:   // at BLOCK_K = 64 ptxas spills tile-loop invariants of every ping-pong instance: conv_tc_kernel runs it
+      if constexpr (BK == 64) return -1;
+      else return launch_pp<96, BK>(ta, tb, p, s);
+    case 64: return launch_pp<64, BK>(ta, tb, p, s);
+    case 48: return launch_pp<48, BK>(ta, tb, p, s);
+    case 32: return launch_pp<32, BK>(ta, tb, p, s);
+    case 16: return launch_pp<16, BK>(ta, tb, p, s);
+  }
+  set_error("conv1d_tc: no kernel for BLOCK_N=%d", bn);
+  return 1;
+}
+
+static int dispatch_pp(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
+  switch (BK) {
+    case 64: return dispatch_pp_n<64>(BN, ta, tb, p, s);
+    case 32: return dispatch_pp_n<32>(BN, ta, tb, p, s);
+    case 16: return dispatch_pp_n<16>(BN, ta, tb, p, s);
+  }
+  set_error("conv1d_tc: no kernel for BLOCK_K=%d", BK);
+  return 1;
+}
+
+// ring stages plan_smem_pp gives a ping-pong launch with nops operand tiles per slot; 0 = it runs conv_tc_kernel
+template <int BK>
+static int pp_stages(int BN, int nops) {
+  TcParams q;
+  bool ok = false;
+  switch (BN) {
+    case 128: ok = plan_smem_pp<128, BK>(nops, q); break;
+    case 96: ok = BK != 64 && plan_smem_pp<96, BK>(nops, q); break;    // see dispatch_pp_n
+    case 64: ok = plan_smem_pp<64, BK>(nops, q); break;
+    case 48: ok = plan_smem_pp<48, BK>(nops, q); break;
+    case 32: ok = plan_smem_pp<32, BK>(nops, q); break;
+    case 16: ok = plan_smem_pp<16, BK>(nops, q); break;
+  }
+  return ok ? q.stages : 0;
+}
+#endif
+
 template <int BN, int BK, bool X3>
 static int launch(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cudaStream_t stream) {
   using L = SmemLayout<BN, BK, X3>;
@@ -511,22 +881,7 @@ static int launch(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cuda
   }
   CUtensorMap to;
   memset(&to, 0, sizeof(to));
-  if (p.stg) {
-    // bf16 output rows (c, l, b) over [B][out_rows][Cout] from row out_row_offset on: row l of batch b is
-    // b * out_rows + l * out_row_stride + out_row_offset; the extents Lout and B clip the rows of a ragged tile
-    EncodeTiledFn enc = get_encode_fn();
-    cuuint64_t dims[3] = {(cuuint64_t)p.Cout, (cuuint64_t)p.Lout, (cuuint64_t)p.B};
-    cuuint64_t strides[2] = {(cuuint64_t)p.Cout * 2 * p.out_row_stride, (cuuint64_t)p.Cout * 2 * p.out_rows};
-    cuuint32_t box[3] = {(cuuint32_t)L::OUT_BOXC, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-    cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&to, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, p.out_act + (size_t)p.out_row_offset * p.Cout, dims,
-                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(L::OUT_SPAN),
-                     CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) {
-      set_error("conv1d_tc: output tensor map encode failed (%d)", (int)r);
-      return 1;
-    }
-  }
+  if (p.stg && encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
   const int tiles = p.n_lt * p.n_bg * p.n_nt;
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -615,6 +970,16 @@ extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
   const int smem = BK == 64 ? smem_plan_bits<64>(BN, kblocks)
                  : BK == 32 ? smem_plan_bits<32>(BN, kblocks) : smem_plan_bits<16>(BN, kblocks);
   return BN | (BK << 12) | smem;
+}
+
+// Ring stages of the ping-pong kernel for an input-gradient launch of this shape (LeakyReLU' mask, bf16 output only;
+// fm: with the feature-matching partner rows, res_bf16: with the gradient skip); 0 = the launch runs conv_tc_kernel.
+extern "C" int rave_conv1d_tc_pp_stages(int B, int Cin, int Cout, int Lout, int K, int fm, int res_bf16) {
+  using namespace rave::tc;
+  const int plan = rave_conv1d_tc_plan(B, Cin, Cout, Lout, K);
+  const int BN = plan & 0xFFF, BK = (plan >> 12) & 0xFFF;
+  const int nops = 1 + (fm ? 1 : 0) + (res_bf16 ? 1 : 0);
+  return BK == 64 ? pp_stages<64>(BN, nops) : BK == 32 ? pp_stages<32>(BN, nops) : BK == 16 ? pp_stages<16>(BN, nops) : 0;
 }
 
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,
@@ -710,6 +1075,12 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   }
   cudaStream_t s = (cudaStream_t)stream;
   if (x3) return conv_tc_dispatch_x3(BK, BN, ta, tb, p, s);
+  // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only): the
+  // ping-pong kernel, unless its operand slots leave no room for the ring
+  if (dact_src && out_act && !bias && !res && !res_act && !out_f32 && act == RAVE_ACT_NONE) {
+    const int r = dispatch_pp(BK, BN, ta, tb, p, s);
+    if (r >= 0) return r;
+  }
   return dispatch_all<false>(BK, BN, ta, tb, p, s);
 }
 

@@ -159,6 +159,16 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Register rebalancing between warpgroups (every thread of the warpgroup executes it): a producer warpgroup gives
+// registers back so that the MMA warpgroups of the same CTA can grow past the launch-time share.  N is a multiple of 8.
+template <int N>
+__device__ __forceinline__ void warpgroup_reg_dealloc() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void warpgroup_reg_alloc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
 // keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void wgmma_fence_regs(float *d) {
