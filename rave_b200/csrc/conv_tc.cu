@@ -20,6 +20,8 @@
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
 #include <string.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 #include "tc_common.cuh"
 
@@ -51,7 +53,6 @@ struct TcParams {
   const float *fm_d;       // feature-matching gradient fused into a dgrad epilogue (or null): dact_src is the bf16
   long fm_half;            //   operand a = LeakyReLU(h) of [real; fake] rows, fm_half elements apart; adds
   int fm_bh;               //   d0 sgn(h_r-h_f) + d1 sgn(h_r) to real rows (b < fm_bh), -d0 sgn(h_r-h_f) to fake rows
-  int x3;                  // split-operand mode ("bf16x3"): activations [.., 2*Cin] = [hi | lo], weights [2][K][Cout][Cin]
   int act_ld;              // row length (elements) of the bf16 operand tensors the epilogue touches (out_act, res_act):
                            // Cout, or 2*Cout in x3 mode
   int act_cs;              // x3: channels per POSITION of an output row (Cout; Cout/stride when the row holds the phases
@@ -136,6 +137,34 @@ __device__ __forceinline__ void st_words(void *ptr, const uint32_t *w) {
 __device__ __forceinline__ float bf_lo(uint32_t w) { return __uint_as_float(w << 16); }
 __device__ __forceinline__ float bf_hi(uint32_t w) { return __uint_as_float(w & 0xFFFF0000u); }
 
+// Input-gradient epilogue arithmetic on one column pair (v0, v1), in this order: lrelu_mask, fm_grad, add_bf16_pair.
+// Chain rule through the LeakyReLU that produced this conv's operand: the sign bits of the saved bf16 operand pair dm.
+__device__ __forceinline__ void lrelu_mask(float &v0, float &v1, uint32_t dm, float slope) {
+  if (dm & 0x00008000u) v0 *= slope;
+  if (dm & 0x80000000u) v1 *= slope;
+}
+// Gradient of d0 * sum|h_r - h_f| + d1 * sum|h_r| with respect to h (dm: this row's operand pair, pm: the partner row's).
+// LeakyReLU is strictly increasing, so sgn(h_r - h_f) = sgn(a_r - a_f) and sgn(h_r) = sgn(a_r): the saved operands are
+// compared as they are.  With t = sgn(a_self - a_partner) both halves get d0 * t (real: d0 sgn(h_r-h_f); fake:
+// -d0 sgn(h_r-h_f) = d0 t), real rows d1 sgn(a_self) on top (d1 = 0 on fake rows).  The epilogue is issue-bound on these
+// launches: ~6 instructions per element instead of ~20 for the literal form.
+__device__ __forceinline__ void fm_grad(float &v0, float &v1, uint32_t dm, uint32_t pm, float d0, float d1) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float as = h ? bf_hi(dm) : bf_lo(dm);
+    const float ap = h ? bf_hi(pm) : bf_lo(pm);
+    const float t = (as > ap ? 1.f : 0.f) - (as < ap ? 1.f : 0.f);
+    const float sr = (as > 0.f ? 1.f : 0.f) - (as < 0.f ? 1.f : 0.f);
+    float &v = h ? v1 : v0;
+    v = fmaf(d1, sr, fmaf(d0, t, v));
+  }
+}
+// + the bf16 gradient-skip pair rb
+__device__ __forceinline__ void add_bf16_pair(float &v0, float &v1, uint32_t rb) {
+  v0 += bf_lo(rb);
+  v1 += bf_hi(rb);
+}
+
 // stg (or null): the output staging tile; out_act then goes there (tile row `row`, channel co - n0) instead of to HBM
 template <int CW, bool X3, int BOXC>
 __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, int co, bool valid, size_t orow,
@@ -168,38 +197,18 @@ __device__ __forceinline__ void tc_epi_chunk(const TcParams &p, uint32_t taddr, 
       v[4 * i] += bb.x; v[4 * i + 1] += bb.y; v[4 * i + 2] += bb.z; v[4 * i + 3] += bb.w;
     }
   }
-  if (!X3 && p.dact_src) {   // chain rule through the LeakyReLU that produced this conv's operand (sign bits of bf16)
+  if (!X3 && p.dact_src) {
 #pragma unroll
-    for (int w = 0; w < NW; ++w) {
-      if (dm[w] & 0x00008000u) v[2 * w] *= p.slope;
-      if (dm[w] & 0x80000000u) v[2 * w + 1] *= p.slope;
-    }
+    for (int w = 0; w < NW; ++w) lrelu_mask(v[2 * w], v[2 * w + 1], dm[w], p.slope);
   }
   if (!X3 && fm_side) {
-    // Gradient of d0 * sum|h_r - h_f| + d1 * sum|h_r| with respect to h.  LeakyReLU is strictly increasing, so
-    // sgn(h_r - h_f) = sgn(a_r - a_f) and sgn(h_r) = sgn(a_r): the saved operands are compared as they are.  With
-    // t = sgn(a_self - a_partner) both halves get d0 * t (real: d0 sgn(h_r-h_f); fake: -d0 sgn(h_r-h_f) = d0 t), real
-    // rows d1 sgn(a_self) on top.  The epilogue is issue-bound on these launches: ~6 instructions per element
-    // instead of ~20 for the literal form.
     const float d0 = __ldg(p.fm_d), d1 = fm_side > 0 ? __ldg(p.fm_d + 1) : 0.f;
 #pragma unroll
-    for (int w = 0; w < NW; ++w) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float as = h ? bf_hi(dm[w]) : bf_lo(dm[w]);
-        const float ap = h ? bf_hi(pm[w]) : bf_lo(pm[w]);
-        const float t = (as > ap ? 1.f : 0.f) - (as < ap ? 1.f : 0.f);
-        const float sr = (as > 0.f ? 1.f : 0.f) - (as < 0.f ? 1.f : 0.f);
-        v[2 * w + h] = fmaf(d1, sr, fmaf(d0, t, v[2 * w + h]));
-      }
-    }
+    for (int w = 0; w < NW; ++w) fm_grad(v[2 * w], v[2 * w + 1], dm[w], pm[w], d0, d1);
   }
   if (!X3 && p.res_bf16) {
 #pragma unroll
-    for (int w = 0; w < NW; ++w) {
-      v[2 * w] += bf_lo(rb[w]);
-      v[2 * w + 1] += bf_hi(rb[w]);
-    }
+    for (int w = 0; w < NW; ++w) add_bf16_pair(v[2 * w], v[2 * w + 1], rb[w]);
   }
   if (p.res_act) {     // residual skip from the unit's own bf16 operand: undo the LeakyReLU
 #pragma unroll
@@ -267,13 +276,140 @@ __device__ __forceinline__ void tc_epilogue(const TcParams &p, uint32_t taddr, i
   if (MAIN < BLOCK_N) tc_epi_chunk<16, X3, BOXC>(p, taddr + MAIN, n0 + MAIN, valid, orow, fm_side, stg, row, MAIN);
 }
 
+// First time step, first batch and first output channel of tile `tile` of the persistent loop (N tiles vary fastest,
+// then time tiles, then batch groups)
+struct TileCoord {
+  int l0, b0, n0;
+};
+template <int BLOCK_N>
+__device__ __forceinline__ TileCoord tile_coord(int tile, const TcParams &p) {
+  const int nt = tile % p.n_nt;
+  const int mt = tile / p.n_nt;
+  const int lt = mt % p.n_lt;
+  const int bg = mt / p.n_lt;
+  return {lt * p.BL, bg * p.BB, nt * BLOCK_N};
+}
+
+// Input row of output row l at tap k: l*stride + k*dil - pad_l = (l + j)*stride + ph, 0 <= ph < stride
+struct TapOrigin {
+  int j, ph;
+};
+__device__ __forceinline__ TapOrigin tap_origin(int k, int dil, int pad_l, int stride) {
+  const int off = k * dil - pad_l;
+  int j = off / stride;
+  int ph = off - j * stride;
+  if (ph < 0) { ph += stride; j -= 1; }
+  return {j, ph};
+}
+
+// The operand ring: `stages` slots at the base of shared memory with a full and an empty barrier each; stage / phase =
+// the slot of the next k-block and the parity its barriers are at.
+struct Ring {
+  uint64_t *full, *empty;
+  int stages;
+  int stage;
+  uint32_t phase;
+  __device__ __forceinline__ void advance() {
+    if (++stage == stages) { stage = 0; phase ^= 1; }
+  }
+};
+
+// Producer (whole warp, elected lane issues): k-block kb of tap k of a tile into the next ring slot once it is free --
+// the activation rows from tap origin o, channels kb * BLOCK_K .., and the weight rows of tap k; x3 also the lo halves.
+template <int BLOCK_N, int BLOCK_K, bool X3>
+__device__ __forceinline__ void produce_kblock(uint8_t *smem, Ring &r, const CUtensorMap *tmap_a,
+                                               const CUtensorMap *tmap_b, const TcParams &p, const TileCoord &t,
+                                               TapOrigin o, int k, int kb) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
+  mbar_wait(&r.empty[r.stage], r.phase ^ 1);
+  uint8_t *sa = smem + r.stage * L::STAGE_BYTES;
+  uint8_t *sb = sa + L::A_BYTES;
+  uint64_t *bar = &r.full[r.stage];
+  if (elect_one()) {
+    mbar_arrive_expect_tx(bar, L::A_BYTES + L::B_BYTES);
+    tma_load_4d(sa, tmap_a, bar, kb * BLOCK_K, o.ph, t.l0 + o.j, t.b0);
+    tma_load_2d(sb, tmap_b, bar, kb * BLOCK_K, k * p.Cout + t.n0);
+    if (X3) {      // lo halves: channels Cin.. of the activation rows, weight slabs K.. (wt is [2][K][Cout][Cin])
+      tma_load_4d(sa + L::A_PART, tmap_a, bar, p.Cin + kb * BLOCK_K, o.ph, t.l0 + o.j, t.b0);
+      tma_load_2d(sb + L::B_PART, tmap_b, bar, kb * BLOCK_K, (p.K + k) * p.Cout + t.n0);
+    }
+  }
+  __syncwarp();
+  r.advance();
+}
+
+// The wgmma of k-block kb of a tile from the ring slot at shared address sa, as one committed group: BLOCK_K / 16 steps
+// of the two m64 halves (x3: plus lo*hi and hi*lo).  The first step of a tile overwrites the accumulators.
+template <int BLOCK_N, int BLOCK_K, bool X3>
+__device__ __forceinline__ void mma_kblock(float (*d)[BLOCK_N / 2], uint32_t sa, int kb) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
+  constexpr int SWZ = BLOCK_K * 2;
+  // rows 64 h .. 64 h + 63 of an operand tile start 64 swizzle spans further: + (64 * SWZ) >> 4 in the address field
+  constexpr uint64_t A_HALF = (64 * SWZ) >> 4;
+  const uint64_t adesc = make_kmajor_desc(sa, SWZ);
+  const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
+    // advance 16 bf16 = 32 bytes inside the swizzle span: +2 in the (addr >> 4) field
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
+  }
+  if (X3) {        // a*w ~ a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the lo*lo term is below fp32 accumulation noise)
+    const uint64_t adesc_lo = make_kmajor_desc(sa + L::A_PART, SWZ);
+    const uint64_t bdesc_lo = make_kmajor_desc(sa + L::A_BYTES + L::B_PART, SWZ);
+#pragma unroll
+    for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc_lo + h * A_HALF + 2 * kk, bdesc + 2 * kk, 1u);
+        Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc_lo + 2 * kk, 1u);
+      }
+    }
+  }
+  wgmma_commit();
+}
+
+// Main loop of one tile (MMA warpgroup): its kblocks k-blocks from the ring.  One wgmma group stays in flight: k-block kb
+// is issued before the group of kb - 1 is waited for, so the tensor pipe does not drain between k-blocks; a slot is
+// released (one arrival per warp) once the group that reads it has completed.  Returns the slot of the last group, which
+// is still in flight (mma_drain).
+template <int BLOCK_N, int BLOCK_K, bool X3>
+__device__ __forceinline__ int mma_mainloop(float (*d)[BLOCK_N / 2], uint32_t smem_base, Ring &r, int kblocks,
+                                            int lane) {
+  using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
+  int prev = 0;
+  for (int kb = 0; kb < kblocks; ++kb) {
+    mbar_wait(&r.full[r.stage], r.phase);
+    mma_kblock<BLOCK_N, BLOCK_K, X3>(d, smem_base + r.stage * L::STAGE_BYTES, kb);
+    wgmma_wait<1>();                                         // the group of k-block kb - 1 has completed
+    if (kb > 0) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&r.empty[prev]);            // this warp's MMAs no longer read that slot
+    }
+    prev = r.stage;
+    r.advance();
+  }
+  return prev;
+}
+
+// End of a tile's main loop: wait for its last wgmma group, then release that group's slot
+template <int BLOCK_N>
+__device__ __forceinline__ void mma_drain(float (*d)[BLOCK_N / 2], const Ring &r, int prev, int lane) {
+  wgmma_wait<0>();
+  wgmma_fence_regs<BLOCK_N / 2>(d[0]);
+  wgmma_fence_regs<BLOCK_N / 2>(d[1]);
+  __syncwarp();
+  if (lane == 0) mbar_arrive(&r.empty[prev]);
+}
+
 template <int BLOCK_N, int BLOCK_K, bool X3>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                const __grid_constant__ CUtensorMap tmap_o, const TcParams p) {
   using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
   const int STAGES = p.stages;
-  constexpr int SWZ = BLOCK_K * 2;
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
 
   extern __shared__ uint8_t smem_raw[];
@@ -308,94 +444,25 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
   griddep_launch_dependents();      // dependents may begin their prologue ...
   griddep_wait();                   // ... and this kernel touches global memory only after its predecessors are done
 
+  Ring ring{full_bar, empty_bar, STAGES, 0, 0};
   if (warp == 4) {
     // =========================== TMA producer (warp-uniform loop, elected lane issues) ===========================
-    int stage = 0;
-    uint32_t phase = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int nt = tile % p.n_nt;
-      const int mt = tile / p.n_nt;
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int l0 = lt * p.BL;
-      const int b0 = bg * p.BB;
-      const int n0 = nt * BLOCK_N;
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
       for (int k = 0; k < p.K; ++k) {
-        // input row = l*stride + k*dil - pad_l = (l + j)*stride + ph
-        const int off = k * p.dil - p.pad_l;
-        int j = off / p.stride;
-        int ph = off - j * p.stride;
-        if (ph < 0) { ph += p.stride; j -= 1; }
-        for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t *sa = smem + stage * L::STAGE_BYTES;
-          uint8_t *sb = sa + L::A_BYTES;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&full_bar[stage], L::A_BYTES + L::B_BYTES);
-            tma_load_4d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, ph, l0 + j, b0);
-            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, k * p.Cout + n0);
-            if (X3) {      // lo halves: channels Cin.. of the activation rows, weight slabs K.. (wt is [2][K][Cout][Cin])
-              tma_load_4d(sa + L::A_PART, &tmap_a, &full_bar[stage], p.Cin + kb * BLOCK_K, ph, l0 + j, b0);
-              tma_load_2d(sb + L::B_PART, &tmap_b, &full_bar[stage], kb * BLOCK_K, (p.K + k) * p.Cout + n0);
-            }
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
+        const TapOrigin o = tap_origin(k, p.dil, p.pad_l, p.stride);
+        for (int kb = 0; kb < p.num_kb; ++kb)
+          produce_kblock<BLOCK_N, BLOCK_K, X3>(smem, ring, &tmap_a, &tmap_b, p, t, o, k, kb);
       }
     }
   } else if (warp < 4) {
     // =========================== MMA warpgroup ===========================
-    // rows 64 h .. 64 h + 63 of an operand tile start 64 swizzle spans further: + (64 * SWZ) >> 4 in the address field
-    constexpr uint64_t A_HALF = (64 * SWZ) >> 4;
     const uint32_t smem_base = smem_u32(smem);
     float d[2][BLOCK_N / 2];
-    int stage = 0;
-    uint32_t phase = 0;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      // One wgmma group stays in flight: k-block kb is issued before the group of kb - 1 is waited for, so the tensor
-      // pipe does not drain between k-blocks.  A stage is released once the group that reads it has completed.
-      int prev = 0;                   // stage of the group still in flight (k-block kb - 1)
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-        const uint64_t adesc = make_kmajor_desc(sa, SWZ);
-        const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
-          // advance 16 bf16 = 32 bytes inside the swizzle span: +2 in the (addr >> 4) field
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
-        }
-        if (X3) {        // a*w ~ a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the lo*lo term is below fp32 accumulation noise)
-          const uint64_t adesc_lo = make_kmajor_desc(sa + L::A_PART, SWZ);
-          const uint64_t bdesc_lo = make_kmajor_desc(sa + L::A_BYTES + L::B_PART, SWZ);
-#pragma unroll
-          for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc_lo + h * A_HALF + 2 * kk, bdesc + 2 * kk, 1u);
-              Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc_lo + 2 * kk, 1u);
-            }
-          }
-        }
-        wgmma_commit();
-        wgmma_wait<1>();                                         // the group of k-block kb - 1 has completed
-        if (kb > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);          // this warp's MMAs no longer read that slot
-        }
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      wgmma_wait<0>();
-      wgmma_fence_regs<BLOCK_N / 2>(d[0]);
-      wgmma_fence_regs<BLOCK_N / 2>(d[1]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);              // the last k-block's slot
+      const int prev = mma_mainloop<BLOCK_N, BLOCK_K, X3>(d, smem_base, ring, kblocks, lane);
+      mma_drain<BLOCK_N>(d, ring, prev, lane);
       const int buf = p.nacc == 2 ? (it & 1) : 0;
       const uint32_t use = p.nacc == 2 ? (it >> 1) : it;         // earlier tiles handed over through this buffer
       mbar_wait(&tempty_bar[buf], (use & 1) ^ 1);                // the epilogue has read the buffer's previous tile
@@ -410,13 +477,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
     const bool issuer = threadIdx.x == 160;
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int nt = tile % p.n_nt;
-      const int mt = tile / p.n_nt;
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int n0 = nt * BLOCK_N;
-      const int b = bg * p.BB + row / p.BL;
-      const int l = lt * p.BL + row % p.BL;
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
+      const int n0 = t.n0;
+      const int b = t.b0 + row / p.BL;
+      const int l = t.l0 + row % p.BL;
       const bool valid = (b < p.B) && (l < p.Lout);
       const size_t orow = (size_t)b * p.out_rows + (size_t)l * p.out_row_stride + p.out_row_offset;
 
@@ -438,7 +502,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
         if (issuer) {
 #pragma unroll
           for (int c = 0; c < BLOCK_N; c += BOXC)
-            tma_store_3d(&tmap_o, stg + (c / BOXC) * (BLOCK_M * L::OUT_SPAN), n0 + c, lt * p.BL, bg * p.BB);
+            tma_store_3d(&tmap_o, stg + (c / BOXC) * (BLOCK_M * L::OUT_SPAN), n0 + c, t.l0, t.b0);
           bulk_commit();
         }
       }
@@ -464,7 +528,7 @@ constexpr int PP_THREADS = 384;
 
 // Epilogue of one tile from the accumulator registers of warpgroup thread (w, lane).  slot = [mask | partner (FM) |
 // gradient skip (RS)] tiles, each BLOCK_N / BOXC boxes of [128 rows][BOXC channels] in the canonical swizzle.  Per
-// element the same fp32 sequence as tc_epi_chunk: mask, feature-matching term, skip, one rounding to bf16.
+// element the same fp32 sequence as tc_epi_chunk (lrelu_mask, fm_grad, add_bf16_pair), one rounding to bf16.
 template <int BLOCK_N, int BOXC, bool FM, bool RS>
 __device__ __forceinline__ void pp_epilogue(float (*d)[BLOCK_N / 2], uint8_t *slot, const TcParams &p, int w, int lane,
                                             int b0) {
@@ -489,25 +553,9 @@ __device__ __forceinline__ void pp_epilogue(float (*d)[BLOCK_N / 2], uint8_t *sl
         const uint32_t off = (base ^ (uint32_t)((j % JB) << 4)) + (j / JB) * (BLOCK_M * SPAN) + (64 * h + 8 * r) * SPAN;
         float v0 = d[h][4 * j + 2 * r], v1 = d[h][4 * j + 2 * r + 1];
         const uint32_t dm = *reinterpret_cast<const uint32_t *>(slot + off);
-        if (dm & 0x00008000u) v0 *= p.slope;
-        if (dm & 0x80000000u) v1 *= p.slope;
-        if (FM) {
-          const uint32_t pm = *reinterpret_cast<const uint32_t *>(part + off);
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float as = e ? bf_hi(dm) : bf_lo(dm);
-            const float ap = e ? bf_hi(pm) : bf_lo(pm);
-            const float t = (as > ap ? 1.f : 0.f) - (as < ap ? 1.f : 0.f);
-            const float sr = (as > 0.f ? 1.f : 0.f) - (as < 0.f ? 1.f : 0.f);
-            float &v = e ? v1 : v0;
-            v = fmaf(d1r, sr, fmaf(d0, t, v));
-          }
-        }
-        if (RS) {
-          const uint32_t rb = *reinterpret_cast<const uint32_t *>(skip + off);
-          v0 += bf_lo(rb);
-          v1 += bf_hi(rb);
-        }
+        lrelu_mask(v0, v1, dm, p.slope);
+        if (FM) fm_grad(v0, v1, dm, *reinterpret_cast<const uint32_t *>(part + off), d0, d1r);
+        if (RS) add_bf16_pair(v0, v1, *reinterpret_cast<const uint32_t *>(skip + off));
         __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
         *reinterpret_cast<uint32_t *>(slot + off) = *reinterpret_cast<uint32_t *>(&o);
       }
@@ -527,7 +575,6 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   constexpr int BOXC = L::OUT_BOXC;
   constexpr int BOX_BYTES = BLOCK_M * L::OUT_SPAN;          // one [128 rows][BOXC channels] box
   constexpr int TILE_BYTES = BLOCK_M * BLOCK_N * 2;         // one operand tile
-  constexpr int SWZ = BLOCK_K * 2;
   const int STAGES = p.stages;
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
 
@@ -572,34 +619,15 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     // =========================== TMA producer (warp-uniform loop, elected lane issues) ===========================
     warpgroup_reg_dealloc<56>();
     if (warp != 0) return;
-    int stage = 0;
-    uint32_t phase = 0;
+    Ring ring{full_bar, empty_bar, STAGES, 0, 0};
     int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int nt = tile % p.n_nt;
-      const int mt = tile / p.n_nt;
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int l0 = lt * p.BL;
-      const int b0 = bg * p.BB;
-      const int n0 = nt * BLOCK_N;
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
       const int c = it & 1;                        // consumer warpgroup of this tile
       for (int k = 0; k < p.K; ++k) {
-        const int off = k * p.dil - p.pad_l;
-        int j = off / p.stride;
-        int ph = off - j * p.stride;
-        if (ph < 0) { ph += p.stride; j -= 1; }
+        const TapOrigin o = tap_origin(k, p.dil, p.pad_l, p.stride);
         for (int kb = 0; kb < p.num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t *sa = smem + stage * L::STAGE_BYTES;
-          uint8_t *sb = sa + L::A_BYTES;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(&full_bar[stage], L::A_BYTES + L::B_BYTES);
-            tma_load_4d(sa, &tmap_a, &full_bar[stage], kb * BLOCK_K, ph, l0 + j, b0);
-            tma_load_2d(sb, &tmap_b, &full_bar[stage], kb * BLOCK_K, k * p.Cout + n0);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
+          produce_kblock<BLOCK_N, BLOCK_K, false>(smem, ring, &tmap_a, &tmap_b, p, t, o, k, kb);
           if (k == 0 && kb == 0) {
             // The tile's epilogue operands, behind its first k-block, into warpgroup c's slot once the tensor stores of
             // that warpgroup's previous tile have read it.  A box past Lout / B is zero-filled and still counts in full.
@@ -608,19 +636,19 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             if (elect_one()) {
               mbar_arrive_expect_tx(&ofull_bar[c], p.ops_bytes);
               for (int cb = 0; cb < BLOCK_N / BOXC; ++cb) {
-                tma_load_3d(slot + cb * BOX_BYTES, &tmap_m, &ofull_bar[c], n0 + cb * BOXC, l0, b0);
+                tma_load_3d(slot + cb * BOX_BYTES, &tmap_m, &ofull_bar[c], t.n0 + cb * BOXC, t.l0, t.b0);
                 if (fm) {
                   // partner rows one batch at a time: a batch group may straddle the [real; fake] boundary
                   for (int i = 0; i < p.BB; ++i) {
-                    const int b = b0 + i;
+                    const int b = t.b0 + i;
                     const int pb = p.fm_bh > 0 ? (b < p.fm_bh ? b + p.fm_bh : b - p.fm_bh) : b;
                     tma_load_3d(slot + TILE_BYTES + cb * BOX_BYTES + i * p.BL * L::OUT_SPAN, &tmap_p, &ofull_bar[c],
-                                n0 + cb * BOXC, l0, pb);
+                                t.n0 + cb * BOXC, t.l0, pb);
                   }
                 }
                 if (rs)
-                  tma_load_3d(slot + (fm ? 2 : 1) * TILE_BYTES + cb * BOX_BYTES, &tmap_r, &ofull_bar[c], n0 + cb * BOXC,
-                              l0, b0);
+                  tma_load_3d(slot + (fm ? 2 : 1) * TILE_BYTES + cb * BOX_BYTES, &tmap_r, &ofull_bar[c],
+                              t.n0 + cb * BOXC, t.l0, t.b0);
               }
             }
             __syncwarp();
@@ -634,7 +662,6 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     const int c = wg - 1;
     const int w = warp & 3;
     const bool issuer = (threadIdx.x & 127) == 0;
-    constexpr uint64_t A_HALF = (64 * SWZ) >> 4;
     const uint32_t smem_base = smem_u32(smem);
     uint8_t *slot = smem + p.ops_off + c * p.ops_bytes;
     float d[2][BLOCK_N / 2];
@@ -642,54 +669,23 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     for (int tile = blockIdx.x + c * gridDim.x; tile < num_tiles; tile += 2 * gridDim.x, ++u) {
       const int it = 2 * u + c;                    // position of the tile in the CTA's sequence
       const uint32_t g0 = (uint32_t)it * (uint32_t)kblocks;      // ring position of its first k-block
-      int stage = (int)(g0 % (uint32_t)STAGES);
-      uint32_t phase = (g0 / (uint32_t)STAGES) & 1;
+      Ring ring{full_bar, empty_bar, STAGES, (int)(g0 % (uint32_t)STAGES), (g0 / (uint32_t)STAGES) & 1};
       if (it > 0) mbar_wait(&order_bar[c], ((it - 1) >> 1) & 1);  // the other warpgroup has issued tile it - 1
-      int prev = 0;
-      for (int kb = 0; kb < kblocks; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = smem_base + stage * L::STAGE_BYTES;
-        const uint64_t adesc = make_kmajor_desc(sa, SWZ);
-        const uint64_t bdesc = make_kmajor_desc(sa + L::A_BYTES, SWZ);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-            Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (kb > 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&empty_bar[prev]);
-        }
-        prev = stage;
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
+      const int prev = mma_mainloop<BLOCK_N, BLOCK_K, false>(d, smem_base, ring, kblocks, lane);
       __syncwarp();
       if (lane == 0) mbar_arrive(&order_bar[c ^ 1]);             // every MMA of this tile is issued
-      wgmma_wait<0>();
-      wgmma_fence_regs<BLOCK_N / 2>(d[0]);
-      wgmma_fence_regs<BLOCK_N / 2>(d[1]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      mma_drain<BLOCK_N>(d, ring, prev, lane);
 
-      const int nt = tile % p.n_nt;
-      const int mt = tile / p.n_nt;
-      const int lt = mt % p.n_lt;
-      const int bg = mt / p.n_lt;
-      const int b0 = bg * p.BB;
-      const int n0 = nt * BLOCK_N;
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
       mbar_wait(&ofull_bar[c], u & 1);
-      pp_epilogue<BLOCK_N, BOXC, FM, RS>(d, slot, p, w, lane, b0);
+      pp_epilogue<BLOCK_N, BOXC, FM, RS>(d, slot, p, w, lane, t.b0);
       // rows past Lout and batches past B fall outside the tensor map and are not written
       fence_proxy_async();
       named_bar_sync(1 + c, 128);
       if (issuer) {
 #pragma unroll
         for (int cb = 0; cb < BLOCK_N / BOXC; ++cb)
-          tma_store_3d(&tmap_o, slot + cb * BOX_BYTES, n0 + cb * BOXC, lt * p.BL, b0);
+          tma_store_3d(&tmap_o, slot + cb * BOX_BYTES, t.n0 + cb * BOXC, t.l0, t.b0);
         bulk_commit();
         bulk_wait_read<0>();
         mbar_arrive(&oempty_bar[c]);
@@ -702,23 +698,6 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
-                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
-                                  CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFn)ptr;
-  }
-  return fn;
-}
-
 static CUtensorMapSwizzle swizzle_enum(int bytes) {
   return bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
                                                                  : CU_TENSOR_MAP_SWIZZLE_32B;
@@ -748,20 +727,63 @@ static int pick_block_n(int Cout, long m_tiles) {
   return best;
 }
 
+// Tile geometry of a launch: M tiles of BB batches x BL time steps, BN (BLOCK_N) output channels per N tile, num_kb
+// k-blocks of BK (BLOCK_K) input channels per tap.  BK = 0 or BN = 0: no kernel covers the shape.
+struct TcGeometry {
+  int BK, BL, BB, n_lt, n_bg, BN, n_nt, num_kb;
+};
+static TcGeometry tc_geometry(int B, int Cin, int Cout, int Lout) {
+  TcGeometry g;
+  g.BK = pick_block_k(Cin);
+  g.BL = 128;
+  while (g.BL > Lout && g.BL > 8) g.BL >>= 1;   // power of two <= max(Lout, 8)
+  g.BB = 128 / g.BL;
+  g.n_lt = ceil_div(Lout, g.BL);
+  g.n_bg = ceil_div(B, g.BB);
+  g.BN = pick_block_n(Cout, (long)g.n_lt * g.n_bg);
+  g.n_nt = g.BN ? Cout / g.BN : 0;
+  g.num_kb = g.BK ? ceil_div(Cin, g.BK) : 0;
+  return g;
+}
+
+// f(BK, BN) with std::integral_constant arguments, for each (BLOCK_K, BLOCK_N) pair the kernels are built for; any other
+// pair is an error (1)
+template <int BK, typename F>
+static int visit_block_n(int BN, F &f) {
+  using std::integral_constant;
+  switch (BN) {
+    case 128: return f(integral_constant<int, BK>(), integral_constant<int, 128>());
+    case 96: return f(integral_constant<int, BK>(), integral_constant<int, 96>());
+    case 64: return f(integral_constant<int, BK>(), integral_constant<int, 64>());
+    case 48: return f(integral_constant<int, BK>(), integral_constant<int, 48>());
+    case 32: return f(integral_constant<int, BK>(), integral_constant<int, 32>());
+    case 16: return f(integral_constant<int, BK>(), integral_constant<int, 16>());
+  }
+  set_error("conv1d_tc: no kernel for BLOCK_N=%d", BN);
+  return 1;
+}
+template <typename F>
+static int visit_tile(int BK, int BN, F &&f) {
+  switch (BK) {
+    case 64: return visit_block_n<64>(BN, f);
+    case 32: return visit_block_n<32>(BN, f);
+    case 16: return visit_block_n<16>(BN, f);
+  }
+  set_error("conv1d_tc: no kernel for BLOCK_K=%d", BK);
+  return 1;
+}
+
 // bf16 rows (c, l, b) over [B][out_rows][Cout] from row out_row_offset on: row l of batch b is
 // b * out_rows + l * out_row_stride + out_row_offset; the extents Lout and B clip the rows of a ragged tile.  Boxes of
 // [box_b batches][BL rows][OUT_BOXC channels], each row one swizzle span.
 template <int BN>
 static int encode_rows_map(CUtensorMap *m, const __nv_bfloat16 *base, const TcParams &p, int box_b) {
   using L = SmemLayout<BN, 64, false>;
-  EncodeTiledFn enc = get_encode_fn();
-  cuuint64_t dims[3] = {(cuuint64_t)p.Cout, (cuuint64_t)p.Lout, (cuuint64_t)p.B};
-  cuuint64_t strides[2] = {(cuuint64_t)p.Cout * 2 * p.out_row_stride, (cuuint64_t)p.Cout * 2 * p.out_rows};
-  cuuint32_t box[3] = {(cuuint32_t)L::OUT_BOXC, (cuuint32_t)p.BL, (cuuint32_t)box_b};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<__nv_bfloat16 *>(base) + (size_t)p.out_row_offset * p.Cout,
-                   dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(L::OUT_SPAN),
-                   CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const cuuint64_t dims[3] = {(cuuint64_t)p.Cout, (cuuint64_t)p.Lout, (cuuint64_t)p.B};
+  const cuuint64_t strides[2] = {(cuuint64_t)p.Cout * 2 * p.out_row_stride, (cuuint64_t)p.Cout * 2 * p.out_rows};
+  const cuuint32_t box[3] = {(cuuint32_t)L::OUT_BOXC, (cuuint32_t)p.BL, (cuuint32_t)box_b};
+  const CUresult r = encode_bf16_map(m, 3, base + (size_t)p.out_row_offset * p.Cout, dims, strides, box,
+                                     swizzle_enum(L::OUT_SPAN), CU_TENSOR_MAP_L2_PROMOTION_NONE);
   if (r != CUDA_SUCCESS) {
     set_error("conv1d_tc: bf16 row tensor map encode failed (%d)", (int)r);
     return 1;
@@ -769,39 +791,30 @@ static int encode_rows_map(CUtensorMap *m, const __nv_bfloat16 *base, const TcPa
   return 0;
 }
 
-// Shared-memory split of a ping-pong launch: two operand slots (mask, + partner rows with fm_d, + gradient skip with
-// res_bf16: [128][BLOCK_N] bf16 each), the ring in what is left (at most 8 stages).  False when fewer than 2 stages fit
-// (mask + partner + skip at BLOCK_N = 128, BLOCK_K = 64); such a launch runs conv_tc_kernel.
-template <int BLOCK_N, int BLOCK_K>
-static bool plan_smem_pp(int nops, TcParams &p) {
-  using L = SmemLayout<BLOCK_N, BLOCK_K, false>;
-  p.ops_bytes = nops * BLOCK_M * BLOCK_N * 2;
-  const int s = (SMEM_MAX - L::FIXED - 2 * p.ops_bytes) / L::STAGE_BYTES;
-  p.stages = s > 8 ? 8 : s;
-  p.ops_off = p.stages * L::STAGE_BYTES;
-  p.bar_off = p.ops_off + 2 * p.ops_bytes;
-  return p.stages >= 2;
+// BLOCK_N = 96 at BLOCK_K = 64: ptxas spills tile-loop invariants of every ping-pong instance, so none is built and
+// conv_tc_kernel runs these launches
+template <int BN, int BK>
+constexpr bool pp_built = !(BN == 96 && BK == 64);
+
+// Ring stages of a ping-pong launch whose operand slots hold nops tiles each (mask, + partner rows with fm_d, + gradient
+// skip with res_bf16: [128][BLOCK_N] bf16 each); the ring gets the rest (at most 8 stages).  0: the launch runs
+// conv_tc_kernel -- no instance for the tile, or fewer than 2 stages fit (mask + partner + skip at BLOCK_N = 128,
+// BLOCK_K = 64).
+template <int BN, int BK>
+constexpr int pp_stages(int nops) {
+  using L = SmemLayout<BN, BK, false>;
+  if (!pp_built<BN, BK>) return 0;
+  const int s = (SMEM_MAX - L::FIXED - 2 * nops * BLOCK_M * BN * 2) / L::STAGE_BYTES;
+  return s < 2 ? 0 : s > 8 ? 8 : s;
 }
 
-// 0: launched, 1: error, -1: the operand slots leave no room for the ring (run conv_tc_kernel instead)
 template <int BN, int BK>
-static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cudaStream_t stream) {
+static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, int stages, cudaStream_t stream) {
   using L = SmemLayout<BN, BK, false>;
-  if (!plan_smem_pp<BN, BK>(1 + (p.fm_d ? 1 : 0) + (p.res_bf16 ? 1 : 0), p)) return -1;
-  const int smem = p.bar_off + L::FIXED;
-  const int v = (p.fm_d ? 2 : 0) + (p.res_bf16 ? 1 : 0);
-  void (*kern)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, TcParams) =
-      v == 3 ? conv_tc_pp_kernel<BN, BK, true, true> : v == 2 ? conv_tc_pp_kernel<BN, BK, true, false>
-      : v == 1 ? conv_tc_pp_kernel<BN, BK, false, true> : conv_tc_pp_kernel<BN, BK, false, false>;
-  static int attr[4] = {0, 0, 0, 0};   // dynamic shared memory each instance has been allowed so far
-  if (smem > attr[v]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) {
-      set_error("conv1d_tc: cudaFuncSetAttribute(%d bytes): %s", smem, cudaGetErrorString(e));
-      return 1;
-    }
-    attr[v] = smem;
-  }
+  p.stages = stages;
+  p.ops_bytes = (1 + (p.fm_d ? 1 : 0) + (p.res_bf16 ? 1 : 0)) * BLOCK_M * BN * 2;
+  p.ops_off = p.stages * L::STAGE_BYTES;
+  p.bar_off = p.ops_off + 2 * p.ops_bytes;
   // mask, skip and output boxes cover the tile's batch group; partner rows go one batch per box.  With fm_bh < 0
   // (the launch covers the fake half) the partner of batch b is batch b of the half stored right before dact_src.
   CUtensorMap tm, tp, tr, to;
@@ -810,128 +823,26 @@ static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, c
   if (encode_rows_map<BN>(&tm, p.dact_src, p, p.BB) || encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
   if (p.fm_d && encode_rows_map<BN>(&tp, p.fm_bh > 0 ? p.dact_src : p.dact_src - p.fm_half, p, 1)) return 1;
   if (p.res_bf16 && encode_rows_map<BN>(&tr, p.res_bf16, p, p.BB)) return 1;
-  const int tiles = p.n_lt * p.n_bg * p.n_nt;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = tiles < sms ? tiles : sms;
-  launch_pdl(kern, dim3(grid), dim3(PP_THREADS), smem, stream, ta, tb, tm, tp, tr, to, p);
-  RAVE_CHECK_LAUNCH("conv1d_tc");
-  return 0;
+  const int grid = persistent_grid(p.n_lt * p.n_bg * p.n_nt), smem = p.bar_off + L::FIXED;
+  const auto go = [&](auto fm, auto rs) {
+    return launch_tc<conv_tc_pp_kernel<BN, BK, decltype(fm)::value, decltype(rs)::value>>(
+        "conv1d_tc", grid, PP_THREADS, smem, stream, ta, tb, tm, tp, tr, to, p);
+  };
+  const std::true_type y;
+  const std::false_type n;
+  return p.fm_d ? (p.res_bf16 ? go(y, y) : go(y, n)) : (p.res_bf16 ? go(n, y) : go(n, n));
 }
-
-#ifndef RAVE_TC_X3_UNIT
-template <int BK>
-static int dispatch_pp_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
-  switch (bn) {
-    case 128: return launch_pp<128, BK>(ta, tb, p, s);
-    case 96:   // at BLOCK_K = 64 ptxas spills tile-loop invariants of every ping-pong instance: conv_tc_kernel runs it
-      if constexpr (BK == 64) return -1;
-      else return launch_pp<96, BK>(ta, tb, p, s);
-    case 64: return launch_pp<64, BK>(ta, tb, p, s);
-    case 48: return launch_pp<48, BK>(ta, tb, p, s);
-    case 32: return launch_pp<32, BK>(ta, tb, p, s);
-    case 16: return launch_pp<16, BK>(ta, tb, p, s);
-  }
-  set_error("conv1d_tc: no kernel for BLOCK_N=%d", bn);
-  return 1;
-}
-
-static int dispatch_pp(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
-  switch (BK) {
-    case 64: return dispatch_pp_n<64>(BN, ta, tb, p, s);
-    case 32: return dispatch_pp_n<32>(BN, ta, tb, p, s);
-    case 16: return dispatch_pp_n<16>(BN, ta, tb, p, s);
-  }
-  set_error("conv1d_tc: no kernel for BLOCK_K=%d", BK);
-  return 1;
-}
-
-// ring stages plan_smem_pp gives a ping-pong launch with nops operand tiles per slot; 0 = it runs conv_tc_kernel
-template <int BK>
-static int pp_stages(int BN, int nops) {
-  TcParams q;
-  bool ok = false;
-  switch (BN) {
-    case 128: ok = plan_smem_pp<128, BK>(nops, q); break;
-    case 96: ok = BK != 64 && plan_smem_pp<96, BK>(nops, q); break;    // see dispatch_pp_n
-    case 64: ok = plan_smem_pp<64, BK>(nops, q); break;
-    case 48: ok = plan_smem_pp<48, BK>(nops, q); break;
-    case 32: ok = plan_smem_pp<32, BK>(nops, q); break;
-    case 16: ok = plan_smem_pp<16, BK>(nops, q); break;
-  }
-  return ok ? q.stages : 0;
-}
-#endif
 
 template <int BN, int BK, bool X3>
 static int launch(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, cudaStream_t stream) {
   using L = SmemLayout<BN, BK, X3>;
   plan_smem<BN, BK, X3>(p.K * p.num_kb, p);
   if (!p.out_act) p.stg = 0;
-  const int smem = p.bar_off + L::FIXED;
-  static int attr = 0;              // dynamic shared memory this instance has been allowed so far
-  if (smem > attr) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, BK, X3>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) {
-      set_error("conv1d_tc: cudaFuncSetAttribute(%d bytes): %s", smem, cudaGetErrorString(e));
-      return 2;
-    }
-    attr = smem;
-  }
   CUtensorMap to;
   memset(&to, 0, sizeof(to));
   if (p.stg && encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
-  const int tiles = p.n_lt * p.n_bg * p.n_nt;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = tiles < sms ? tiles : sms;
-  launch_pdl(conv_tc_kernel<BN, BK, X3>, dim3(grid), dim3(NUM_THREADS), smem, stream, ta, tb, to, p);
-  RAVE_CHECK_LAUNCH("conv1d_tc");
-  return 0;
-}
-
-template <int BK, bool X3>
-static int dispatch_n(int bn, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p,
-                      cudaStream_t s) {
-  switch (bn) {
-    case 128: return launch<128, BK, X3>(ta, tb, p, s);
-    case 96: return launch<96, BK, X3>(ta, tb, p, s);
-    case 64: return launch<64, BK, X3>(ta, tb, p, s);
-    case 48: return launch<48, BK, X3>(ta, tb, p, s);
-    case 32: return launch<32, BK, X3>(ta, tb, p, s);
-    case 16: return launch<16, BK, X3>(ta, tb, p, s);
-  }
-  set_error("conv1d_tc: no kernel for BLOCK_N=%d", bn);
-  return 1;
-}
-
-// shared-memory split rave_conv1d_tc_plan reports (a launch that writes out_act)
-template <int BK>
-static int smem_plan_bits(int BN, int kblocks) {
-  TcParams q;
-  switch (BN) {
-    case 128: plan_smem<128, BK, false>(kblocks, q); break;
-    case 96: plan_smem<96, BK, false>(kblocks, q); break;
-    case 64: plan_smem<64, BK, false>(kblocks, q); break;
-    case 48: plan_smem<48, BK, false>(kblocks, q); break;
-    case 32: plan_smem<32, BK, false>(kblocks, q); break;
-    case 16: plan_smem<16, BK, false>(kblocks, q); break;
-    default: return 0;
-  }
-  return (q.nacc - 1) << 24 | q.stg << 25 | q.stages << 26;
-}
-
-template <bool X3>
-static int dispatch_all(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
-  switch (BK) {
-    case 64: return dispatch_n<64, X3>(BN, ta, tb, p, s);
-    case 32: return dispatch_n<32, X3>(BN, ta, tb, p, s);
-    case 16: return dispatch_n<16, X3>(BN, ta, tb, p, s);
-  }
-  set_error("conv1d_tc: no kernel for BLOCK_K=%d", BK);
-  return 1;
+  return launch_tc<conv_tc_kernel<BN, BK, X3>>("conv1d_tc", persistent_grid(p.n_lt * p.n_bg * p.n_nt), NUM_THREADS,
+                                               p.bar_off + L::FIXED, stream, ta, tb, to, p);
 }
 
 // The split-operand (x3) instantiations live in their own translation unit (conv_tc_x3.cu includes this file with
@@ -939,7 +850,9 @@ static int dispatch_all(int BK, int BN, const CUtensorMap &ta, const CUtensorMap
 int conv_tc_dispatch_x3(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s);
 #ifdef RAVE_TC_X3_UNIT
 int conv_tc_dispatch_x3(int BK, int BN, const CUtensorMap &ta, const CUtensorMap &tb, const TcParams &p, cudaStream_t s) {
-  return dispatch_all<true>(BK, BN, ta, tb, p, s);
+  return visit_tile(BK, BN, [&](auto bk, auto bn) {
+    return launch<decltype(bn)::value, decltype(bk)::value, true>(ta, tb, p, s);
+  });
 }
 #endif
 
@@ -957,29 +870,25 @@ extern "C" int rave_conv1d_tc_supported(int Cin, int Cout, int K, int stride, in
 // Which kernel instance rave_conv1d_tc_fwd runs for a shape (writing out_act): BLOCK_N | BLOCK_K << 12 |
 // (accumulator buffers - 1) << 24 | staged output << 25 | ring stages << 26; 0 = none.
 extern "C" int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K) {
-  using namespace rave;
   using namespace rave::tc;
-  const int BK = pick_block_k(Cin);
-  if (!BK || Cout % 16) return 0;
-  int BL = 128;
-  while (BL > Lout && BL > 8) BL >>= 1;
-  const long m_tiles = (long)ceil_div(Lout, BL) * ceil_div(B, 128 / BL);
-  const int BN = pick_block_n(Cout, m_tiles);
-  if (!BN) return 0;
-  const int kblocks = K * ceil_div(Cin, BK);
-  const int smem = BK == 64 ? smem_plan_bits<64>(BN, kblocks)
-                 : BK == 32 ? smem_plan_bits<32>(BN, kblocks) : smem_plan_bits<16>(BN, kblocks);
-  return BN | (BK << 12) | smem;
+  const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
+  if (!g.BK || !g.BN) return 0;
+  TcParams q;
+  visit_tile(g.BK, g.BN, [&](auto bk, auto bn) {
+    plan_smem<decltype(bn)::value, decltype(bk)::value, false>(K * g.num_kb, q);
+    return 0;
+  });
+  return g.BN | (g.BK << 12) | (q.nacc - 1) << 24 | q.stg << 25 | q.stages << 26;
 }
 
 // Ring stages of the ping-pong kernel for an input-gradient launch of this shape (LeakyReLU' mask, bf16 output only;
 // fm: with the feature-matching partner rows, res_bf16: with the gradient skip); 0 = the launch runs conv_tc_kernel.
 extern "C" int rave_conv1d_tc_pp_stages(int B, int Cin, int Cout, int Lout, int K, int fm, int res_bf16) {
   using namespace rave::tc;
-  const int plan = rave_conv1d_tc_plan(B, Cin, Cout, Lout, K);
-  const int BN = plan & 0xFFF, BK = (plan >> 12) & 0xFFF;
+  const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
+  if (!g.BK || !g.BN) return 0;
   const int nops = 1 + (fm ? 1 : 0) + (res_bf16 ? 1 : 0);
-  return BK == 64 ? pp_stages<64>(BN, nops) : BK == 32 ? pp_stages<32>(BN, nops) : BK == 16 ? pp_stages<16>(BN, nops) : 0;
+  return visit_tile(g.BK, g.BN, [&](auto bk, auto bn) { return pp_stages<decltype(bn)::value, decltype(bk)::value>(nops); });
 }
 
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,
@@ -1010,10 +919,11 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   RAVE_CHECK_ARG((((uintptr_t)out_f32 | (uintptr_t)out_act | (uintptr_t)res | (uintptr_t)res_bf16 | (uintptr_t)dact_src |
                    (uintptr_t)res_act) & 31) == 0,
                  "conv1d_tc: epilogue tensors must be 32-byte aligned (256-bit row segments)");
-  EncodeTiledFn enc = get_encode_fn();
-  RAVE_CHECK_ARG(enc, "conv1d_tc: cuTensorMapEncodeTiled not available");
+  RAVE_CHECK_ARG(get_encode_fn(), "conv1d_tc: cuTensorMapEncodeTiled not available");
 
-  const int BK = pick_block_k(Cin);
+  const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
+  RAVE_CHECK_ARG(g.BN > 0, "conv1d_tc: no BLOCK_N for Cout=%d", Cout);
+  const int BK = g.BK, BN = g.BN;
   // 256-byte L2 promotion over-fetches when a TMA row is a 64-byte (or shorter) span of a 192-byte channel row
   // (measured on the Cin = 96 layers: 209.6 -> 184.7 us); neutral to slightly positive for 128-byte spans.
   const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
@@ -1033,55 +943,45 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   p.fm_d = fm_d;
   p.fm_bh = fm_bh > 0 ? fm_bh : 0;                 // fm_bh < 0: every row is a fake row (partner |fm_bh| batches before)
   p.fm_half = (long)(fm_bh > 0 ? fm_bh : -fm_bh) * p.out_rows * Cout;
-  p.x3 = x3 ? 1 : 0;
   p.act_ld = x3 ? 2 * Cout : Cout;
   p.act_cs = act_cs > 0 ? act_cs : Cout;
   RAVE_CHECK_ARG(!x3 || (Cout % p.act_cs == 0 && p.act_cs % 16 == 0),
                  "conv1d_tc(x3): %d channels per position do not tile the %d-column rows in 16-column chunks", p.act_cs,
                  Cout);
   RAVE_CHECK_ARG(!x3 || !res_act || p.act_cs == Cout, "conv1d_tc(x3): res_act needs one position per row");
-  int BL = 128;
-  while (BL > Lout && BL > 8) BL >>= 1;   // power of two <= max(Lout, 8)
-  p.BL = BL; p.BB = 128 / BL;
-  p.n_lt = ceil_div(Lout, BL);
-  p.n_bg = ceil_div(B, p.BB);
-  const int BN = pick_block_n(Cout, (long)p.n_lt * p.n_bg);
-  RAVE_CHECK_ARG(BN > 0, "conv1d_tc: no BLOCK_N for Cout=%d", Cout);
-  p.n_nt = Cout / BN;
-  p.num_kb = ceil_div(Cin, BK);
+  p.BL = g.BL; p.BB = g.BB; p.n_lt = g.n_lt; p.n_bg = g.n_bg; p.n_nt = g.n_nt; p.num_kb = g.num_kb;
 
   // A: channel-last activations viewed as (c, phase, l/stride, b)
   CUtensorMap ta, tb;
   {
     const cuuint64_t ca = (cuuint64_t)Cin * (x3 ? 2 : 1);       // channels per activation row ([hi | lo] in x3 mode)
-    cuuint64_t dims[4] = {ca, (cuuint64_t)stride, (cuuint64_t)ceil_div(Lin, stride), (cuuint64_t)B};
-    cuuint64_t strides[3] = {ca * 2, ca * 2 * stride, ca * 2 * in_pitch};
-    cuuint32_t box[4] = {(cuuint32_t)BK, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xa), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(BK * 2), promo,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[4] = {ca, (cuuint64_t)stride, (cuuint64_t)ceil_div(Lin, stride), (cuuint64_t)B};
+    const cuuint64_t strides[3] = {ca * 2, ca * 2 * stride, ca * 2 * in_pitch};
+    const cuuint32_t box[4] = {(cuuint32_t)BK, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
+    const CUresult r = encode_bf16_map(&ta, 4, xa, dims, strides, box, swizzle_enum(BK * 2), promo);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "conv1d_tc: tensor map A encode failed (%d)", (int)r);
   }
   {
-    cuuint64_t dims[2] = {(cuuint64_t)Cin, (cuuint64_t)K * Cout * (x3 ? 2 : 1)};
-    cuuint64_t strides[1] = {(cuuint64_t)Cin * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BN};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&tb, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void *>(wt), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle_enum(BK * 2), promo,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[2] = {(cuuint64_t)Cin, (cuuint64_t)K * Cout * (x3 ? 2 : 1)};
+    const cuuint64_t strides[1] = {(cuuint64_t)Cin * 2};
+    const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)BN};
+    const CUresult r = encode_bf16_map(&tb, 2, wt, dims, strides, box, swizzle_enum(BK * 2), promo);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "conv1d_tc: tensor map B encode failed (%d)", (int)r);
   }
   cudaStream_t s = (cudaStream_t)stream;
   if (x3) return conv_tc_dispatch_x3(BK, BN, ta, tb, p, s);
   // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only): the
-  // ping-pong kernel, unless its operand slots leave no room for the ring
-  if (dact_src && out_act && !bias && !res && !res_act && !out_f32 && act == RAVE_ACT_NONE) {
-    const int r = dispatch_pp(BK, BN, ta, tb, p, s);
-    if (r >= 0) return r;
-  }
-  return dispatch_all<false>(BK, BN, ta, tb, p, s);
+  // ping-pong kernel where pp_stages gives it the launch
+  const bool pp = dact_src && out_act && !bias && !res && !res_act && !out_f32 && act == RAVE_ACT_NONE;
+  const int nops = 1 + (fm_d ? 1 : 0) + (res_bf16 ? 1 : 0);
+  return visit_tile(BK, BN, [&](auto bk, auto bn) {
+    constexpr int BK_ = decltype(bk)::value, BN_ = decltype(bn)::value;
+    if constexpr (pp_built<BN_, BK_>) {
+      const int stages = pp ? pp_stages<BN_, BK_>(nops) : 0;
+      if (stages) return launch_pp<BN_, BK_>(ta, tb, p, stages, s);
+    }
+    return launch<BN_, BK_, false>(ta, tb, p, s);
+  });
 }
 
 extern "C" int rave_conv1d_tc_fwd(const void *xa, const void *wt, const float *bias, const float *res,
@@ -1198,10 +1098,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
   if (my_chunks > 0) {
     if (warp == 4) {
       // warp-uniform producer loop (see elect_one)
-      const int off = k * p.dil - p.pad_l;
-      int j = off / p.stride;
-      int ph = off - j * p.stride;
-      if (ph < 0) { ph += p.stride; j -= 1; }
+      const TapOrigin o = tap_origin(k, p.dil, p.pad_l, p.stride);
       int stage = 0;
       uint32_t phase = 0;
       for (int ch = ch_begin; ch < ch_end; ++ch) {
@@ -1216,7 +1113,7 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
           tma_load_4d(sa + WG_SLAB, &tmap_p, &full_bar[stage], m0 + 64, 0, l0, b0);
 #pragma unroll
           for (int s = 0; s < NS; ++s)
-            tma_load_4d(sb + s * WG_SLAB, &tmap_q, &full_bar[stage], n0 + 64 * s, ph, l0 + j, b0);
+            tma_load_4d(sb + s * WG_SLAB, &tmap_q, &full_bar[stage], n0 + 64 * s, o.ph, l0 + o.j, b0);
         }
         __syncwarp();
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
@@ -1321,22 +1218,11 @@ tapmajor_to_weight_kernel(const float *__restrict__ dwt, float *__restrict__ dw,
   }
 }
 
+// one CTA per (tap, m-tile, n-tile, split)
 template <int BN>
 static int launch_wg(const CUtensorMap &tp, const CUtensorMap &tq, const WgParams &p, cudaStream_t stream) {
-  using L = WgSmem<BN>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL);
-    if (e != cudaSuccess) {
-      set_error("wgrad_tc: cudaFuncSetAttribute(%d bytes): %s", L::TOTAL, cudaGetErrorString(e));
-      return 2;
-    }
-    attr = true;
-  }
-  const int grid = p.K * p.n_mt * p.n_nt * p.splits;
-  launch_pdl(wgrad_tc_kernel<BN>, dim3(grid), dim3(NUM_THREADS), L::TOTAL, stream, tp, tq, p);
-  RAVE_CHECK_LAUNCH("wgrad_tc");
-  return 0;
+  return launch_tc<wgrad_tc_kernel<BN>>("wgrad_tc", p.K * p.n_mt * p.n_nt * p.splits, NUM_THREADS, WgSmem<BN>::TOTAL,
+                                        stream, tp, tq, p);
 }
 
 }  // namespace tc
@@ -1390,8 +1276,7 @@ extern "C" int rave_conv1d_tc_wgrad(const void *P, const void *Q, float *dwt, fl
   RAVE_CHECK_ARG(q_pitch >= ceil_div(Lq, stride) * stride,
                  "wgrad_tc: Q pitch %d < Lq %d rounded up to the stride %d (slack rows must be zero)", q_pitch, Lq,
                  stride);
-  EncodeTiledFn enc = get_encode_fn();
-  RAVE_CHECK_ARG(enc, "wgrad_tc: cuTensorMapEncodeTiled not available");
+  RAVE_CHECK_ARG(get_encode_fn(), "wgrad_tc: cuTensorMapEncodeTiled not available");
   cudaStream_t s = (cudaStream_t)stream;
 
   WgParams p;
@@ -1403,24 +1288,19 @@ extern "C" int rave_conv1d_tc_wgrad(const void *P, const void *Q, float *dwt, fl
   p.BB = WG_ROWS / p.BL;
 
   CUtensorMap tp, tq;
+  const cuuint32_t box[4] = {64, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
   {
-    cuuint64_t dims[4] = {(cuuint64_t)Cm, 1, (cuuint64_t)Lp, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)Cm * 2, (cuuint64_t)Cm * 2, (cuuint64_t)Cm * 2 * p_pitch};
-    cuuint32_t box[4] = {64, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tp, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(P), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[4] = {(cuuint64_t)Cm, 1, (cuuint64_t)Lp, (cuuint64_t)B};
+    const cuuint64_t strides[3] = {(cuuint64_t)Cm * 2, (cuuint64_t)Cm * 2, (cuuint64_t)Cm * 2 * p_pitch};
+    const CUresult r = encode_bf16_map(&tp, 4, P, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "wgrad_tc: tensor map P encode failed (%d)", (int)r);
   }
   {
-    cuuint64_t dims[4] = {(cuuint64_t)Cn, (cuuint64_t)stride, (cuuint64_t)ceil_div(Lq, stride), (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)Cn * 2, (cuuint64_t)Cn * 2 * stride, (cuuint64_t)Cn * 2 * q_pitch};
-    cuuint32_t box[4] = {64, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&tq, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(Q), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[4] = {(cuuint64_t)Cn, (cuuint64_t)stride, (cuuint64_t)ceil_div(Lq, stride), (cuuint64_t)B};
+    const cuuint64_t strides[3] = {(cuuint64_t)Cn * 2, (cuuint64_t)Cn * 2 * stride, (cuuint64_t)Cn * 2 * q_pitch};
+    const CUresult r = encode_bf16_map(&tq, 4, Q, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B,
+                                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "wgrad_tc: tensor map Q encode failed (%d)", (int)r);
   }
   p.dbias_part = nullptr;

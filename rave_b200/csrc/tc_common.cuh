@@ -8,6 +8,9 @@
 #include <stdint.h>
 #include <string.h>
 
+#include <utility>
+
+#include "common.cuh"
 #include "wgmma_sm90.cuh"
 
 namespace rave {
@@ -77,8 +80,6 @@ __device__ __forceinline__ void stg256(void *p, const uint32_t *r) {
                : "memory");
 }
 
-__device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
-
 // One lane of a fully converged warp.  The producer loops run WARP-UNIFORM (all 32 lanes execute the loop, only the
 // TMA instructions are predicated on the elected lane): stage indices, shared-memory addresses and coordinates then
 // live in uniform registers instead of being broadcast from one lane per instruction.
@@ -119,11 +120,6 @@ __device__ __forceinline__ void tma_load_3d(void *smem, const CUtensorMap *m, ui
       ::"r"(smem_u32(smem)), "l"(m), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
 }
-// pull a box into L2 only (no shared-memory destination, no barrier): hides the HBM latency of a later tma_load_3d
-__device__ __forceinline__ void tma_prefetch_3d(const CUtensorMap *m, int c0, int c1, int c2) {
-  asm volatile("cp.async.bulk.prefetch.tensor.3d.L2.global [%0, {%1, %2, %3}];" ::"l"(m), "r"(c0), "r"(c1), "r"(c2)
-               : "memory");
-}
 __device__ __forceinline__ void tma_store_3d(const CUtensorMap *m, const void *smem, int c0, int c1, int c2) {
   asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];" ::"l"(m),
                "r"(smem_u32(smem)), "r"(c0), "r"(c1), "r"(c2)
@@ -142,10 +138,6 @@ __device__ __forceinline__ void bulk_wait_read() {      // at most N bulk groups
 __device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
-}
-__device__ __forceinline__ void lds128(const void *p, uint32_t *r) {
-  asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
-               : "r"(smem_u32(p)));
 }
 __device__ __forceinline__ void sts128(void *p, const uint32_t *r) {
   asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(smem_u32(p)), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
@@ -263,9 +255,6 @@ __global__ void __launch_bounds__(256) dbias_sum_kernel(const float *__restrict_
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void griddep_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-#ifndef __CUDA_ARCH__
-#include <utility>
-#endif
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                                      Args &&...args) {
@@ -285,6 +274,61 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
 #else
   return cudaSuccess;
 #endif
+}
+
+// Grid of a persistent kernel: one CTA per SM, fewer when there are fewer tiles.
+static inline int persistent_grid(int tiles) {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  return tiles < sms ? tiles : sms;
+}
+
+// launch_pdl of Kernel with `smem` bytes of dynamic shared memory (the opt-in is raised once per new maximum of the
+// instance); 0 = launched, 2 = CUDA error (message under `name`).
+template <auto Kernel, typename... Args>
+static int launch_tc(const char *name, int grid, int threads, int smem, cudaStream_t stream, Args &&...args) {
+  static int allowed = 0;
+  if (smem > allowed) {
+    cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) {
+      set_error("%s: cudaFuncSetAttribute(%d bytes): %s", name, smem, cudaGetErrorString(e));
+      return 2;
+    }
+    allowed = smem;
+  }
+  launch_pdl(Kernel, dim3(grid), dim3(threads), smem, stream, std::forward<Args>(args)...);
+  RAVE_CHECK_LAUNCH(name);
+  return 0;
+}
+
+// ------------------------------------------------------------------ tensor maps
+typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
+                                  const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
+                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion,
+                                  CUtensorMapFloatOOBfill);
+
+// cuTensorMapEncodeTiled from the driver the runtime uses (null if it has none)
+static inline EncodeTiledFn get_encode_fn() {
+  static EncodeTiledFn fn = nullptr;
+  if (!fn) {
+    void *ptr = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = (EncodeTiledFn)ptr;
+  }
+  return fn;
+}
+
+// Tiled map of a bf16 tensor of `rank` dimensions (innermost first; strides in bytes of dimensions 1 ..), dense
+// boxes, out-of-range elements zero-filled.  The caller has checked get_encode_fn().
+static inline CUresult encode_bf16_map(CUtensorMap *m, int rank, const void *base, const cuuint64_t *dims,
+                                       const cuuint64_t *strides, const cuuint32_t *box, CUtensorMapSwizzle swizzle,
+                                       CUtensorMapL2promotion promo) {
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  return get_encode_fn()(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void *>(base), dims, strides,
+                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
 }
 
 // ------------------------------------------------------------------ descriptors

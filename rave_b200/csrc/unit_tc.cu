@@ -556,44 +556,11 @@ dilated_unit_ws_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_
   if (issuer) bulk_wait_all();
 }
 
-typedef CUresult (*EncodeTiledFnU)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *,
-                                   const cuuint64_t *, const cuuint32_t *, const cuuint32_t *, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFnU unit_encode_fn() {
-  static EncodeTiledFnU fn = nullptr;
-  if (!fn) {
-    void *ptr = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = (EncodeTiledFnU)ptr;
-  }
-  return fn;
-}
-
 template <int C, int BK, int NC>
 static int launch_unit(const CUtensorMap &ta, const CUtensorMap &t3, const CUtensorMap &t1, const UnitParams &p,
                        cudaStream_t stream) {
-  using L = UnitCfg<C, BK, NC>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dilated_unit_tc_kernel<C, BK, NC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         L::TOTAL);
-    if (e != cudaSuccess) {
-      set_error("dilated_unit_tc: cudaFuncSetAttribute(%d bytes): %s", L::TOTAL, cudaGetErrorString(e));
-      return 2;
-    }
-    attr = true;
-  }
-  const int tiles = p.n_lt * p.n_bg;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  const int grid = tiles < sms ? tiles : sms;
-  launch_pdl(dilated_unit_tc_kernel<C, BK, NC>, dim3(grid), dim3(U_THREADS), L::TOTAL, stream, ta, t3, t1, p);
-  RAVE_CHECK_LAUNCH("dilated_unit_tc");
-  return 0;
+  return launch_tc<dilated_unit_tc_kernel<C, BK, NC>>("dilated_unit_tc", persistent_grid(p.n_lt * p.n_bg), U_THREADS,
+                                                      UnitCfg<C, BK, NC>::TOTAL, stream, ta, t3, t1, p);
 }
 
 // N chunk of dilated_unit_tc_kernel per width.  NC = 128 would need 128 accumulator registers per MMA thread on top of
@@ -604,25 +571,8 @@ static int unit_chunk(int C) { return C % 96 == 0 ? 96 : 64; }
 template <int C>
 static int launch_unit_ws(const CUtensorMap &ta, const CUtensorMap &t3, const CUtensorMap &t1, const CUtensorMap &tout,
                           const CUtensorMap &ta1, const UnitParams &p, cudaStream_t stream) {
-  using W = UwCfg<C>;
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(dilated_unit_ws_kernel<C>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         W::TOTAL);
-    if (e != cudaSuccess) {
-      set_error("dilated_unit_tc(ws): cudaFuncSetAttribute(%d bytes): %s", W::TOTAL, cudaGetErrorString(e));
-      return 2;
-    }
-    attr = true;
-  }
-  const int tiles = p.n_lt * p.n_bg;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-  launch_pdl(dilated_unit_ws_kernel<C>, dim3(tiles < sms ? tiles : sms), dim3(UW_THREADS), W::TOTAL, stream, ta, t3,
-             t1, tout, ta1, p);
-  RAVE_CHECK_LAUNCH("dilated_unit_tc(ws)");
-  return 0;
+  return launch_tc<dilated_unit_ws_kernel<C>>("dilated_unit_tc(ws)", persistent_grid(p.n_lt * p.n_bg), UW_THREADS,
+                                             UwCfg<C>::TOTAL, stream, ta, t3, t1, tout, ta1, p);
 }
 
 }  // namespace tc
@@ -648,8 +598,7 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
   RAVE_CHECK_ARG(act_out == RAVE_ACT_NONE || act_out == RAVE_ACT_LEAKY, "dilated_unit_tc: output activation %d", act_out);
   RAVE_CHECK_ARG((((uintptr_t)xa | (uintptr_t)a1_out | (uintptr_t)out_f32 | (uintptr_t)out_act) & 31) == 0 &&
                      (((uintptr_t)w3t | (uintptr_t)w1t) & 15) == 0, "dilated_unit_tc: tensors must be 32-byte aligned");
-  EncodeTiledFnU enc = unit_encode_fn();
-  RAVE_CHECK_ARG(enc, "dilated_unit_tc: cuTensorMapEncodeTiled not available");
+  RAVE_CHECK_ARG(get_encode_fn(), "dilated_unit_tc: cuTensorMapEncodeTiled not available");
   const int BK = C % 64 == 0 ? 64 : 32;
   UnitParams p;
   p.B = B; p.C = C; p.L = L; p.pitch = pitch; p.dil = dil; p.pad_l = pad_l;
@@ -669,24 +618,20 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
   const CUtensorMapSwizzle swz = BK == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
   const int NC = unit_chunk(C);
+  // [B][pitch][C] operand rows viewed as (c, 1, row, b); weights [taps * C][C]
+  const cuuint64_t adims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
+  const cuuint64_t astrides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
+  const cuuint64_t wstrides[1] = {(cuuint64_t)C * 2};
   CUtensorMap ta, t3, t1;
   {
-    cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
-    cuuint32_t box[4] = {(cuuint32_t)BK, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(&ta, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xa), dims, strides, box, estr,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint32_t box[4] = {(cuuint32_t)BK, 1, (cuuint32_t)p.BL, (cuuint32_t)p.BB};
+    const CUresult r = encode_bf16_map(&ta, 4, xa, adims, astrides, box, swz, promo);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc: tensor map A encode failed (%d)", (int)r);
   }
   for (int which = 0; which < 2; ++which) {
-    cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
-    cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-    cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)NC};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(which == 0 ? &t3 : &t1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                     const_cast<void *>(which == 0 ? w3t : w1t), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     swz, promo, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
+    const cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)NC};
+    const CUresult r = encode_bf16_map(which == 0 ? &t3 : &t1, 2, which == 0 ? w3t : w1t, dims, wstrides, box, swz, promo);
     RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc: weight tensor map encode failed (%d)", (int)r);
   }
   cudaStream_t s = (cudaStream_t)stream;
@@ -695,23 +640,16 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
     // (tap, K block) slab per box
     CUtensorMap tah, t3s, t1s;
     {
-      cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
-      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
-      cuuint32_t box[4] = {32, 1, (cuuint32_t)(128 + 2 * dil), 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(&tah, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void *>(xa), dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      const cuuint32_t box[4] = {32, 1, (cuuint32_t)(128 + 2 * dil), 1};
+      const CUresult r = encode_bf16_map(&tah, 4, xa, adims, astrides, box, CU_TENSOR_MAP_SWIZZLE_64B,
+                                         CU_TENSOR_MAP_L2_PROMOTION_NONE);
       RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): tensor map A encode failed (%d)", (int)r);
     }
     for (int which = 0; which < 2; ++which) {
-      cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
-      cuuint64_t strides[1] = {(cuuint64_t)C * 2};
-      cuuint32_t box[2] = {32, (cuuint32_t)C};
-      cuuint32_t estr[2] = {1, 1};
-      CUresult r = enc(which == 0 ? &t3s : &t1s, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
-                       const_cast<void *>(which == 0 ? w3t : w1t), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      const cuuint64_t dims[2] = {(cuuint64_t)C, (cuuint64_t)(which == 0 ? 3 : 1) * C};
+      const cuuint32_t box[2] = {32, (cuuint32_t)C};
+      const CUresult r = encode_bf16_map(which == 0 ? &t3s : &t1s, 2, which == 0 ? w3t : w1t, dims, wstrides, box,
+                                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
       RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): weight tensor map encode failed (%d)", (int)r);
     }
     // bf16 outputs leave through TMA: [B][pitch][C] viewed as (c, 1, row, b) boxes of one 32-channel K block x 128 rows
@@ -722,13 +660,9 @@ extern "C" int rave_dilated_unit_tc_fwd(const void *xa, const void *w3t, const v
     for (int which = 0; which < 2; ++which) {
       void *base = which == 0 ? out_act : a1_out;
       if (!base) continue;
-      cuuint64_t dims[4] = {(cuuint64_t)C, 1, (cuuint64_t)L, (cuuint64_t)B};
-      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)C * 2, (cuuint64_t)C * 2 * pitch};
-      cuuint32_t box[4] = {32, 1, 128, 1};
-      cuuint32_t estr[4] = {1, 1, 1, 1};
-      CUresult r = enc(which == 0 ? &tout : &ta1, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, estr,
-                       CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      const cuuint32_t box[4] = {32, 1, 128, 1};
+      const CUresult r = encode_bf16_map(which == 0 ? &tout : &ta1, 4, base, adims, astrides, box,
+                                         CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_NONE);
       RAVE_CHECK_ARG(r == CUDA_SUCCESS, "dilated_unit_tc(ws): output tensor map encode failed (%d)", (int)r);
     }
     return C == 64 ? launch_unit_ws<64>(tah, t3s, t1s, tout, ta1, p, s) : launch_unit_ws<96>(tah, t3s, t1s, tout, ta1, p, s);
