@@ -16,10 +16,10 @@ import torch.nn.functional as F
 
 from . import _lib, ops
 from .blocks import weight_norm
-from .discriminator import DiscConv2dK1
+from .discriminator import DiscConv2dK1, TimeStackedConv2d, _feature_tap, _feature_tap_stack
 
 # MRD feature taps also write the next conv's time-stacked operand in the same pass where the geometry allows it
-# (_feature_tap_stack); False runs the tap and the stacking as separate passes
+# (discriminator._feature_tap_stack); False runs the tap and the stacking as separate passes
 FUSE_TAP_STACK = True
 
 
@@ -32,10 +32,12 @@ def WNConv2dK1(*args, **kwargs):
     return nn.Sequential(conv, nn.LeakyReLU(0.1))
 
 
-class DiscConv2d(nn.Conv2d):
+class DiscConv2d(TimeStackedConv2d):
     """nn.Conv2d with kernel (kt, kf), stride (1, sf), padding (pt, pf) on the library's conv1d kernel: the kt time taps
-    become kt x Cin input channels of a conv along frequency (rows = (batch, time) pairs).  Same parameters / state_dict
-    keys as nn.Conv2d; input and output are [B, C, T, F] tensors."""
+    become kt x Cin input channels of a conv along frequency (rows = (batch, time) pairs: TimeStackedConv2d, time on the
+    first axis).  Same parameters / state_dict keys as nn.Conv2d; input and output are [B, C, T, F] tensors."""
+
+    TIME_AXIS = 0
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
@@ -57,43 +59,6 @@ class DiscConv2d(nn.Conv2d):
         y = ops.conv1d(xi, w, self.bias, None, self.stride[1], 1, (pf, pf), ops.ACT_NONE, 0.0, None)
         return y.view(B, T, self.out_channels, y.shape[-1]).permute(0, 2, 1, 3)
 
-    def _tc_chain_spec(self, C):
-        """One-layer engine chain of this conv along frequency; the (dt, c) channel order is a permuted VIEW of the
-        parameter, so the weight-norm backward of the chain reaches weight_v / weight_g through autograd."""
-        from . import engine
-        kt, kf = self.kernel_size
-        pt, pf = self.padding
-        cin = kt * C
-        proxy = self.__dict__.get("_tc_proxy")
-        if proxy is None:
-            proxy = self.__dict__["_tc_proxy"] = _ParamView()
-            if self.__dict__.get("_tc_proxy_static"):       # engine.enable_static_prep ran before the first forward
-                proxy.__dict__["_tc_static"] = {}
-            spec = engine.LayerSpec("conv", proxy, cin, self.out_channels, kf, self.stride[1], 1, (pf, pf),
-                                    ops.ACT_NONE, 0.0, None, True, True)
-            spec.cin_pad = (-cin) % 16
-            spec.cout_pad = (-self.out_channels) % 16
-            self.__dict__["_tc_spec"] = spec
-        spec = self.__dict__["_tc_spec"]
-        if spec.Cin != cin:
-            raise _lib.RaveB200Error(f"DiscConv2d: planned for {spec.Cin // kt} input channels, called with {C}")
-        self._tc_refresh_proxy()
-        return spec
-
-    def _tc_refresh_proxy(self):
-        """(Re)build the proxy's (dt, c)-ordered views of the parameters (a permuted reshape is a copy: it goes stale
-        when the parameters move, so engine.refresh_static_prep calls this before it rewrites the static layouts)."""
-        proxy = self.__dict__["_tc_proxy"]
-        kf = self.kernel_size[1]
-        co = self.out_channels
-        cin = self.__dict__["_tc_spec"].Cin
-        if hasattr(self, "weight_v"):
-            proxy.weight_v = self.weight_v.permute(0, 2, 1, 3).reshape(co, cin, kf)
-            proxy.weight_g = self.weight_g.reshape(co, 1, 1)
-        else:
-            proxy.weight = self.weight.permute(0, 2, 1, 3).reshape(co, cin, kf)
-        proxy.bias = self.bias
-
     def _forward_tc(self, x, B, C, T, Fq):
         """bf16 mode: the same conv along frequency as a one-layer chain of the wgmma engine (forward, dgrad and wgrad
         on the tensor cores; 23 % of the v3 discriminator FLOPs ran on the fp32 CUDA-core kernels: 176 ms of a 280 ms
@@ -108,65 +73,10 @@ class DiscConv2d(nn.Conv2d):
         Fo = engine.chain_lengths([spec], Fq)[0]
         return out[:, :Fo, :co].reshape(B, T, Fo, co).permute(0, 3, 1, 2)
 
-    def cout_ok(self) -> bool:
-        return self.out_channels % 16 == 0
-
     def tc_ready(self, x, C) -> bool:
         from . import engine
         return (engine.precision() == "bf16" and x.is_cuda and engine.ACT_DTYPE == torch.bfloat16
                 and self.kernel_size[0] * C <= 112)
-
-    def stacked_geometry(self, Fq: int, C: int):
-        """(Fp, Cp) of this conv's time-stacked operand for an input of Fq positions and C channels."""
-        spec = self._tc_chain_spec(C)
-        return Fq + (-Fq) % spec.stride, self.kernel_size[0] * C + spec.cin_pad
-
-    def forward_cl(self, x_cl, xs=None):
-        """Channel-last in, channel-last out: x_cl [B, T, F, C] fp32 (a view with dense (f, c) rows) -> the chain's own
-        output buffer [(b t), Fo, Cout(+pad to 16)] fp32, which IS [B, T, Fo, Cout] channel-last: no layout pass on
-        either side of the conv.  `xs`: the time-stacked bf16 operand when the producer already wrote it
-        (ops.leaky_fm_stack: the previous layer's feature tap)."""
-        from . import engine
-        B, T, Fq, C = x_cl.shape
-        spec = self._tc_chain_spec(C)
-        kt, pt = self.kernel_size[0], self.padding[0]
-        Fp, Cp = self.stacked_geometry(Fq, C)
-        if xs is None:
-            xs = ops.time_stack_nhwc(x_cl, kt, pt, Cp, Fp)
-        elif tuple(xs.shape) != (B * T, Fp, Cp) or xs.dtype != engine.ACT_DTYPE:
-            raise _lib.RaveB200Error("DiscConv2d.forward_cl: the pre-stacked operand does not match this conv's geometry")
-        (out,) = engine.run_chain(xs, [spec], Fq)
-        Fo = engine.chain_lengths([spec], Fq)[0]
-        if out.shape[1] != Fo:
-            raise _lib.RaveB200Error("DiscConv2d: the one-layer chain's output pitch is its length")
-        return out
-
-
-def _feature_tap(out, slope, B):
-    """Post-activation feature of a chain output (rows = [real; fake] when the batch B is even): LeakyReLU and the two L1
-    feature-matching sums in one pass (ops.leaky_fm), or the plain activation for an unpaired batch."""
-    if B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous():
-        return ops.leaky_fm(out, slope)
-    return ops.activation(out, ops.ACT_LEAKY, slope), None
-
-
-def _feature_tap_stack(out, slope, B, T, nxt):
-    """_feature_tap that also writes the time-stacked operand of the next MRD conv `nxt` (a DiscConv2d) in the same pass,
-    when the geometry allows it (kt = 3, pt = 1, no channel padding on either side): returns (a, stats, xs | None)."""
-    C = out.shape[2]
-    if (FUSE_TAP_STACK and nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous()
-            and nxt.kernel_size[0] == 3 and nxt.padding[0] == 1 and nxt.in_channels == C and C % 4 == 0
-            and out.shape[0] == B * T):
-        Fp, Cp = nxt.stacked_geometry(out.shape[1], C)
-        if Cp == 3 * C:
-            return ops.leaky_fm_stack(out, slope, T, Fp)
-    a, st = _feature_tap(out, slope, B)
-    return a, st, None
-
-
-class _ParamView:
-    """Attribute holder standing in for a conv module inside a one-layer engine chain (engine._layer_params reads
-    weight_v / weight_g / bias or weight / bias; the prepared-weight cache lives in its __dict__)."""
 
 
 def WNConv2d(*args, **kwargs):
@@ -317,7 +227,7 @@ class MRD(nn.Module):
                 out = conv.forward_cl(cur, xs_next)                          # [(b t), Fo, 32]
                 # the tap of every layer but the stack's last also writes the next conv's time-stacked operand
                 nxt = stack[li + 1][0] if li + 1 < len(stack) else None
-                a, st, xs_next = _feature_tap_stack(out, layer[1].negative_slope, B, t, nxt)
+                a, st, xs_next = _feature_tap_stack(out, layer[1].negative_slope, B, t, nxt, FUSE_TAP_STACK)
                 cur = a.view(B, t, out.shape[1], out.shape[2])
                 feat = cur.permute(0, 3, 1, 2)
                 feat._cl_base = a

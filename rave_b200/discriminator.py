@@ -52,6 +52,108 @@ class DiscConv2dK1(nn.Conv2d):
         return y.view(B, W, y.shape[1], y.shape[2]).permute(0, 2, 3, 1)
 
 
+class TimeStackedConv2d(nn.Conv2d):
+    """nn.Conv2d with unit time stride and 'same' time padding whose kt time taps (time t + j dt - pt for tap j) become
+    kt x Cin input channels of ONE conv along frequency over rows (b, t): in bf16 mode a one-layer chain of the wgmma
+    engine (forward, dgrad and wgrad on the tensor cores), channel-last on both sides.  Subclasses say which axis of
+    kernel_size / padding / stride / dilation is time, check their arguments and keep their fp32 `forward`."""
+
+    TIME_AXIS: int            # set by the subclass: 0 or 1, frequency is the other one
+
+    def cout_ok(self) -> bool:
+        return self.out_channels % 16 == 0
+
+    def _tc_chain_spec(self, C):
+        """One-layer engine chain of this conv along frequency, planned on an engine.ParamProxy: the (j, c) channel
+        order is a permuted VIEW of the parameter, so the weight-norm backward of the chain reaches weight_v / weight_g
+        through autograd."""
+        from . import engine
+        t, f = self.TIME_AXIS, 1 - self.TIME_AXIS
+        kt, pf = self.kernel_size[t], self.padding[f]
+        cin = kt * C
+        proxy = self.__dict__.get("_tc_proxy")
+        if proxy is None:
+            spec = engine.LayerSpec("conv", None, cin, self.out_channels, self.kernel_size[f], self.stride[f], 1, (pf, pf),
+                                    ops.ACT_NONE, 0.0, None, True, True)
+            spec.cin_pad = (-cin) % 16
+            spec.cout_pad = (-self.out_channels) % 16
+            proxy = engine.ParamProxy(self, spec, self._tc_refresh_proxy)
+        if proxy.spec.Cin != cin:
+            raise RaveB200Error(f"{type(self).__name__}: planned for {proxy.spec.Cin // kt} input channels, called "
+                                f"with {C}")
+        self._tc_refresh_proxy()
+        return proxy.spec
+
+    def _tc_refresh_proxy(self):
+        """(Re)build the proxy's (j, c)-ordered views of the parameters (a permuted reshape is a copy: it goes stale
+        when the parameters move, so engine.refresh_static_prep calls this before it rewrites the static layouts)."""
+        proxy = self.__dict__["_tc_proxy"]
+        t, f = self.TIME_AXIS, 1 - self.TIME_AXIS
+        shape = (self.out_channels, proxy.spec.Cin, self.kernel_size[f])
+        order = (0, 2 + t, 1, 2 + f)                      # [Cout][Cin][.][.] -> [Cout][kt][Cin][kf]
+        if hasattr(self, "weight_v"):
+            proxy.weight_v = self.weight_v.permute(order).reshape(shape)
+            proxy.weight_g = self.weight_g.reshape(self.out_channels, 1, 1)
+        else:
+            proxy.weight = self.weight.permute(order).reshape(shape)
+        proxy.bias = self.bias
+
+    def stacked_geometry(self, Fq: int, C: int):
+        """(Fp, Cp) of this conv's time-stacked operand for an input of Fq positions and C channels."""
+        spec = self._tc_chain_spec(C)
+        return Fq + (-Fq) % spec.stride, self.kernel_size[self.TIME_AXIS] * C + spec.cin_pad
+
+    def forward_cl(self, x_cl, xs=None):
+        """Channel-last in, channel-last out: x_cl [B, T, F, C] fp32 (a view with dense (f, c) rows) -> the chain's own
+        output buffer [(b t), Fo, Cout(+pad to 16)] fp32, which IS [B, T, Fo, Cout] channel-last: no layout pass on
+        either side of the conv.  `xs`: the time-stacked bf16 operand when the producer already wrote it
+        (ops.leaky_fm_stack: the previous layer's feature tap)."""
+        from . import engine
+        B, T, Fq, C = x_cl.shape
+        spec = self._tc_chain_spec(C)
+        t = self.TIME_AXIS
+        Fp, Cp = self.stacked_geometry(Fq, C)
+        if xs is None:
+            xs = ops.time_stack_nhwc(x_cl, self.kernel_size[t], self.padding[t], Cp, Fp, *_dil_arg(self.dilation[t]))
+        elif tuple(xs.shape) != (B * T, Fp, Cp) or xs.dtype != engine.ACT_DTYPE:
+            raise RaveB200Error(f"{type(self).__name__}.forward_cl: the pre-stacked operand does not match this conv's "
+                                f"geometry")
+        (out,) = engine.run_chain(xs, [spec], Fq)
+        if out.shape[1] != engine.chain_lengths([spec], Fq)[0]:
+            raise RaveB200Error(f"{type(self).__name__}: the one-layer chain's output pitch is its length")
+        return out
+
+
+def _dil_arg(dt: int):
+    """Trailing time-dilation argument of ops.time_stack_nhwc / ops.leaky_fm_stack: left out when it is 1, their default
+    (the CPU emulation of these two calls, tests/tc_emulator.py, takes no dilation)."""
+    return () if dt == 1 else (dt,)
+
+
+def _feature_tap(out, slope, B):
+    """Post-activation feature of a chain output (rows = [real; fake] when the batch B is even): LeakyReLU and the two L1
+    feature-matching sums in one pass (ops.leaky_fm), or the plain activation for an unpaired batch."""
+    if B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous():
+        return ops.leaky_fm(out, slope)
+    return ops.activation(out, ops.ACT_LEAKY, slope), None
+
+
+def _feature_tap_stack(out, slope, B, T, nxt, fuse: bool = True):
+    """_feature_tap that, with `fuse`, also writes the time-stacked operand of the next conv `nxt` (a TimeStackedConv2d)
+    in the same pass when the geometry allows it (kt = 3, pt = its time dilation, no channel padding on either side):
+    returns (a, stats, xs | None)."""
+    C = out.shape[2]
+    if (fuse and nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous()
+            and nxt.in_channels == C and C % 4 == 0 and out.shape[0] == B * T):
+        kt, pt, dt = (v[nxt.TIME_AXIS] for v in (nxt.kernel_size, nxt.padding, nxt.dilation))
+        if kt == 3 and pt == dt:
+            Fp, Cp = nxt.stacked_geometry(out.shape[1], C)
+            if Cp == 3 * C:
+                return ops.leaky_fm_stack(out, slope, T, Fp, *_dil_arg(dt))
+    a, st = _feature_tap(out, slope, B)
+    return a, st, None
+
+
 def _map_conv(conv):
     if conv is nn.Conv1d or conv is DiscConv1d:
         return DiscConv1d
@@ -337,10 +439,12 @@ def spectrogram(n_fft: int):
     return _Spectrogram(n_fft)
 
 
-class SpectralConv2d(nn.Conv2d):
+class SpectralConv2d(TimeStackedConv2d):
     """nn.Conv2d with kernel (kf, kt), stride (sf, 1), dilation (1, dt), padding (pf, dt (kt - 1) / 2) on [B, C, F, T]
-    tensors, on the library's conv1d kernels: the kt time taps (time t + j dt - pt for tap j) become kt x Cin input
-    channels of a conv along frequency over rows (b, t).  Same parameters / state_dict keys as nn.Conv2d."""
+    tensors, on the library's conv1d kernels (TimeStackedConv2d, time on the last axis).  Same parameters / state_dict
+    keys as nn.Conv2d."""
+
+    TIME_AXIS = 1
 
     def __init__(self, *args, **kwargs):
         super().__init__(*args, **kwargs)
@@ -368,70 +472,6 @@ class SpectralConv2d(nn.Conv2d):
         from . import engine
         return engine.precision() == "bf16" and x.is_cuda and engine.ACT_DTYPE == torch.bfloat16
 
-    def cout_ok(self) -> bool:
-        return self.out_channels % 16 == 0
-
-    def _tc_chain_spec(self, C):
-        """One-layer engine chain of this conv along frequency; the (j, c) channel order is a permuted VIEW of the
-        parameter, so the weight-norm backward of the chain reaches weight_v / weight_g through autograd."""
-        from . import engine
-        from .descript_discriminator import _ParamView
-        kf, kt = self.kernel_size
-        pf = self.padding[0]
-        cin = kt * C
-        proxy = self.__dict__.get("_tc_proxy")
-        if proxy is None:
-            proxy = self.__dict__["_tc_proxy"] = _ParamView()
-            if self.__dict__.get("_tc_proxy_static"):       # engine.enable_static_prep ran before the first forward
-                proxy.__dict__["_tc_static"] = {}
-            spec = engine.LayerSpec("conv", proxy, cin, self.out_channels, kf, self.stride[0], 1, (pf, pf),
-                                    ops.ACT_NONE, 0.0, None, True, True)
-            spec.cin_pad = (-cin) % 16
-            spec.cout_pad = (-self.out_channels) % 16
-            self.__dict__["_tc_spec"] = spec
-        spec = self.__dict__["_tc_spec"]
-        if spec.Cin != cin:
-            raise RaveB200Error(f"SpectralConv2d: planned for {spec.Cin // kt} input channels, called with {C}")
-        self._tc_refresh_proxy()
-        return spec
-
-    def _tc_refresh_proxy(self):
-        """(Re)build the proxy's (j, c)-ordered copies of the parameters (engine.refresh_static_prep calls this once the
-        parameters moved, before it rewrites the static layouts)."""
-        proxy = self.__dict__["_tc_proxy"]
-        kf = self.kernel_size[0]
-        co = self.out_channels
-        cin = self.__dict__["_tc_spec"].Cin
-        if hasattr(self, "weight_v"):
-            proxy.weight_v = self.weight_v.permute(0, 3, 1, 2).reshape(co, cin, kf)
-            proxy.weight_g = self.weight_g.reshape(co, 1, 1)
-        else:
-            proxy.weight = self.weight.permute(0, 3, 1, 2).reshape(co, cin, kf)
-        proxy.bias = self.bias
-
-    def stacked_geometry(self, Fq: int, C: int):
-        """(Fp, Cp) of this conv's time-stacked operand for an input of Fq positions and C channels."""
-        spec = self._tc_chain_spec(C)
-        return Fq + (-Fq) % spec.stride, self.kernel_size[1] * C + spec.cin_pad
-
-    def forward_cl(self, x_cl, xs=None):
-        """Channel-last in, channel-last out: x_cl [B, T, F, C] fp32 (dense (f, c) rows) -> the chain's own output buffer
-        [(b t), Fo, Cout(+pad to 16)] fp32, which IS [B, T, Fo, Cout] channel-last.  `xs`: the time-stacked bf16
-        operand when the producer already wrote it (ops.leaky_fm_stack of the previous layer's feature tap)."""
-        from . import engine
-        B, T, Fq, C = x_cl.shape
-        spec = self._tc_chain_spec(C)
-        kt, pt, dt = self.kernel_size[1], self.padding[1], self.dilation[1]
-        Fp, Cp = self.stacked_geometry(Fq, C)
-        if xs is None:
-            xs = ops.time_stack_nhwc(x_cl, kt, pt, Cp, Fp, dt)
-        elif tuple(xs.shape) != (B * T, Fp, Cp) or xs.dtype != engine.ACT_DTYPE:
-            raise RaveB200Error("SpectralConv2d.forward_cl: the pre-stacked operand does not match this conv's geometry")
-        (out,) = engine.run_chain(xs, [spec], Fq)
-        if out.shape[1] != engine.chain_lengths([spec], Fq)[0]:
-            raise RaveB200Error("SpectralConv2d: the one-layer chain's output pitch is its length")
-        return out
-
 
 def rectified_2d_conv_block(capacity, kernel_sizes, strides=None, dilations=None, in_size=None, out_size=None,
                             activation: bool = True):
@@ -446,22 +486,6 @@ def rectified_2d_conv_block(capacity, kernel_sizes, strides=None, dilations=None
     if not activation:
         return conv
     return nn.Sequential(conv, nn.LeakyReLU(.2))
-
-
-def _tap_stack(out, slope, B, T, nxt):
-    """Post-activation feature tap of a chain output (descript_discriminator._feature_tap) that also writes the
-    time-stacked operand of the next conv `nxt` in the same pass when the geometry allows it (kt = 3, pt = its time
-    dilation, no channel padding on either side): returns (a, stats, xs | None)."""
-    from .descript_discriminator import _feature_tap
-    C = out.shape[2]
-    if (nxt is not None and B % 2 == 0 and out.dtype == torch.float32 and out.is_contiguous()
-            and nxt.kernel_size[1] == 3 and nxt.padding[1] == nxt.dilation[1] and nxt.in_channels == C and C % 4 == 0
-            and out.shape[0] == B * T):
-        Fp, Cp = nxt.stacked_geometry(out.shape[1], C)
-        if Cp == 3 * C:
-            return ops.leaky_fm_stack(out, slope, T, Fp, nxt.dilation[1])
-    a, st = _feature_tap(out, slope, B)
-    return a, st, None
 
 
 class EncodecConvNet(nn.Module):
@@ -506,7 +530,7 @@ class EncodecConvNet(nn.Module):
             Fo = out.shape[1]
             if isinstance(layer, nn.Sequential):
                 nxt = convs[i + 1] if i + 1 < len(convs) else None
-                a, st, xs = _tap_stack(out, layer[1].negative_slope, B, T, nxt)
+                a, st, xs = _feature_tap_stack(out, layer[1].negative_slope, B, T, nxt)
                 cur = a.view(B, T, Fo, out.shape[2])
                 feat = cur.permute(0, 3, 2, 1)
                 feat._cl_base = a

@@ -19,6 +19,7 @@ Strided convs' dgrad and ConvTranspose1d's forward are evaluated as `stride` int
 each a stride-1 conv over the taps of that phase (no zero-insertion, no wasted MACs).
 """
 from dataclasses import dataclass, field
+from functools import partial
 from typing import Dict, List, Optional, Tuple
 
 import torch
@@ -29,7 +30,7 @@ from . import _lib, ops
 _state = {"precision": "fp32", "prep_epoch": 0}
 ACT_DTYPE = torch.bfloat16   # storage type of operand / gradient streams (tests may widen it)
 
-# output positions per tensor-core row of a raw first layer with 16-column operand rows (see TcChainFn.forward); rows
+# output positions per tensor-core row of a raw first layer with 16-column operand rows (see RawFirstLayer); rows
 # of 32 columns (multichannel, Cin*K > 16) take half as many; pitches that are not a multiple of it run with one
 # position (plain W-channel rows)
 C1_GROUP = 4
@@ -339,13 +340,54 @@ class _PreparedWeights:
 # `enable_static_prep(model.discriminator)` its prepared layouts live in persistent buffers that the chains read as they
 # are, and that `refresh_static_prep` rewrites IN PLACE right after the discriminator's optimiser step (inside the
 # D-step graph).  Whoever changes those parameters some other way (load_state_dict, an eager optimiser) must refresh.
+# The records live in `module.__dict__["_tc_static"]`: a `_PreparedWeights` (refreshed with all the others by one batched
+# prep call) or a `_StaticTensors` (refreshed on its own).
+
+class _StaticTensors:
+    """Static record of tensors the batched prep call does not make (the block-diagonal weights of a RawFirstLayer, the
+    row norms of a layer that needs no layout): `refresh()` copies `build()`'s fresh values into `tensors` in place.
+    `value` is what a chain gets on a hit: the tensors, unless another object carries them."""
+
+    def __init__(self, tensors, build, value=None):
+        self.tensors, self.build = tensors, build
+        self.value = tensors if value is None else value
+
+    def refresh(self):
+        for old, new in zip(self.tensors, self.build()):
+            if old is not None:
+                old.copy_(new)
+
+
+class ParamProxy:
+    """Stands in for the conv module of a one-layer chain whose operand order is a permutation of its owner's
+    parameters (discriminator.TimeStackedConv2d): `_layer_params` reads weight_v / weight_g / bias or weight / bias
+    from it, `spec.module` is this object, and the prepared-weight cache and static records live in its __dict__.
+    A permuted reshape is a copy, stale once the parameters move: `rebuild()` (the owner's) rewrites the attributes."""
+
+    def __init__(self, owner: nn.Module, spec: LayerSpec, rebuild):
+        self.spec, self.rebuild = spec, rebuild
+        spec.module = self
+        if "_tc_static" in owner.__dict__:       # enable_static_prep ran before the owner's first forward
+            self.__dict__["_tc_static"] = {}
+        owner.__dict__["_tc_proxy"] = self
+
+
+def _proxy_of(m: nn.Module) -> Optional[ParamProxy]:
+    proxy = m.__dict__.get("_tc_proxy")
+    return proxy if isinstance(proxy, ParamProxy) else None
+
+
+def _static_of(module):
+    """The static records of `module` (a conv module or a ParamProxy), or None when it has none: they exist for the
+    bf16 operand mode only."""
+    return module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
+
 
 def _static_holders(root: nn.Module):
-    """Modules under `root` that own prepared weights, plus the parameter-view proxies of one-layer chains (the MRD's
-    DiscConv2d plans its conv on a `_ParamView` holding permuted views of its parameters: descript_discriminator.py)."""
+    """Modules under `root` that own prepared weights, plus the ParamProxy of every one-layer chain."""
     for m in root.modules():
         yield m
-        proxy = m.__dict__.get("_tc_proxy")
+        proxy = _proxy_of(m)
         if proxy is not None:
             yield proxy
 
@@ -354,97 +396,94 @@ def enable_static_prep(root: nn.Module) -> None:
     for m in root.modules():
         if hasattr(m, "weight_v") or (hasattr(m, "weight") and isinstance(getattr(m, "weight"), nn.Parameter)):
             m.__dict__.setdefault("_tc_static", {})
-            if hasattr(m, "_tc_chain_spec"):          # proxy of a one-layer chain: created lazily, marked here or there
-                m.__dict__["_tc_proxy_static"] = True
-                proxy = m.__dict__.get("_tc_proxy")
-                if proxy is not None:
-                    proxy.__dict__.setdefault("_tc_static", {})
+            proxy = _proxy_of(m)                 # one created later marks itself (ParamProxy.__init__)
+            if proxy is not None:
+                proxy.__dict__.setdefault("_tc_static", {})
 
 
 def disable_static_prep(root: nn.Module) -> None:
     for m in _static_holders(root):
         m.__dict__.pop("_tc_static", None)
-        m.__dict__.pop("_tc_proxy_static", None)
 
 
 @torch.no_grad()
 def refresh_static_prep(root: nn.Module) -> int:
     """Recompute every static prepared layout under `root` into its existing buffers; returns how many."""
-    items, into, extra = {False: [], True: []}, {False: [], True: []}, []
+    items, into, single = {False: [], True: []}, {False: [], True: []}, []
     for m in root.modules():
-        if "_tc_proxy" in m.__dict__ and m.__dict__["_tc_proxy"].__dict__.get("_tc_static"):
-            m._tc_refresh_proxy()        # the proxy's permuted parameter copies are stale once the parameters moved
+        proxy = _proxy_of(m)
+        if proxy is not None and proxy.__dict__.get("_tc_static"):
+            proxy.rebuild()              # the proxy's permuted parameter copies are stale once the parameters moved
     for m in _static_holders(root):
-        st = m.__dict__.get("_tc_static")
-        if not st:
-            continue
-        for key, pw in st.items():
-            if key[0] == "c1":
-                extra.append(pw)
+        for key, rec in (m.__dict__.get("_tc_static") or {}).items():
+            if isinstance(rec, _StaticTensors):
+                single.append(rec)
                 continue
-            if pw.raw is None:        # norm-only entry of a Cin = 1 first layer: refreshed through its ("c1", "norm") record
-                continue
-            v, g, _ = _layer_params(pw.spec)
+            v, g, _ = _layer_params(rec.spec)
             x3 = bool(key[2])
-            items[x3].append((v.detach(), g.detach() if g is not None else None, pw.tapsA, pw.tapsB, pw.C0p, pw.C1p))
-            into[x3].append(pw.raw)
+            items[x3].append((v.detach(), g.detach() if g is not None else None, rec.tapsA, rec.tapsB, rec.C0p, rec.C1p))
+            into[x3].append(rec.raw)
     for x3 in (False, True):
         if items[x3]:
             ops.weight_prep_tc_multi(items[x3], x3=x3, into=into[x3])
-    for rec in extra:
-        rec["refresh"]()
-    return len(items[False]) + len(items[True]) + len(extra)
+    for rec in single:
+        rec.refresh()
+    return len(items[False]) + len(items[True]) + len(single)
+
+
+def _row_norms(spec: LayerSpec):
+    v, g, _ = _layer_params(spec)
+    return (ops.weight_norm_raw(v.detach(), g.detach())[1],)
+
+
+def _capturing(t: torch.Tensor) -> bool:
+    return t.is_cuda and torch.cuda.is_current_stream_capturing()
 
 
 def prepare_layers(jobs, x3: bool = False):
-    """jobs: list of (spec, v, g, need_dgrad, need_fwd).  Returns the list of _PreparedWeights, re-using the
-    per-module cache (keyed on parameter versions; bypassed while a CUDA graph is being captured) and
+    """jobs: list of (spec, v, g, need_dgrad, need_fwd).  Returns the list of _PreparedWeights, re-using the module's
+    static records or its cache (keyed on parameter versions; bypassed while a CUDA graph is being captured) and
     preparing all misses with one multi-tensor launch pair.  x3: split-operand ([hi slabs | lo slabs]) layouts."""
+    slot = "_tc_prep_x3" if x3 else "_tc_prep"
     out = [None] * len(jobs)
-    todo = []
+    misses = []
     for i, (spec, v, g, need_dgrad, need_fwd) in enumerate(jobs):
-        capturing = v.is_cuda and torch.cuda.is_current_stream_capturing()
-        static = spec.module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
-        if static is not None:
-            hit = static.get((need_dgrad, need_fwd, x3))
-            if hit is not None:
-                out[i] = hit
-                continue
+        capturing = _capturing(v)
+        static = _static_of(spec.module)
+        skey = (need_dgrad, need_fwd, x3)
         key = (v._version, g._version if g is not None else -1, need_dgrad, need_fwd, str(ACT_DTYPE), str(v.device),
                v.data_ptr(), _state["prep_epoch"], x3)
-        slot = "_tc_prep_x3" if x3 else "_tc_prep"
-        if not capturing and static is None:
+        if static is not None:
+            hit = static.get(skey)
+            if hit is not None:
+                out[i] = hit.value if isinstance(hit, _StaticTensors) else hit
+                continue
+        elif not capturing:
             hit = spec.module.__dict__.get(slot)
             if hit is not None and hit[0] == key:
                 out[i] = hit[1]
                 continue
-        todo.append((i, key, capturing, _PreparedWeights(spec, need_dgrad, need_fwd), v, g))
-    work = [(i, key, cap, pw, v, g) for (i, key, cap, pw, v, g) in todo if pw.tapsA or pw.tapsB]
+        misses.append((i, skey, key, capturing, _PreparedWeights(spec, need_dgrad, need_fwd), v, g))
+    work = [(pw, v, g) for (_, _, _, _, pw, v, g) in misses if pw.tapsA or pw.tapsB]
     if work:
-        res = ops.weight_prep_tc_multi([(v, g, pw.tapsA, pw.tapsB, pw.C0p, pw.C1p) for (_, _, _, pw, v, g) in work],
-                                       x3=x3)
-        for (i, key, cap, pw, v, g), (norm, outA, outB) in zip(work, res):
-            out[i] = pw.finalize(norm, outA, outB, 2 if x3 else 1)
-            pw.raw = (norm, outA, outB)
-            static = pw.spec.module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
-            if static is not None:
-                if not cap:          # buffers of a capture belong to the graph's pool: only eager calls create a slot
-                    static[(pw.need_dgrad, pw.need_fwd, x3)] = out[i]
-            elif not cap:
-                pw.spec.module.__dict__["_tc_prep_x3" if x3 else "_tc_prep"] = (key, out[i])
-    for (i, key, cap, pw, v, g) in todo:
-        if out[i] is None:            # nothing to re-layout (a c1 layer without dgrad): only the norm
+        res = ops.weight_prep_tc_multi([(v, g, pw.tapsA, pw.tapsB, pw.C0p, pw.C1p) for (pw, v, g) in work], x3=x3)
+        for (pw, _, _), raw in zip(work, res):
+            pw.finalize(*raw, 2 if x3 else 1)
+            pw.raw = raw
+    for (i, skey, key, capturing, pw, v, g) in misses:
+        out[i] = pw
+        if pw.raw is None:            # nothing to re-layout (a raw first layer without dgrad): only the norm
             pw.norm = ops.weight_norm_raw(v, g)[1] if g is not None else None
-            out[i] = pw
-            static = pw.spec.module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
-            if static is not None and not cap and pw.norm is not None:
-                norm_t, spec_ = pw.norm, pw.spec
-
-                def _refresh(norm_t=norm_t, spec_=spec_):
-                    v_, g_, _ = _layer_params(spec_)
-                    norm_t.copy_(ops.weight_norm_raw(v_.detach(), g_.detach())[1])
-                static[(pw.need_dgrad, pw.need_fwd, x3)] = pw
-                static[("c1", "norm")] = {"refresh": _refresh}
+        if capturing:                 # buffers of a capture belong to the graph's pool: only eager calls create a slot
+            continue
+        static = _static_of(pw.spec.module)
+        if static is None:
+            if pw.raw is not None:
+                pw.spec.module.__dict__[slot] = (key, pw)
+        elif pw.raw is not None:
+            static[skey] = pw
+        elif pw.norm is not None:
+            static[skey] = _StaticTensors((pw.norm,), partial(_row_norms, pw.spec), value=pw)
     return out
 
 
@@ -456,6 +495,114 @@ def _out_len(spec: LayerSpec, Lin: int) -> int:
     if spec.kind == "conv":
         return ops.conv_out_len(Lin, spec.K, spec.stride, spec.dil, spec.pad[0], spec.pad[1])
     return (Lin - 1) * spec.stride - 2 * spec.pad[0] + spec.K
+
+
+def _pitch(Lout: int, nxt: Optional[LayerSpec]) -> int:
+    """Rows allocated per batch for a stream of Lout positions: the consumer's 4-D tensor map needs a multiple of its
+    stride."""
+    s_next = nxt.stride if (nxt is not None and nxt.kind == "conv") else 1
+    return (Lout + s_next - 1) // s_next * s_next
+
+
+def _zero_rows(tensors, lo: int, hi: int) -> None:
+    """Zero the slack rows [:, lo:hi] (positions past the true length) of every tensor given; None entries are skipped."""
+    if hi > lo:
+        for t in tensors:
+            if t is not None:
+                t[:, lo:hi].zero_()
+
+
+class RawFirstLayer:
+    """First layer of a chain that reads the raw fp32 signal in place (raw_input_ok), one object per forward, kept for
+    the backward.  The Cin*K taps become the W (16 or 32) "channels" of a tiny im2col X[r][l][c*K + k].  G = 64 / W
+    consecutive positions are then read as ONE 64-channel row (X viewed as [R][L/G][64], 128-byte TMA rows instead of
+    2W-byte ones) against the block-diagonal weight kron(I_G, w): the output row holds the G x Cout results of those
+    positions, i.e. the same bytes as out[r][G*lg + p][co].  The geometry (W, G, the padded length Xp) is decided here
+    and nowhere else: the output, its gradient and X are all viewed through `_rows`."""
+
+    def __init__(self, spec: LayerSpec, cin: int, period: int, pool: int, src_shape, pitch: int, Lin: int, Lout: int):
+        self.spec, self.period, self.pool, self.src_shape = spec, period, pool, tuple(src_shape)
+        self.pitch, self.Lin, self.Lout = pitch, Lin, Lout
+        self.W = ops.cin_width(cin, spec.K)
+        G = max(1, C1_GROUP * 16 // self.W)
+        self.G = G if pitch % G == 0 else 1      # the output (and so its gradient) must split into rows of G positions
+        self.Xp = (Lout + self.G - 1) // self.G * self.G
+        self.X = None             # im2col operand, [B][Xp][W]
+        self.w_dgrad = None       # [1][G*W][G*Cout_p]
+
+    def _rows(self, t):
+        """[B][L][C] viewed with G positions per row; None passes through."""
+        return t.view(t.shape[0], t.shape[1] // self.G, self.G * t.shape[2]) if t is not None else None
+
+    @staticmethod
+    def _build_weights(s: LayerSpec, G: int, W: int):
+        """(forward weight [1][G*Cout_p][G*W], its transpose for the dgrad, bias repeated G times) from the parameters
+        as they are now."""
+        v, g, b = _layer_params(s)
+        cout_p = s.Cout + s.cout_pad
+        w_eff = ops.weight_norm_raw(v.detach(), g.detach())[0] if g is not None else v.detach()
+        w_blk = nn.functional.pad(w_eff.reshape(s.Cout, s.Cin * s.K), (0, W - s.Cin * s.K, 0, s.cout_pad))  # [Cout_p, W]
+        if G > 1:
+            eye = torch.eye(G, dtype=w_blk.dtype, device=w_blk.device)
+            w_blk = (eye[:, None, :, None] * w_blk[None, :, None, :]).reshape(G * cout_p, G * W)
+        if b is not None:
+            b = nn.functional.pad(b.detach(), (0, s.cout_pad)) if s.cout_pad else b.detach()
+            if G > 1:
+                b = b.repeat(G)
+        return (w_blk.to(ACT_DTYPE).unsqueeze(0).contiguous(), w_blk.t().contiguous().to(ACT_DTYPE).unsqueeze(0), b)
+
+    def weights(self):
+        """The three tensors of _build_weights: the module's static record when it has one (made by the first eager
+        call), else built from the current parameters."""
+        build = partial(self._build_weights, self.spec, self.G, self.W)
+        static = _static_of(self.spec.module)
+        rec = static.get(("raw", self.G)) if static is not None else None
+        if rec is not None:
+            return rec.tensors
+        tensors = build()
+        if static is not None and not _capturing(self.X):
+            static[("raw", self.G)] = _StaticTensors(tensors, build)
+        return tensors
+
+    def forward(self, a, out_f32, out_act, act_code, act_slope):
+        s, rows = self.spec, self.Xp // self.G
+        im2col = ops.im2col_c1 if a.dim() == 2 else ops.im2col_cin         # mono rows [Bs, T] / [Bs, Cin, T]
+        self.X = im2col(a, self.Lin, self.Lout, self.Xp, s.K, s.stride, s.pad[0], self.period, self.pool)
+        w_fwd, self.w_dgrad, bias_g = self.weights()
+        ops.conv1d_tc(self._rows(self.X), w_fwd, bias_g, None, 1, 1, (0, 0), act_code, act_slope, want_f32=False,
+                      want_act=False, out_f32=self._rows(out_f32), out_act=self._rows(out_act), Lout=rows, Lin=rows,
+                      out_rows=self.pitch // self.G)
+        # positions Lout .. Xp-1 of the last group saw zero taps but got the bias
+        _zero_rows((out_f32, out_act), self.Lout, self.Xp)
+
+    def wgrad(self, g, db):
+        """Weight gradient partials [1][K][Cout][Cin] from the output gradient g [B][pitch][Cout_p]; the bias gradient
+        goes to `db` (or nowhere: None)."""
+        s, G, W = self.spec, self.G, self.W
+        cout_p = s.Cout + s.cout_pad
+        if G > 1:
+            # the wanted [Cout][W] gradient is the sum of the G diagonal blocks of the [G*Cout][G*W] result
+            rows = (self.Lout + G - 1) // G
+            dbw = torch.zeros(G * cout_p, dtype=torch.float32, device=g.device) if db is not None else None
+            d = ops.conv1d_tc_wgrad(self._rows(g), self._rows(self.X), 1, 1, 1, 0, Lp=rows, Lq=rows, dbias=dbw)
+            dw_full = torch.diagonal(d.sum(0)[0].view(G, cout_p, G, W), dim1=0, dim2=2).sum(-1)   # [Cout_p][W]
+            if db is not None:
+                db.copy_(dbw.view(G, cout_p).sum(0))
+        else:
+            dw_full = ops.conv1d_tc_wgrad(g, self.X, 1, 1, 1, 0, Lp=self.Lout, Lq=self.Lout, dbias=db).sum(0)[0]
+        dw_ck = dw_full[:s.Cout, :s.Cin * s.K].reshape(s.Cout, s.Cin, s.K)                     # [Cout][Cin][K]
+        return dw_ck.permute(2, 0, 1).reshape(1, s.K, s.Cout, s.Cin).contiguous()              # [1][K][C0][C1]
+
+    def dgrad(self, g, fake_only: bool):
+        """Gradient of the source signal: P[r][l][c*K + k] = <g[r][l][:], w[:][c][k]> on the tensor cores (slack rows
+        of g are zero), then a gather.  fake_only: g holds the second half of the source batches."""
+        s = self.spec
+        rows = g.shape[1] // self.G if self.G > 1 else self.Lout
+        P, _ = ops.conv1d_tc(self._rows(g), self.w_dgrad, None, None, 1, 1, (0, 0), ops.ACT_NONE, 0.0, want_f32=True,
+                             want_act=False, Lout=rows, Lin=rows)
+        gather = ops.gather_c1 if len(self.src_shape) == 2 else ops.gather_cin
+        return gather(P.view(g.shape[0], -1, self.W), self.src_shape, self.Lin, self.Lout, s.K, s.stride, s.pad[0],
+                      self.period, self.pool, batch0=self.src_shape[0] // 2 if fake_only else 0)
 
 
 class TcChainFn(torch.autograd.Function):
@@ -495,20 +642,24 @@ class TcChainFn(torch.autograd.Function):
         if alpha_idx and (x3 or fm):
             raise _lib.RaveB200Error("Snake chains run in the plain bf16 mode only (no split operands, no fused fm)")
         hraw: Dict[int, torch.Tensor] = {}     # raw (pre-Snake) bf16 input stream of layer i
-        c1 = x_in.dim() == 2 or src is not None
-        period, pool = src if (c1 and src is not None) else (1, 1)
-        cin = x_in.shape[1] if (c1 and x_in.dim() == 3) else 1
+        raw: Optional[RawFirstLayer] = None
+        period = 1
+        if x_in.dim() == 2 or src is not None:         # raw fp32 signal, read in place by the first layer
+            period, pool = src if src is not None else (1, 1)
+            cin = x_in.shape[1] if x_in.dim() == 3 else 1
+            if not raw_input_ok(specs[0], cin):
+                raise _lib.RaveB200Error("raw fp32 rows are only accepted by a first conv with Cin = the signal's "
+                                         "channels, Cin * K <= 32 and no dilation")
+            Lout0 = _out_len(specs[0], L0)
+            raw = RawFirstLayer(specs[0], cin, period, pool, x_in.shape, _pitch(Lout0, specs[1] if n > 1 else None),
+                                L0, Lout0)
         B = x_in.shape[0] * period
-        ctx.c1_src = (period, pool, tuple(x_in.shape))
         ctx.B = B
         # backward on the fake half only (see backward): always available to the fused feature-matching chains, and to
         # plain conv stacks (no residuals, no Snake: the Descript discriminator) whose caller asked for it
         plain = all(s.kind == "conv" and s.res_src is None and s.res_opnd is None and s.res_raw is None
                     and s.pre_act != ops.ACT_SNAKE for s in specs)
         ctx.fake_grad_only = bool(fake_grad_only) and (fm or (plain and B % 2 == 0 and not x3))
-        if c1 and not raw_input_ok(specs[0], cin):
-            raise _lib.RaveB200Error("raw fp32 rows are only accepted by a first conv with Cin = the signal's channels, "
-                                     "Cin * K <= 32 and no dilation")
         dev = x_in.device
         a = x_in
         f32: Dict[int, torch.Tensor] = {}
@@ -517,21 +668,24 @@ class TcChainFn(torch.autograd.Function):
         lens = [L0]
         outputs = []
         stats = torch.zeros(max(n - 1, 1), 2, dtype=torch.float32, device=dev) if fm else None
-        prepared = prepare_layers([(s, flat[3 * i].detach(), flat[3 * i + 1].detach() if flat[3 * i + 1] is not None
-                                    else None, need_dgrad and not (c1 and i == 0), not (c1 and i == 0))
-                                   for i, s in enumerate(specs)], x3=x3)
+        jobs = []
+        for i, s in enumerate(specs):
+            own = raw is not None and i == 0        # a RawFirstLayer makes its own layouts: only the row norms here
+            jobs.append((s, flat[3 * i].detach(), flat[3 * i + 1].detach() if flat[3 * i + 1] is not None else None,
+                         need_dgrad and not own, not own))
+        prepared = prepare_layers(jobs, x3=x3)
         fused_second = False
         for i, s in enumerate(specs):
             if fused_second:           # the 1x1 conv of a unit the previous iteration ran as one fused launch
                 fused_second = False
                 continue
             v, g, bias = flat[3 * i], flat[3 * i + 1], flat[3 * i + 2]
-            use_c1 = c1 and i == 0
+            use_raw = raw is not None and i == 0
             pw = prepared[i]
             Lin = lens[-1]
             Lout = _out_len(s, Lin)
             s1 = specs[i + 1] if i + 1 < n else None
-            if (FUSE_UNITS and not x3 and not fm and not use_c1 and s1 is not None and ACT_DTYPE == torch.bfloat16
+            if (FUSE_UNITS and not x3 and not fm and not use_raw and s1 is not None and ACT_DTYPE == torch.bfloat16
                     and s.kind == "conv" and s1.kind == "conv" and s.K == 3 and s1.K == 1 and s.stride == 1
                     and s1.stride == 1 and s.pre_act == ops.ACT_LEAKY and s1.pre_act == ops.ACT_LEAKY
                     and s1.res_opnd == i and s.res_src is None and s.res_opnd is None and bias is None
@@ -541,16 +695,12 @@ class TcChainFn(torch.autograd.Function):
                 # Residual(DilatedUnit) = act -> conv3(dil) -> act -> conv1x1 -> + x in ONE kernel: the intermediate
                 # operand stays in shared memory (written to HBM only when a backward will need it)
                 s2 = specs[i + 2] if i + 2 < n else None
-                s_next = s2.stride if (s2 is not None and s2.kind == "conv") else 1
-                pitch = (Lout + s_next - 1) // s_next * s_next
+                pitch = _pitch(Lout, s2)
                 if pitch == a.shape[1]:
                     want_f32 = s1.want_f32
                     out_f32 = torch.empty(B, pitch, s.Cout, dtype=torch.float32, device=dev) if want_f32 else None
                     out_act = torch.empty(B, pitch, s.Cout, dtype=ACT_DTYPE, device=dev) if s2 is not None else None
-                    if pitch > Lout:
-                        for t in (out_f32, out_act):
-                            if t is not None:
-                                t[:, Lout:].zero_()
+                    _zero_rows((out_f32, out_act), Lout, pitch)
                     a1, _, _ = ops.dilated_unit_tc(a, pw.fwd, prepared[i + 1].fwd, s.dil, s.pad[0], s.pre_slope,
                                                    s1.pre_slope, s2.pre_act if s2 is not None else ops.ACT_NONE,
                                                    s2.pre_slope if s2 is not None else 0.0, L=Lout, want_a1=need_dgrad,
@@ -575,9 +725,7 @@ class TcChainFn(torch.autograd.Function):
             if snake_next:              # the epilogue writes h as bf16; ops.snake_cl_fwd makes the operand (below)
                 act_code = ops.ACT_NONE
             want_f32 = s.want_f32 and not (fm and nxt is not None)
-            # rows allocated per batch: the consumer's 4-D tensor map needs a multiple of its stride
-            s_next = nxt.stride if (nxt is not None and nxt.kind == "conv") else 1
-            pitch = (Lout + s_next - 1) // s_next * s_next
+            pitch = _pitch(Lout, nxt)
             cout_p = s.Cout + s.cout_pad
             bias_p = bias
             if bias is not None and s.cout_pad:
@@ -592,72 +740,10 @@ class TcChainFn(torch.autograd.Function):
                 res = f32[s.res_src]
             out_f32 = torch.empty(B, pitch, cout_p, dtype=torch.float32, device=dev) if want_f32 else None
             out_act = torch.empty(B, pitch, AW * cout_p, dtype=ACT_DTYPE, device=dev) if want_act else None
-            if pitch > Lout:
-                for t in (out_f32, out_act):
-                    if t is not None:
-                        t[:, Lout:].zero_()
+            _zero_rows((out_f32, out_act), Lout, pitch)
             acts.append(a)
-            if use_c1:
-                # raw first layer: the Cin*K taps become the W (16 or 32) "channels" of a tiny im2col X[r][l][c*K + k].
-                # G = 64 / W consecutive positions are then read as ONE 64-channel row (X viewed as [R][L/G][64],
-                # 128-byte TMA rows instead of 2W-byte ones) against the block-diagonal weight kron(I_G, w): the output
-                # row holds the G x Cout results of those positions, i.e. the same bytes as out[r][G*lg + p][co].
-                Wc = ops.cin_width(cin, s.K)
-                G = max(1, C1_GROUP * 16 // Wc)
-                if pitch % G:
-                    G = 1
-                Xp = (Lout + G - 1) // G * G
-                if a.dim() == 2:         # mono rows [Bs, T]
-                    X = ops.im2col_c1(a, Lin, Lout, Xp, s.K, s.stride, s.pad[0], period, pool)
-                else:
-                    X = ops.im2col_cin(a, Lin, Lout, Xp, s.K, s.stride, s.pad[0], period, pool)
-                ctx.c1_X = X
-                ctx.c1_group = G
-                ctx.c1_width = Wc
-
-                def c1_weights(s=s, G=G, cout_p=cout_p, Wc=Wc):
-                    v_, g_, b_ = _layer_params(s)
-                    w_eff = ops.weight_norm_raw(v_.detach(), g_.detach())[0] if g_ is not None else v_.detach()
-                    w_ck = nn.functional.pad(w_eff.reshape(s.Cout, s.Cin * s.K),
-                                             (0, Wc - s.Cin * s.K, 0, s.cout_pad))                 # [Cout_p, W]
-                    if G > 1:
-                        eye = torch.eye(G, dtype=w_ck.dtype, device=w_ck.device)
-                        w_blk = (eye[:, None, :, None] * w_ck[None, :, None, :]).reshape(G * cout_p, G * Wc)
-                    else:
-                        w_blk = w_ck
-                    bp = b_
-                    if b_ is not None and s.cout_pad:
-                        bp = nn.functional.pad(b_.detach(), (0, s.cout_pad))
-                    bias_g_ = bp.detach().repeat(G) if (bp is not None and G > 1) else (bp.detach() if bp is not None
-                                                                                         else None)
-                    return (w_blk.to(ACT_DTYPE).unsqueeze(0).contiguous(),                     # [1][G*Cout_p][G*W]
-                            w_blk.t().contiguous().to(ACT_DTYPE).unsqueeze(0), bias_g_)        # [1][G*W][G*Cout_p]
-
-                static = s.module.__dict__.get("_tc_static") if ACT_DTYPE == torch.bfloat16 else None
-                skey = ("c1", G, Wc, cout_p)
-                rec = static.get(skey) if static is not None else None
-                if rec is None:
-                    w_fwd, w_dg, bias_g = c1_weights()
-                    if static is not None and not torch.cuda.is_current_stream_capturing():
-                        def _refresh(w_fwd=w_fwd, w_dg=w_dg, bias_g=bias_g, fn=c1_weights):
-                            a_, b_, c_ = fn()
-                            w_fwd.copy_(a_)
-                            w_dg.copy_(b_)
-                            if bias_g is not None:
-                                bias_g.copy_(c_)
-                        static[skey] = {"t": (w_fwd, w_dg, bias_g), "refresh": _refresh}
-                else:
-                    w_fwd, w_dg, bias_g = rec["t"]
-                ctx.c1_wt_dgrad = w_dg
-                ops.conv1d_tc(X.view(B, Xp // G, G * Wc), w_fwd, bias_g,
-                              None, 1, 1, (0, 0), act_code, act_slope, want_f32=False, want_act=False,
-                              out_f32=out_f32.view(B, pitch // G, G * cout_p) if out_f32 is not None else None,
-                              out_act=out_act.view(B, pitch // G, G * cout_p) if out_act is not None else None,
-                              Lout=Xp // G, Lin=Xp // G, out_rows=pitch // G)
-                if Xp > Lout:            # positions Lout .. Xp-1 of the last group saw zero taps but got the bias
-                    for t in (out_f32, out_act):
-                        if t is not None:
-                            t[:, Lout:Xp].zero_()
+            if use_raw:
+                raw.forward(a, out_f32, out_act, act_code, act_slope)
             elif s.kind == "conv":
                 ops.conv1d_tc(a, pw.fwd, bias_p, res, s.stride, s.dil, s.pad, act_code, act_slope,
                               want_f32=False, want_act=False, out_f32=out_f32, out_act=out_act, Lout=Lout,
@@ -675,10 +761,7 @@ class TcChainFn(torch.autograd.Function):
                               out_f32=out_f32.view(B, rows_q, st * cout_p) if out_f32 is not None else None,
                               out_act=out_act.view(B, rows_q, st * AW * cout_p) if out_act is not None else None,
                               out_rows=rows_q, Lout=rows_q, Lin=Lin, x3=x3, act_cs=cout_p if x3 else 0)
-                if pitch > Lout:         # positions beyond the true length were computed too: back to zero
-                    for t in (out_f32, out_act):
-                        if t is not None:
-                            t[:, Lout:].zero_()
+                _zero_rows((out_f32, out_act), Lout, pitch)     # positions beyond the true length were computed too
             if snake_next:
                 hraw[i + 1] = out_act
                 out_act = ops.snake_cl_fwd(out_act, flat[alpha_idx[i + 1]])
@@ -706,7 +789,7 @@ class TcChainFn(torch.autograd.Function):
         ctx.lens = lens
         ctx.params = flat
         ctx.fm = fm
-        ctx.c1 = c1
+        ctx.raw = raw
         ctx.x_requires_grad = x_in.requires_grad
         ctx.out_index = [i for i, s in enumerate(specs) if s.is_output]
         if fm:
@@ -762,9 +845,9 @@ class TcChainFn(torch.autograd.Function):
         for i in range(n - 1, -1, -1):
             s = specs[i]
             pw = ctx.prepared[i]
-            use_c1 = ctx.c1 and i == 0
+            raw = ctx.raw if i == 0 else None
             a_full = ctx.acts[i]
-            a_in = a_full if use_c1 else half(a_full)
+            a_in = a_full if raw is not None else half(a_full)
             Lin, Lout = ctx.lens[i], ctx.lens[i + 1]
             g = g_cur
             if g is None:
@@ -783,23 +866,8 @@ class TcChainFn(torch.autograd.Function):
             if v.requires_grad:
                 if i in db_off:
                     db = db_all[db_off[i]:db_off[i] + cout_p]
-                if use_c1:
-                    G, Wc = ctx.c1_group, ctx.c1_width
-                    X = ctx.c1_X
-                    if G > 1 and g.shape[1] % G == 0 and X.shape[1] % G == 0:
-                        # same G-positions-per-row view as the forward: 64-channel rows for the TMA loads; the wanted
-                        # [Cout][W] gradient is the sum of the G diagonal blocks of the [G*Cout][G*W] result
-                        dbw = torch.zeros(G * cout_p, dtype=torch.float32, device=g.device) if db is not None else None
-                        d = ops.conv1d_tc_wgrad(g.view(B, g.shape[1] // G, G * cout_p), X.view(B, X.shape[1] // G, G * Wc),
-                                                1, 1, 1, 0, Lp=(Lout + G - 1) // G, Lq=(Lout + G - 1) // G, dbias=dbw)
-                        blk = d.sum(0)[0].view(G, cout_p, G, Wc)
-                        dw_full = torch.diagonal(blk, dim1=0, dim2=2).sum(-1)                  # [Cout_p][W]
-                        if db is not None:
-                            db.copy_(dbw.view(G, cout_p).sum(0))
-                    else:
-                        dw_full = ops.conv1d_tc_wgrad(g, X, 1, 1, 1, 0, Lp=Lout, Lq=Lout, dbias=db).sum(0)[0]
-                    dw_ck = dw_full[:s.Cout, :s.Cin * s.K].reshape(s.Cout, s.Cin, s.K)         # [Cout][Cin][K]
-                    dwt = dw_ck.permute(2, 0, 1).reshape(1, s.K, s.Cout, s.Cin).contiguous()   # [1][K][C0][C1]
+                if raw is not None:
+                    dwt = raw.wgrad(g, db)
                 else:
                     P_op, Q_op = (g, a_in) if s.kind == "conv" else (a_in, g)
                     Lp_, Lq_ = (Lout, Lin) if s.kind == "conv" else (Lin, Lout)
@@ -833,7 +901,7 @@ class TcChainFn(torch.autograd.Function):
                 # feature-matching gradient of hidden feature `prev`: computed inside this layer's dgrad epilogue from
                 # the saved operand a_in (real and fake rows), no gradient tensor of its own
                 fm_d = dstats[prev]
-                if s.pre_act != ops.ACT_LEAKY or use_c1:
+                if s.pre_act != ops.ACT_LEAKY or raw is not None:
                     raise _lib.RaveB200Error("fused feature-matching gradient needs a LeakyReLU operand")
             if e is not None:
                 add = e if add is None else (add + e)
@@ -842,23 +910,8 @@ class TcChainFn(torch.autograd.Function):
             add_conv = None if snake_here else add       # Snake: the skip / external gradient joins after dSnake
             fm_partner = a_full[:Bh] if (fo and fm_d is not None) else None
             in_pitch = a_in.shape[1]
-            if use_c1:                  # P[r][l][c*K + k] = <g[r][l][:], w[:][c][k]> on the tensor cores, then a gather
-                G, Wc = ctx.c1_group, ctx.c1_width
-                gpitch = g.shape[1]
-                if G > 1 and gpitch % G == 0:
-                    # same G-positions-per-row view as the forward (slack rows of g are zero)
-                    P, _ = ops.conv1d_tc(g.view(B, gpitch // G, G * cout_p), ctx.c1_wt_dgrad, None, None, 1, 1, (0, 0),
-                                         ops.ACT_NONE, 0.0, want_f32=True, want_act=False, Lout=gpitch // G,
-                                         Lin=gpitch // G)
-                    P = P.view(B, gpitch, Wc)
-                else:
-                    wt_d = ctx.c1_wt_dgrad if G == 1 else ctx.c1_wt_dgrad[:, :Wc, :cout_p].contiguous()
-                    P, _ = ops.conv1d_tc(g, wt_d, None, None, 1, 1, (0, 0), ops.ACT_NONE, 0.0, want_f32=True,
-                                         want_act=False, Lout=Lout, Lin=Lout)
-                period, pool, src_shape = ctx.c1_src
-                gather = ops.gather_c1 if len(src_shape) == 2 else ops.gather_cin
-                gx = gather(P, src_shape, Lin, Lout, s.K, s.stride, s.pad[0], period, pool,
-                            batch0=src_shape[0] // 2 if fo else 0)
+            if raw is not None:
+                gx = raw.dgrad(g, fo)
                 break
             if fo and i == 0:
                 # fake-rows-only backward: the chain's input gradient is [zeros; gx_fake] -- the last dgrad writes its
@@ -868,8 +921,7 @@ class TcChainFn(torch.autograd.Function):
                 gp = gx_full[Bh:]
             else:
                 gp = torch.empty(B, in_pitch, cin_p, dtype=ACT_DTYPE, device=g.device)
-            if in_pitch > Lin:
-                gp[:, Lin:].zero_()
+            _zero_rows((gp,), Lin, in_pitch)
             if s.kind == "conv":
                 if s.stride == 1:
                     padp = (s.K - 1) * s.dil - s.pad[0]
@@ -892,8 +944,7 @@ class TcChainFn(torch.autograd.Function):
                                   want_f32=False, want_act=False, out_act=v4(gp), out_rows=rows_q, Lout=rows_q,
                                   Lin=Lout, res_bf16=v4(add_conv), dact_src=v4(dact), fm_d=fm_d,
                                   fm_partner=v4(fm_partner))
-                    if in_pitch > Lin:
-                        gp[:, Lin:].zero_()
+                    _zero_rows((gp,), Lin, in_pitch)
             else:
                 ops.conv1d_tc(g, pw.dgrad, None, None, s.stride, 1, (s.pad[0], 0), ops.ACT_NONE, s.pre_slope,
                               want_f32=False, want_act=False, out_act=gp, Lout=Lin, Lin=Lout, out_rows=in_pitch,
@@ -911,7 +962,7 @@ class TcChainFn(torch.autograd.Function):
             for job, (dv, dg) in zip(wn_jobs, res):
                 i = job[0]
                 grads[3 * i], grads[3 * i + 1] = dv, dg
-        if fo and gx is not None and not ctx.c1 and gx.shape[0] == Bh:
+        if fo and gx is not None and ctx.raw is None and gx.shape[0] == Bh:
             if gx_full is not None and gx.data_ptr() == gx_full[Bh:].data_ptr() and gx.shape == gx_full[Bh:].shape:
                 gx = gx_full                 # the real rows' gradient is identically unused: zeros
             else:
