@@ -135,6 +135,19 @@ int rave_am_tanh_bwd(const float *dy, const float *x, float *dx, int B, int C, i
 /* VariationalEncoder.reparametrize (rave/blocks.py:725-737) in one pass: z [B][2C][L] = (mean | scale);
  * zs[b][c][t] = eps * (softplus(scale) + 1e-4) + mean;  *kl_sum += sum (mean^2 + var - log var - 1)  (zero it first) */
 int rave_reparam_fwd(const float *z, const float *eps, float *zs, float *kl_sum, int B, int C, int L, void *stream);
+/* WasserteinEncoder.reparametrize's regulariser (rave/blocks.py:761-774), fp32, fixed-order sums.  Rows: x_i = z[b][:][t]
+ * of z [B][D][L] (i = b * L + t, read in place), y_i = prior[i][:] of prior [N][D], N = B * L <= 65536, D <= 64.
+ *   fwd: means = (mean_ij k(x_i, x_j), mean_ij k(y_i, y_j), mean_ij k(x_i, y_j)), k(a, b) = exp(-|a - b|^2 / D^2);
+ *        *mmd = means[0] + means[1] - 2 means[2]
+ *   bwd: dz [B][D][L] = g[0] * (-4 / (D^2 N^2)) * (sum_j k(x_i, x_j) (x_i - x_j) - sum_j k(x_i, y_j) (x_i - y_j)),
+ *        g = the device scalar gradient of *mmd */
+int rave_mmd_fwd(const float *z, const float *prior, float *means, float *mmd, int B, int D, int L, void *stream);
+int rave_mmd_bwd(const float *z, const float *prior, const float *g, float *dz, int B, int D, int L, void *stream);
+/* SphericalEncoder.reparametrize (rave/blocks.py:839-842): out = z / |z|_2 over C per (b, t) of z [B][C][L], norm [B][L];
+ * bwd: dz = (g - out (out . g)) / norm */
+int rave_sphere_norm_fwd(const float *z, float *out, float *norm, int B, int C, int L, void *stream);
+int rave_sphere_norm_bwd(const float *g, const float *out, const float *norm, float *dz, int B, int C, int L,
+                         void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * tensor-core conv engine (wgmma + TMA, register accumulators), implicit GEMM, time on the MMA M axis:

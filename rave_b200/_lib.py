@@ -36,6 +36,10 @@ SIGNATURES = {
     "rave_am_tanh_fwd": (c_int, [_P, _P, _I, _I, _I, _P]),
     "rave_am_tanh_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _P]),
     "rave_reparam_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_mmd_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_mmd_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_sphere_norm_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _P]),
+    "rave_sphere_norm_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "rave_conv1d_tc_supported": (c_int, [_I, _I, _I, _I, _I]),
     "rave_dilated_unit_tc_supported": (c_int, [_I, _I]),
     "rave_dilated_unit_tc_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _I, _F, _P]),

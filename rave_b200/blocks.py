@@ -626,13 +626,76 @@ class VariationalEncoder(nn.Module):
         return z
 
 
+class WasserteinEncoder(nn.Module):
+    """rave/blocks.py:748-791 (configs/wasserstein.gin; the reference's spelling): a Wasserstein auto-encoder whose
+    regulariser is the MMD between the latent rows z[b, :, t] and a standard normal sample of the same shape, and whose
+    latent may be extended by `noise_augmentation` channels of standard normal noise."""
+
+    def __init__(self, encoder_cls, noise_augmentation: int = 0, n_channels: int = 1):
+        super().__init__()
+        self.encoder = encoder_cls(n_channels=n_channels)
+        self.register_buffer("warmed_up", torch.tensor(0))
+        self.noise_augmentation = noise_augmentation
+        self._warmed_up_host = None      # host mirror of the buffer, as in VariationalEncoder
+
+    def compute_mean_kernel(self, x, y):
+        kernel_input = (x[:, None] - y[None]).pow(2).mean(2) / x.shape[-1]
+        return torch.exp(-kernel_input).mean()
+
+    def compute_mmd(self, x, y):
+        x_kernel = self.compute_mean_kernel(x, x)
+        y_kernel = self.compute_mean_kernel(y, y)
+        xy_kernel = self.compute_mean_kernel(x, y)
+        return x_kernel + y_kernel - 2 * xy_kernel
+
+    def reparametrize(self, z, eps: Optional[tuple] = None):
+        """`eps` = (prior [B·L, D], noise [B, noise_augmentation, L] or None) lets a caller inject both draws (parity
+        tests: the CPU and CUDA Philox streams differ); by default they are drawn in the reference's order, the prior
+        sample first.  CUDA fp32 input runs the MMD kernels (rave_mmd_fwd / _bwd), other input the reference's
+        expression."""
+        B, D, L = z.shape
+        prior, noise = eps if eps is not None else (None, None)
+        if prior is None:
+            prior = torch.randn(B * L, D, device=z.device, dtype=z.dtype)
+        if z.is_cuda and z.dtype == torch.float32:
+            reg = ops.mmd(z, prior)[0]
+        else:
+            reg = self.compute_mmd(z.permute(0, 2, 1).reshape(-1, D), prior).mean()
+        if self.noise_augmentation:
+            if noise is None:
+                noise = torch.randn(B, self.noise_augmentation, L, device=z.device, dtype=z.dtype)
+            z = torch.cat([z, noise], 1)
+        return z, reg
+
+    def set_warmed_up(self, state: bool):
+        state = bool(state)
+        if self._warmed_up_host is None or self._warmed_up_host != state:
+            self.warmed_up = torch.tensor(int(state), device=self.warmed_up.device)
+            self._warmed_up_host = state
+
+    def _is_warmed_up(self) -> bool:
+        if self._warmed_up_host is None:          # e.g. right after load_state_dict: read the buffer once
+            self._warmed_up_host = bool(self.warmed_up)
+        return self._warmed_up_host
+
+    def forward(self, x: torch.Tensor):
+        z = self.encoder(x)
+        if self._is_warmed_up():
+            z = z.detach()
+        return z
+
+
 class SphericalEncoder(nn.Module):
+    """rave/blocks.py:833-849 (configs/spherical.gin).  Its `set_warmed_up` does nothing: the encoder keeps training in
+    phase 2."""
 
     def __init__(self, encoder_cls, n_channels: int = 1) -> None:
         super().__init__()
         self.encoder = encoder_cls(n_channels=n_channels)
 
     def reparametrize(self, z):
+        if z.is_cuda and z.dtype == torch.float32:
+            return ops.sphere_norm(z), z.new_zeros(())
         norm_z = z / torch.norm(z, p=2, dim=1, keepdim=True)
         return norm_z, torch.zeros_like(z).mean()
 

@@ -40,6 +40,19 @@ ARCH = {
     # `--config v2 --config hybrid`: mel-spectrogram encoder input and a GRU generator head (HYBRID below)
     "v2_hybrid": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False, disc="v2",
                       update_discriminator_every=4, phase_1_duration=1000000, hybrid=True),
+    # `--config v2 --config wasserstein`: Wasserstein auto-encoder (MMD regulariser), 16 latent channels extended by 128
+    # noise channels for the generator; gin replaces v2.gin's weight dict (feature_matching 20 stays, from
+    # rave/model.py's defaults).  configs/wasserstein.gin also binds BetaWarmupCallback(100, 100, 1): beta_factor = 100.
+    "v2_wasserstein": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False, disc="v2",
+                           update_discriminator_every=4, phase_1_duration=200000, regularization="wasserstein",
+                           latent_size=16, n_out=1, noise_augmentation=128,
+                           weights={"fullband_spectral_distance": 2, "multiband_spectral_distance": 2,
+                                    "adversarial": 2}),
+    # `--config v2 --config spherical`: latent projected on the unit sphere, no regulariser; the encoder keeps training
+    # in phase 2 (SphericalEncoder.set_warmed_up does nothing)
+    "v2_spherical": dict(capacity=96, ratios=[4, 4, 4, 2], activation="leaky", adain=False, disc="v2",
+                         update_discriminator_every=4, phase_1_duration=200000, regularization="spherical",
+                         latent_size=16, n_out=1),
 }
 
 # configs/hybrid.gin on top of any v2-style configuration: EncoderV2(data_size=N_MELS, ratios=[2, 2, 2], dilations=[1])
@@ -127,16 +140,18 @@ def make_discriminator_v2_spectral(capacity=96, n_channels=1, spectral_capacity=
     ], n_channels=n_channels)
 
 
-def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n_channels=1,
+def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=None, n_channels=1,
                padding_mode="centered", phase_1_duration=None, disc_capacity=None, ratios=None, spectral_capacity=32,
                hybrid=None):
     """The full `RAVE` model of a named configuration (`spectral_capacity`: EncodecConvNet capacity of "v2_spectral",
     configs/spectral_discriminator.gin:11).  `hybrid=True` adds `--config hybrid` to any configuration with a
-    VariationalEncoder (default: the configuration's own, True for "v2_hybrid")."""
+    VariationalEncoder (default: the configuration's own, True for "v2_hybrid").  `latent_size` defaults to the
+    configuration's (128 unless it sets one)."""
     a = ARCH[name]
     hyb_enc, recurrent = _hybrid_parts(a.get("hybrid", False) if hybrid is None else hybrid)
-    if hyb_enc is not None and a.get("discrete"):
+    if hyb_enc is not None and (a.get("discrete") or a.get("regularization")):
         raise NotImplementedError("hybrid: the mel-input encoder is built for VariationalEncoder configurations")
+    latent_size = latent_size if latent_size is not None else a.get("latent_size", 128)
     cap = capacity or a["capacity"]
     act = _activation_factory(a["activation"])
     adain_f = (lambda dim: blocks.AdaptiveInstanceNormalization(dim)) if a["adain"] else None
@@ -164,9 +179,15 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
                           num_quantizers=16, noise_augmentation=noise_aug)
     else:
         enc_kw = {**dict(data_size=16, ratios=rat, dilations=V2_DILATIONS), **(hyb_enc or {})}
-        encoder = partial(blocks.VariationalEncoder,
-                          partial(blocks.EncoderV2, capacity=cap, latent_size=latent_size, n_out=2, kernel_size=3,
-                                  activation=act, adain=adain_f, **enc_kw))
+        enc_cls = partial(blocks.EncoderV2, capacity=cap, latent_size=latent_size, n_out=a.get("n_out", 2),
+                          kernel_size=3, activation=act, adain=adain_f, **enc_kw)
+        reg = a.get("regularization")
+        if reg == "wasserstein":                                                 # wasserstein.gin:10-16
+            encoder = partial(blocks.WasserteinEncoder, encoder_cls=enc_cls, noise_augmentation=noise_aug)
+        elif reg == "spherical":                                                 # spherical.gin:8-13
+            encoder = partial(blocks.SphericalEncoder, encoder_cls=enc_cls)
+        else:
+            encoder = partial(blocks.VariationalEncoder, enc_cls)
     noise = None
     if name == "v2_small":                                                       # v2_small.gin:42-57
         noise = partial(blocks.NoiseGeneratorV2, hidden_size=64, data_size=16, ratios=[2, 2, 2],
@@ -186,7 +207,7 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=128, n
             feature_matching_fun=partial(core.mean_difference, norm="L1", relative=True),
             num_skipped_features=a.get("num_skipped_features", 1),
             audio_distance=distance, multiband_audio_distance=distance,
-            weights={"feature_matching": 20},                                 # v2.gin:87-89
+            weights=a.get("weights", {"feature_matching": 20}),               # v2.gin:87-89
             update_discriminator_every=a["update_discriminator_every"], n_channels=n_channels,
             output_mode="raw" if raw else "pqmf",
             spectrogram=mel_spectrogram(sampling_rate) if hyb_enc is not None else None,

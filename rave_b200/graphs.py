@@ -1,7 +1,7 @@
 """Whole-step CUDA graphs: the phase-2 training step is ~1.3k kernel launches (ours + the loss
 arithmetic + Adam); issued from Python that is tens of milliseconds of host time, several times the
 GPU time of the bf16 step.  `GraphedTrainer` captures the generator step and the discriminator step of
-`RAVE.train_body` once (after eager warm-up) and replays them, so the step costs its GPU time.
+`RAVE.train_body` once (after eager warm-up; in phase 1 only the generator step) and replays them, so the step costs its GPU time.
 
 Replay-safe because train_body has no host-side decisions or syncs, the optimisers are `capturable`
 (lr and step counters live on the device; LinearLR updates the lr tensor in place between replays) and
@@ -23,10 +23,11 @@ from . import _lib, engine
 
 
 def _encoder_is_frozen(model) -> bool:
-    from .blocks import VariationalEncoder
+    from .blocks import VariationalEncoder, WasserteinEncoder
     enc = model.encoder
-    # compute_losses sets the encoder's own flag from model.warmed_up before every forward
-    return isinstance(enc, VariationalEncoder) and bool(model.warmed_up)
+    # compute_losses sets the encoder's own flag from model.warmed_up before every forward; a SphericalEncoder ignores
+    # it and keeps training in phase 2
+    return isinstance(enc, (VariationalEncoder, WasserteinEncoder)) and bool(model.warmed_up)
 
 
 def _refresh_static_after_load(m, keys):
@@ -44,8 +45,9 @@ class GraphedTrainer:
         self.grad_hook = grad_hook
         self.x_static = example_batch.clone()
         model.optimizers(capturable=True)
-        if not model.warmed_up:
-            raise RuntimeError("capture phase-2 steps (model.warmed_up = True); phase 1 has no D-step")
+        # phase 2 captures a G-step and a D-step; phase 1 (no discriminator in the loop) only the G-step
+        self.phase2 = bool(model.warmed_up)
+        kinds = (True, False) if self.phase2 else (False,)
         self._weights_at_capture = dict(model.weights)
         model._beta_dev = torch.tensor(float(model.beta_factor), dtype=torch.float32, device=example_batch.device)
         gen_opt, dis_opt = model.optimizers()
@@ -74,12 +76,12 @@ class GraphedTrainer:
         side.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(side):
             for i in range(warmup_steps):
-                for is_dis in (True, False):
+                for is_dis in kinds:
                     model.train_body(self.x_static, is_dis, None, grad_hook)
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         pool = None
-        for is_dis in (True, False):
+        for is_dis in kinds:
             g = torch.cuda.CUDAGraph()
             n0 = _lib.launch_count()
             # thread_local: other threads (NCCL watchdog, samplers) may touch CUDA while we capture
@@ -117,6 +119,9 @@ class GraphedTrainer:
     def step(self, batch: torch.Tensor, batch_idx: int):
         """Same contract as RAVE.training_step: returns the logged scalars (device tensors)."""
         is_dis = self.model.is_discriminator_step(batch_idx)
+        if bool(self.model.warmed_up) != self.phase2:
+            raise RuntimeError(f"GraphedTrainer: captured phase-{2 if self.phase2 else 1} steps but model.warmed_up is "
+                               f"{bool(self.model.warmed_up)}; build a new GraphedTrainer")
         if self.model.weights != self._weights_at_capture:
             raise RuntimeError("GraphedTrainer: model.weights changed after capture (the loss weights are constants of "
                                "the captured graphs); build a new GraphedTrainer")

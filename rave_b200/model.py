@@ -359,10 +359,11 @@ class RAVE(nn.Module):
                 feature_matching_distance = feature_matching_distance + core.stacked_l1_terms(
                     tapped, bool(kw.get("relative", False)))
         else:
-            pred_real = torch.tensor(0.).to(x_raw)
-            pred_fake = torch.tensor(0.).to(x_raw)
-            loss_dis = torch.tensor(0.).to(x_raw)
-            loss_adv = torch.tensor(0.).to(x_raw)
+            # device zeros (not host tensors copied over: a phase-1 step is captured by GraphedTrainer too)
+            pred_real = x_raw.new_zeros(())
+            pred_fake = x_raw.new_zeros(())
+            loss_dis = x_raw.new_zeros(())
+            loss_adv = x_raw.new_zeros(())
 
         if side is not None:
             torch.cuda.current_stream().wait_stream(side)

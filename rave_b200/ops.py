@@ -288,6 +288,64 @@ def reparam(z, eps):
     return ReparamFn.apply(z, eps)
 
 
+class MMDFn(torch.autograd.Function):
+    """WasserteinEncoder's regulariser (rave/blocks.py:761-774) as one library pass: the MMD between the rows
+    x_i = z[b, :, t] of z [B, D, L] and the prior sample [B·L, D], kernel exp(-|a - b|² / D²).  Returns (mmd, the three
+    kernel means (xx, yy, xy)); only the MMD is differentiable, and only with respect to z.  The backward recomputes the
+    kernel and reads the upstream gradient from device memory."""
+
+    @staticmethod
+    def forward(ctx, z, prior):
+        z, prior = _f32c(z), _f32c(prior)
+        B, D, L = z.shape
+        if tuple(prior.shape) != (B * L, D):
+            raise _lib.RaveB200Error(f"mmd: prior {tuple(prior.shape)} for z {tuple(z.shape)}, want {(B * L, D)}")
+        means = torch.empty(3, dtype=torch.float32, device=z.device)
+        mmd = torch.empty((), dtype=torch.float32, device=z.device)
+        call("rave_mmd_fwd", ptr(z), ptr(prior), ptr(means), ptr(mmd), B, D, L, stream_ptr())
+        ctx.save_for_backward(z, prior)
+        ctx.mark_non_differentiable(means)
+        return mmd, means
+
+    @staticmethod
+    def backward(ctx, g_mmd, g_means):
+        z, prior = ctx.saved_tensors
+        B, D, L = z.shape
+        dz = torch.empty_like(z)
+        call("rave_mmd_bwd", ptr(z), ptr(prior), ptr(_f32c(g_mmd)), ptr(dz), B, D, L, stream_ptr())
+        return dz, None
+
+
+def mmd(z, prior):
+    return MMDFn.apply(z, prior)
+
+
+class SphereNormFn(torch.autograd.Function):
+    """SphericalEncoder.reparametrize (rave/blocks.py:839-842): z / |z|₂ over the channels of each (b, t) column."""
+
+    @staticmethod
+    def forward(ctx, z):
+        z = _f32c(z)
+        B, C, L = z.shape
+        out = torch.empty_like(z)
+        norm = torch.empty(B, L, dtype=torch.float32, device=z.device)
+        call("rave_sphere_norm_fwd", ptr(z), ptr(out), ptr(norm), B, C, L, stream_ptr())
+        ctx.save_for_backward(out, norm)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        out, norm = ctx.saved_tensors
+        B, C, L = out.shape
+        dz = torch.empty_like(out)
+        call("rave_sphere_norm_bwd", ptr(_f32c(g)), ptr(out), ptr(norm), ptr(dz), B, C, L, stream_ptr())
+        return dz
+
+
+def sphere_norm(z):
+    return SphereNormFn.apply(z)
+
+
 def am_tanh(x):
     """tanh(x[:, :C] * sigmoid(x[:, C:])) -- GeneratorV2 tail, rave/blocks.py:704-711."""
     return AmTanhFn.apply(x)
