@@ -193,6 +193,9 @@ int rave_conv1d_tc_plan(int B, int Cin, int Cout, int Lout, int K);
 /* ring stages of the ping-pong kernel for an input-gradient launch of this shape (dact_src set, bf16 output only; fm:
  * with fm_d, res_bf16: with the gradient skip); 0 = the launch runs the single-warpgroup kernel */
 int rave_conv1d_tc_pp_stages(int B, int Cin, int Cout, int Lout, int K, int fm, int res_bf16);
+/* ring stages of the ping-pong kernel for a forward launch of this shape (bias and / or LeakyReLU, bf16 output only:
+ * no res, res_bf16, res_act, dact_src or out_f32); 0 = the launch runs the single-warpgroup kernel */
+int rave_conv1d_tc_pp_fwd_stages(int B, int Cin, int Cout, int Lout, int K);
 int rave_conv1d_tc_fwd(const void *xa_bf16, const void *wt_bf16, const float *bias, const float *res,
                        const void *res_bf16, const void *dact_src_bf16, const void *res_act_bf16, float res_slope,
                        float *out_f32, void *out_act_bf16,

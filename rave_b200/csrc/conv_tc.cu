@@ -14,7 +14,8 @@
 // shared memory allows (plan_smem) there are two such buffers, and the bf16 rows go to a swizzled staging tile that one
 // epilogue thread writes out with TMA tensor stores.
 // Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.  The input-gradient launches (LeakyReLU' mask,
-// bf16 out only) run conv_tc_pp_kernel instead: two MMA warpgroups in ping-pong, epilogue from registers.
+// bf16 out only) and the forward launches with bias / LeakyReLU and a bf16 output only run the ping-pong kernel instead
+// (conv_tc_pp_kernel, conv_tc_pp_fwd_kernel): two MMA warpgroups on alternate tiles, epilogue from registers.
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
@@ -512,7 +513,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 }
 
 // =============================================================================================
-// Ping-pong dgrad kernel.  The launches whose epilogue applies the LeakyReLU' mask (dact_src), optionally with the fused
+// Ping-pong kernel.  The launches whose epilogue applies the LeakyReLU' mask (dact_src), optionally with the fused
 // feature-matching term and the bf16 gradient skip, and writes bf16 only (the input gradients of every chain) read up
 // to three operand tiles per output tile; in conv_tc_kernel that epilogue is as long as the main loop and the MMAs wait
 // for it.  Here two MMA warpgroups take alternate tiles of the persistent loop: each runs a whole 128 x BLOCK_N tile
@@ -521,10 +522,19 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant
 // the producer starts a tile it also loads the tile's epilogue operands with TMA into that warpgroup's operand slot,
 // on a barrier of their own, so they land during the main loop; the bf16 result replaces the mask in the slot (same
 // swizzled position) and leaves by TMA tensor stores.
+// The forward launches with bias / LeakyReLU and a bf16 output only (the discriminator convs) run the same kernel
+// with the forward epilogue: no operands to load, the slot holds the output tile alone.  On the short-k launches
+// conv_tc_kernel's four epilogue warps (one per SM sub-partition, fed through a 64 KB fp32 hand-over buffer) bound
+// the launch; here eight warps run the epilogue from registers.
 // Warp roles: warpgroup 0 = TMA producer (warp 0; warps 1-3 leave after giving their registers back), warpgroups 1
 // and 2 = MMA + epilogue.
 // =============================================================================================
 constexpr int PP_THREADS = 384;
+
+// Operand set of a ping-pong instance (template argument of conv_tc_pp_body).  Input gradient: LeakyReLU' mask,
+// + feature-matching partner rows (PP_FM), + gradient skip (PP_RS).  Forward (PP_FWD): + bias (PP_BIAS), LeakyReLU
+// (PP_LEAKY).
+enum PpEpi : int { PP_FM = 1, PP_RS = 2, PP_FWD = 4, PP_BIAS = 8, PP_LEAKY = 16 };
 
 // Epilogue of one tile from the accumulator registers of warpgroup thread (w, lane).  slot = [mask | partner (FM) |
 // gradient skip (RS)] tiles, each BLOCK_N / BOXC boxes of [128 rows][BOXC channels] in the canonical swizzle.  Per
@@ -563,27 +573,67 @@ __device__ __forceinline__ void pp_epilogue(float (*d)[BLOCK_N / 2], uint8_t *sl
   }
 }
 
-// FM, RS: fm_d, res_bf16 set.  One instance per operand set: the epilogue compiled once for run-time flags made the
-// v2 step slower (DESIGN section 5.3).
-template <int BLOCK_N, int BLOCK_K, bool FM, bool RS>
-__global__ void __launch_bounds__(PP_THREADS, 1)
-conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                  const __grid_constant__ CUtensorMap tmap_m, const __grid_constant__ CUtensorMap tmap_p,
-                  const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o,
-                  const TcParams p) {
+// Forward epilogue of one tile from the accumulator registers into the output slot (the boxes and fragment mapping of
+// pp_epilogue).  Per element the fp32 sequence of tc_epi_chunk: + bias[co], max(v, slope v) for LeakyReLU, one rounding
+// to bf16.  Column pair j outermost: one bias load per pair serves the thread's four rows.
+template <int BLOCK_N, int BOXC, bool BIAS, bool LEAKY>
+__device__ __forceinline__ void pp_fwd_epilogue(float (*d)[BLOCK_N / 2], uint8_t *slot, const TcParams &p, int w,
+                                                int lane, int n0) {
+  constexpr int SPAN = BOXC * 2, JB = BOXC / 8;
+  const uint32_t base = stg_offset<BOXC>(16 * w + (lane >> 2), 0) + 4 * (lane & 3);
+  const uint32_t sslot = smem_u32(slot);
+  const float2 *bias = reinterpret_cast<const float2 *>(p.bias + n0 + 2 * (lane & 3));   // columns 8 j + 2 (lane % 4)
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const float2 bb = BIAS ? __ldg(bias + 4 * j) : make_float2(0.f, 0.f);
+    const uint32_t col = (base ^ (uint32_t)((j % JB) << 4)) + (j / JB) * (BLOCK_M * SPAN);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        float v0 = d[h][4 * j + 2 * r], v1 = d[h][4 * j + 2 * r + 1];
+        if (BIAS) {
+          v0 += bb.x;
+          v1 += bb.y;
+        }
+        if (LEAKY) {
+          v0 = fmaxf(v0, v0 * p.slope);
+          v1 = fmaxf(v1, v1 * p.slope);
+        }
+        __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
+        // volatile: each store stays next to its arithmetic (with plain stores ptxas ran all of a tile's arithmetic
+        // ahead of the stores and spilled tile-loop invariants at BLOCK_N = 128)
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sslot + col + (64 * h + 8 * r) * SPAN),
+                     "r"(*reinterpret_cast<uint32_t *>(&o))
+                     : "memory");
+      }
+    }
+  }
+}
+
+// The ping-pong kernel of operand set E (PpEpi flags).  Tensor maps: a, b = MMA operands, o = bf16 output rows;
+// input gradients also m = mask, pm = partner rows (PP_FM), r = gradient skip (PP_RS).
+template <int BLOCK_N, int BLOCK_K, int E>
+__device__ __forceinline__ void conv_tc_pp_body(const CUtensorMap *tmap_a, const CUtensorMap *tmap_b,
+                                                const CUtensorMap *tmap_m, const CUtensorMap *tmap_p,
+                                                const CUtensorMap *tmap_r, const CUtensorMap *tmap_o,
+                                                const TcParams &p) {
   using L = SmemLayout<BLOCK_N, BLOCK_K, false>;
   constexpr int BOXC = L::OUT_BOXC;
   constexpr int BOX_BYTES = BLOCK_M * L::OUT_SPAN;          // one [128 rows][BOXC channels] box
   constexpr int TILE_BYTES = BLOCK_M * BLOCK_N * 2;         // one operand tile
+  constexpr bool FWD = E & PP_FWD, FM = E & PP_FM, RS = E & PP_RS;
   const int STAGES = p.stages;
   static_assert(BLOCK_N % 16 == 0 && BLOCK_N >= 16 && BLOCK_N <= 128, "invalid wgmma N");
+  static_assert(!FWD || !(FM || RS), "the forward epilogue has no gradient operands");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + p.bar_off);
   uint64_t *empty_bar = full_bar + STAGES;
   uint64_t *ofull_bar = empty_bar + STAGES;      // producer -> warpgroup c: its operand slot holds the tile's operands
-  uint64_t *oempty_bar = ofull_bar + 2;          // warpgroup c -> producer: the tensor stores have read the slot
+  uint64_t *oempty_bar = ofull_bar + 2;          // warpgroup c -> producer (forward: -> itself): the tensor stores
+                                                 // have read the slot
   uint64_t *order_bar = oempty_bar + 2;          // warpgroup 1 - c -> c: c may issue its main loop
 
   const int wg = threadIdx.x >> 7;
@@ -591,15 +641,14 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   const int lane = threadIdx.x & 31;
   const int num_tiles = p.n_lt * p.n_bg * p.n_nt;
   const int kblocks = p.K * p.num_kb;
-  constexpr bool fm = FM, rs = RS;
 
   if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmap_a);
-    tma_prefetch_desc(&tmap_b);
-    tma_prefetch_desc(&tmap_m);
-    tma_prefetch_desc(&tmap_o);
-    if (fm) tma_prefetch_desc(&tmap_p);
-    if (rs) tma_prefetch_desc(&tmap_r);
+    tma_prefetch_desc(tmap_a);
+    tma_prefetch_desc(tmap_b);
+    tma_prefetch_desc(tmap_o);
+    if constexpr (!FWD) tma_prefetch_desc(tmap_m);
+    if constexpr (FM) tma_prefetch_desc(tmap_p);
+    if constexpr (RS) tma_prefetch_desc(tmap_r);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
       mbar_init(&empty_bar[s], 4);               // one arrival per MMA warp of the consuming warpgroup
@@ -627,8 +676,8 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       for (int k = 0; k < p.K; ++k) {
         const TapOrigin o = tap_origin(k, p.dil, p.pad_l, p.stride);
         for (int kb = 0; kb < p.num_kb; ++kb) {
-          produce_kblock<BLOCK_N, BLOCK_K, false>(smem, ring, &tmap_a, &tmap_b, p, t, o, k, kb);
-          if (k == 0 && kb == 0) {
+          produce_kblock<BLOCK_N, BLOCK_K, false>(smem, ring, tmap_a, tmap_b, p, t, o, k, kb);
+          if (!FWD && k == 0 && kb == 0) {
             // The tile's epilogue operands, behind its first k-block, into warpgroup c's slot once the tensor stores of
             // that warpgroup's previous tile have read it.  A box past Lout / B is zero-filled and still counts in full.
             mbar_wait(&oempty_bar[c], ((it >> 1) & 1) ^ 1);
@@ -636,18 +685,18 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             if (elect_one()) {
               mbar_arrive_expect_tx(&ofull_bar[c], p.ops_bytes);
               for (int cb = 0; cb < BLOCK_N / BOXC; ++cb) {
-                tma_load_3d(slot + cb * BOX_BYTES, &tmap_m, &ofull_bar[c], t.n0 + cb * BOXC, t.l0, t.b0);
-                if (fm) {
+                tma_load_3d(slot + cb * BOX_BYTES, tmap_m, &ofull_bar[c], t.n0 + cb * BOXC, t.l0, t.b0);
+                if (FM) {
                   // partner rows one batch at a time: a batch group may straddle the [real; fake] boundary
                   for (int i = 0; i < p.BB; ++i) {
                     const int b = t.b0 + i;
                     const int pb = p.fm_bh > 0 ? (b < p.fm_bh ? b + p.fm_bh : b - p.fm_bh) : b;
-                    tma_load_3d(slot + TILE_BYTES + cb * BOX_BYTES + i * p.BL * L::OUT_SPAN, &tmap_p, &ofull_bar[c],
+                    tma_load_3d(slot + TILE_BYTES + cb * BOX_BYTES + i * p.BL * L::OUT_SPAN, tmap_p, &ofull_bar[c],
                                 t.n0 + cb * BOXC, t.l0, pb);
                   }
                 }
-                if (rs)
-                  tma_load_3d(slot + (fm ? 2 : 1) * TILE_BYTES + cb * BOX_BYTES, &tmap_r, &ofull_bar[c],
+                if (RS)
+                  tma_load_3d(slot + (FM ? 2 : 1) * TILE_BYTES + cb * BOX_BYTES, tmap_r, &ofull_bar[c],
                               t.n0 + cb * BOXC, t.l0, t.b0);
               }
             }
@@ -677,15 +726,20 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       mma_drain<BLOCK_N>(d, ring, prev, lane);
 
       const TileCoord t = tile_coord<BLOCK_N>(tile, p);
-      mbar_wait(&ofull_bar[c], u & 1);
-      pp_epilogue<BLOCK_N, BOXC, FM, RS>(d, slot, p, w, lane, t.b0);
+      if constexpr (FWD) {
+        mbar_wait(&oempty_bar[c], (u & 1) ^ 1);    // the tensor stores of this warpgroup's previous tile read the slot
+        pp_fwd_epilogue<BLOCK_N, BOXC, (E & PP_BIAS) != 0, (E & PP_LEAKY) != 0>(d, slot, p, w, lane, t.n0);
+      } else {
+        mbar_wait(&ofull_bar[c], u & 1);
+        pp_epilogue<BLOCK_N, BOXC, FM, RS>(d, slot, p, w, lane, t.b0);
+      }
       // rows past Lout and batches past B fall outside the tensor map and are not written
       fence_proxy_async();
       named_bar_sync(1 + c, 128);
       if (issuer) {
 #pragma unroll
         for (int cb = 0; cb < BLOCK_N / BOXC; ++cb)
-          tma_store_3d(&tmap_o, slot + cb * BOX_BYTES, t.n0 + cb * BOXC, t.l0, t.b0);
+          tma_store_3d(tmap_o, slot + cb * BOX_BYTES, t.n0 + cb * BOXC, t.l0, t.b0);
         bulk_commit();
         bulk_wait_read<0>();
         mbar_arrive(&oempty_bar[c]);
@@ -693,6 +747,27 @@ conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
     }
     if (issuer) bulk_wait_all();
   }
+}
+
+// Input gradients.  FM, RS: fm_d, res_bf16 set.  One instance per operand set: the epilogue compiled once for run-time
+// flags made the v2 step slower (DESIGN section 5.3).
+template <int BLOCK_N, int BLOCK_K, bool FM, bool RS>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+conv_tc_pp_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                  const __grid_constant__ CUtensorMap tmap_m, const __grid_constant__ CUtensorMap tmap_p,
+                  const __grid_constant__ CUtensorMap tmap_r, const __grid_constant__ CUtensorMap tmap_o,
+                  const TcParams p) {
+  conv_tc_pp_body<BLOCK_N, BLOCK_K, (FM ? PP_FM : 0) | (RS ? PP_RS : 0)>(&tmap_a, &tmap_b, &tmap_m, &tmap_p, &tmap_r,
+                                                                         &tmap_o, p);
+}
+
+// Forward.  BIAS: bias set, LEAKY: act = RAVE_ACT_LEAKY; one instance per operand set as above.
+template <int BLOCK_N, int BLOCK_K, bool BIAS, bool LEAKY>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+conv_tc_pp_fwd_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                      const __grid_constant__ CUtensorMap tmap_o, const TcParams p) {
+  conv_tc_pp_body<BLOCK_N, BLOCK_K, PP_FWD | (BIAS ? PP_BIAS : 0) | (LEAKY ? PP_LEAKY : 0)>(
+      &tmap_a, &tmap_b, nullptr, nullptr, nullptr, &tmap_o, p);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -791,46 +866,71 @@ static int encode_rows_map(CUtensorMap *m, const __nv_bfloat16 *base, const TcPa
   return 0;
 }
 
-// BLOCK_N = 96 at BLOCK_K = 64: ptxas spills tile-loop invariants of every ping-pong instance, so none is built and
-// conv_tc_kernel runs these launches
-template <int BN, int BK>
-constexpr bool pp_built = !(BN == 96 && BK == 64);
+// BLOCK_N = 96 at BLOCK_K = 64: ptxas spills tile-loop invariants of every input-gradient ping-pong instance, so none
+// is built and conv_tc_kernel runs these launches
+template <int BN, int BK, bool FWD>
+constexpr bool pp_built = FWD || !(BN == 96 && BK == 64);
 
 // Ring stages of a ping-pong launch whose operand slots hold nops tiles each (mask, + partner rows with fm_d, + gradient
-// skip with res_bf16: [128][BLOCK_N] bf16 each); the ring gets the rest (at most 8 stages).  0: the launch runs
-// conv_tc_kernel -- no instance for the tile, or fewer than 2 stages fit (mask + partner + skip at BLOCK_N = 128,
-// BLOCK_K = 64).
-template <int BN, int BK>
+// skip with res_bf16, or the forward output alone: [128][BLOCK_N] bf16 each); the ring gets the rest (at most 8
+// stages).  0: the launch runs conv_tc_kernel -- no instance for the tile, or fewer than 2 stages fit (mask + partner +
+// skip at BLOCK_N = 128, BLOCK_K = 64).
+template <int BN, int BK, bool FWD>
 constexpr int pp_stages(int nops) {
   using L = SmemLayout<BN, BK, false>;
-  if (!pp_built<BN, BK>) return 0;
+  if (!pp_built<BN, BK, FWD>) return 0;
   const int s = (SMEM_MAX - L::FIXED - 2 * nops * BLOCK_M * BN * 2) / L::STAGE_BYTES;
   return s < 2 ? 0 : s > 8 ? 8 : s;
 }
 
+// Ring stages of a forward launch (bias / LeakyReLU -> bf16 only) of kblocks k-blocks per tile on the ping-pong
+// kernel; 0: it runs conv_tc_kernel.  The ping-pong kernel takes the launch when its ring is at least as deep as the
+// one plan_smem gives conv_tc_kernel and either the tile has at most 24 k-blocks or BLOCK_N = 128 (there the 64 KB
+// hand-over buffer leaves conv_tc_kernel 3-4 stages; the ping-pong slot leaves 5).  Tensor-bound launches of 36-72
+// k-blocks per tile at BLOCK_N = 64 and 96 measured 8-22 % slower on the ping-pong kernel (conv_tc_kernel already hides
+// their epilogue behind the main loop and keeps 7-8 stages); see DESIGN section 5.6.
 template <int BN, int BK>
+static int pp_fwd_stages(int kblocks) {
+  const int s = pp_stages<BN, BK, true>(1);
+  TcParams q;
+  plan_smem<BN, BK, false>(kblocks, q);
+  return s >= q.stages && (BN == 128 || kblocks <= 24) ? s : 0;
+}
+
+// FWD: a forward launch (bias / LeakyReLU; the slot holds the output tile alone), else an input-gradient launch
+template <int BN, int BK, bool FWD>
 static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, int stages, cudaStream_t stream) {
   using L = SmemLayout<BN, BK, false>;
   p.stages = stages;
   p.ops_bytes = (1 + (p.fm_d ? 1 : 0) + (p.res_bf16 ? 1 : 0)) * BLOCK_M * BN * 2;
   p.ops_off = p.stages * L::STAGE_BYTES;
   p.bar_off = p.ops_off + 2 * p.ops_bytes;
-  // mask, skip and output boxes cover the tile's batch group; partner rows go one batch per box.  With fm_bh < 0
-  // (the launch covers the fake half) the partner of batch b is batch b of the half stored right before dact_src.
-  CUtensorMap tm, tp, tr, to;
-  memset(&tp, 0, sizeof(tp));
-  memset(&tr, 0, sizeof(tr));
-  if (encode_rows_map<BN>(&tm, p.dact_src, p, p.BB) || encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
-  if (p.fm_d && encode_rows_map<BN>(&tp, p.fm_bh > 0 ? p.dact_src : p.dact_src - p.fm_half, p, 1)) return 1;
-  if (p.res_bf16 && encode_rows_map<BN>(&tr, p.res_bf16, p, p.BB)) return 1;
   const int grid = persistent_grid(p.n_lt * p.n_bg * p.n_nt), smem = p.bar_off + L::FIXED;
-  const auto go = [&](auto fm, auto rs) {
-    return launch_tc<conv_tc_pp_kernel<BN, BK, decltype(fm)::value, decltype(rs)::value>>(
-        "conv1d_tc", grid, PP_THREADS, smem, stream, ta, tb, tm, tp, tr, to, p);
-  };
   const std::true_type y;
   const std::false_type n;
-  return p.fm_d ? (p.res_bf16 ? go(y, y) : go(y, n)) : (p.res_bf16 ? go(n, y) : go(n, n));
+  CUtensorMap tm, tp, tr, to;
+  if (encode_rows_map<BN>(&to, p.out_act, p, p.BB)) return 1;
+  if constexpr (FWD) {
+    const auto go = [&](auto bias, auto leaky) {
+      return launch_tc<conv_tc_pp_fwd_kernel<BN, BK, decltype(bias)::value, decltype(leaky)::value>>(
+          "conv1d_tc", grid, PP_THREADS, smem, stream, ta, tb, to, p);
+    };
+    const bool leaky = p.act == RAVE_ACT_LEAKY;
+    return p.bias ? (leaky ? go(y, y) : go(y, n)) : (leaky ? go(n, y) : go(n, n));
+  } else {
+    // mask, skip and output boxes cover the tile's batch group; partner rows go one batch per box.  With fm_bh < 0
+    // (the launch covers the fake half) the partner of batch b is batch b of the half stored right before dact_src.
+    memset(&tp, 0, sizeof(tp));
+    memset(&tr, 0, sizeof(tr));
+    if (encode_rows_map<BN>(&tm, p.dact_src, p, p.BB)) return 1;
+    if (p.fm_d && encode_rows_map<BN>(&tp, p.fm_bh > 0 ? p.dact_src : p.dact_src - p.fm_half, p, 1)) return 1;
+    if (p.res_bf16 && encode_rows_map<BN>(&tr, p.res_bf16, p, p.BB)) return 1;
+    const auto go = [&](auto fm, auto rs) {
+      return launch_tc<conv_tc_pp_kernel<BN, BK, decltype(fm)::value, decltype(rs)::value>>(
+          "conv1d_tc", grid, PP_THREADS, smem, stream, ta, tb, tm, tp, tr, to, p);
+    };
+    return p.fm_d ? (p.res_bf16 ? go(y, y) : go(y, n)) : (p.res_bf16 ? go(n, y) : go(n, n));
+  }
 }
 
 template <int BN, int BK, bool X3>
@@ -888,7 +988,20 @@ extern "C" int rave_conv1d_tc_pp_stages(int B, int Cin, int Cout, int Lout, int 
   const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
   if (!g.BK || !g.BN) return 0;
   const int nops = 1 + (fm ? 1 : 0) + (res_bf16 ? 1 : 0);
-  return visit_tile(g.BK, g.BN, [&](auto bk, auto bn) { return pp_stages<decltype(bn)::value, decltype(bk)::value>(nops); });
+  return visit_tile(g.BK, g.BN, [&](auto bk, auto bn) {
+    return pp_stages<decltype(bn)::value, decltype(bk)::value, false>(nops);
+  });
+}
+
+// Ring stages of the ping-pong kernel for a forward launch of this shape (bias and / or LeakyReLU, bf16 output only);
+// 0 = the launch runs conv_tc_kernel.
+extern "C" int rave_conv1d_tc_pp_fwd_stages(int B, int Cin, int Cout, int Lout, int K) {
+  using namespace rave::tc;
+  const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
+  if (!g.BK || !g.BN) return 0;
+  return visit_tile(g.BK, g.BN, [&](auto bk, auto bn) {
+    return pp_fwd_stages<decltype(bn)::value, decltype(bk)::value>(K * g.num_kb);
+  });
 }
 
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,
@@ -970,15 +1083,22 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   }
   cudaStream_t s = (cudaStream_t)stream;
   if (x3) return conv_tc_dispatch_x3(BK, BN, ta, tb, p, s);
-  // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only): the
-  // ping-pong kernel where pp_stages gives it the launch
-  const bool pp = dact_src && out_act && !bias && !res && !res_act && !out_f32 && act == RAVE_ACT_NONE;
+  // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only) and
+  // forward launches (bias and / or LeakyReLU, bf16 out only): the ping-pong kernel where pp_stages / pp_fwd_stages
+  // give it the launch
+  const bool bf16_only = out_act && !res && !res_act && !out_f32;
+  const bool pp_dgrad = bf16_only && dact_src && !bias && act == RAVE_ACT_NONE;
+  const bool pp_fwd = bf16_only && !dact_src && !res_bf16 && !fm_d;
   const int nops = 1 + (fm_d ? 1 : 0) + (res_bf16 ? 1 : 0);
   return visit_tile(BK, BN, [&](auto bk, auto bn) {
     constexpr int BK_ = decltype(bk)::value, BN_ = decltype(bn)::value;
-    if constexpr (pp_built<BN_, BK_>) {
-      const int stages = pp ? pp_stages<BN_, BK_>(nops) : 0;
-      if (stages) return launch_pp<BN_, BK_>(ta, tb, p, stages, s);
+    if constexpr (pp_built<BN_, BK_, false>) {
+      const int stages = pp_dgrad ? pp_stages<BN_, BK_, false>(nops) : 0;
+      if (stages) return launch_pp<BN_, BK_, false>(ta, tb, p, stages, s);
+    }
+    if constexpr (pp_built<BN_, BK_, true>) {
+      const int stages = pp_fwd ? pp_fwd_stages<BN_, BK_>(K * g.num_kb) : 0;
+      if (stages) return launch_pp<BN_, BK_, true>(ta, tb, p, stages, s);
     }
     return launch<BN_, BK_, false>(ta, tb, p, s);
   });

@@ -95,10 +95,19 @@ def wgrad_runner(torch, ops, ints, ptrs):
     return run, nb
 
 
-def instance(lib, name, ints):
+def instance(lib, name, ints, ptrs):
+    """Kernel of a launch; conv launches the ping-pong kernel takes are marked ` pp` and its ring stages."""
     if name == "rave_conv1d_tc_fwd":
-        v = lib.rave_conv1d_tc_plan(ints[0], ints[1], ints[4], ints[5], ints[6])
-        return f"conv<{v & 0xfff},{(v >> 12) & 0xfff}>"
+        B, Cin, Cout, Lout, K, act = ints[0], ints[1], ints[4], ints[5], ints[6], ints[10]
+        v = lib.rave_conv1d_tc_plan(B, Cin, Cout, Lout, K)
+        bias, res, res_bf16, dact, res_act, o32, oa, fm = [c == "P" for c in ptrs[2:10]]   # order of fwd_runner
+        stages = 0
+        if oa and not (res or res_act or o32):
+            if dact and not bias and act == 0:
+                stages = lib.rave_conv1d_tc_pp_stages(B, Cin, Cout, Lout, K, int(fm), int(res_bf16))
+            elif not (dact or res_bf16 or fm):
+                stages = lib.rave_conv1d_tc_pp_fwd_stages(B, Cin, Cout, Lout, K)
+        return f"conv<{v & 0xfff},{(v >> 12) & 0xfff}>" + (f" pp{stages}" if stages else "")
     if name == "rave_conv1d_tc_wgrad":
         Bc, Cm, Lp, pp, Cn = ints[:5]
         s = lib.rave_conv1d_tc_wgrad_splits(Bc, Cm, Lp, Cn, ints[7])
@@ -164,7 +173,7 @@ def main():
         fl, by = r["cost"]
         t_tc, t_hbm = fl / peak_f, by / peak_b
         per_step = (3 * r["G"] + r["D"]) / 4
-        table.append(dict(entry=name, instance=instance(lib, name, ints), ints=list(ints), ptrs=ptrs, G=r["G"], D=r["D"],
+        table.append(dict(entry=name, instance=instance(lib, name, ints, ptrs), ints=list(ints), ptrs=ptrs, G=r["G"], D=r["D"],
                           us=us, us_per_step=per_step * us, gflop=fl / 1e9, mb=by / 1e6,
                           bound="tensor" if t_tc >= t_hbm else "hbm", frac=max(t_tc, t_hbm) * 1e6 / us))
     table.sort(key=lambda e: -e["us_per_step"])
