@@ -456,6 +456,38 @@ int rave_adam_multi(int n, float *const *params, const float *const *grads, floa
                     float *const *exp_avg_sq, const long *numel, const float *lr, float *step, float beta1, float beta2,
                     float eps, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Latent prior (rave/prior/{core,residual_block,model}.py: VariationalPrior.training_step), fp32 CUDA-core arithmetic,
+ * fixed-order sums.  Streams [B][T][C] follow `cl_bf16`: 1 = channel-last with bf16 operands (wgmma engine), 0 = [B][C][T]
+ * fp32 (parity path); fp32 gradient inputs (dout, dg) use the same layout.
+ *   latent_classes: z [B][2L][T] encoder output (mean | scale), eps [B][L][T] ->
+ *                   classes [B][T-D+1][D] int32 = clamp(floor(R Phi(y_d(b, t + D-1-d))), 0, R-1),
+ *                   y = latent_pca[:D] (eps (softplus(scale) + 1e-4) + mean - latent_mean)   (post_process_latent,
+ *                   DiagonalShift and QuantizedNormal.encode without the one-hot)
+ *   embed_fwd:      pre_net on class indices, w [Cout][R][K], group d = o / (Cout/D):
+ *                   out[b][t][o] = LeakyReLU(bias[o] + sum_{k: t+k-(K-1) >= 0} w[o][c_d(b, t+k-(K-1))][k]) as the fp32
+ *                   stream out_f32 and (cl_bf16) the bf16 operand out_op [B][T][Cout]
+ *   embed_wgrad:    dw [Cout][R][K], dbias [Cout] (nullable) of it from dout (gradient of out) and x (out_op, or out_f32
+ *                   when cl_bf16 = 0, for LeakyReLU'); K <= 8
+ *   gate:           g [B][T][C] = sigmoid(h[.., c]) tanh(h[.., C + c]) of h [B][T][2C]; bwd: dh from dg (fp32)
+ *   head_ce:        x = LeakyReLU(p), p [B][Tp][Cin] post_net.0 output; logits of group d: w [D R][Cin/D] x[d Cin/D ..]
+ *                   + bias; *loss = mean over B D (Tp-1) of the cross-entropy against classes[b][t+1][d];
+ *                   bwd: dx = d loss / d p (times *gloss, a device float) in p's type, dw [D R][Cin/D], dbias [D R]
+ * ------------------------------------------------------------------------------------------- */
+int rave_prior_latent_classes(const float *z, const float *eps, const float *latent_mean, const float *latent_pca,
+                              int *classes, int B, int L, int T, int D, int R, void *stream);
+int rave_prior_embed_fwd(const int *classes, const float *w, const float *bias, float *out_f32, void *out_op_bf16, int B,
+                         int Tp, int D, int R, int Cout, int K, int cl_bf16, float slope, void *stream);
+int rave_prior_embed_wgrad(const int *classes, const float *dout, const void *x, float *dw, float *dbias, int B, int Tp,
+                           int D, int R, int Cout, int K, int cl_bf16, float slope, void *stream);
+int rave_gate_fwd(const void *h, void *g, int B, int C, int T, int cl_bf16, void *stream);
+int rave_gate_bwd(const float *dg, const void *h, void *dh, int B, int C, int T, int cl_bf16, void *stream);
+int rave_prior_head_ce_fwd(const void *x, const float *w, const float *bias, const int *classes, float *loss, int B,
+                           int Tp, int D, int R, int Cin, int cl_bf16, float slope, void *stream);
+int rave_prior_head_ce_bwd(const void *x, const float *w, const float *bias, const int *classes, const float *gloss,
+                           void *dx, float *dw, float *dbias, int B, int Tp, int D, int R, int Cin, int cl_bf16,
+                           float slope, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -107,6 +107,13 @@ SIGNATURES = {
     "rave_cl_to_ncl": (c_int, [_P, _P, _I, _I, _I, _P]),
     "rave_act_to_bf16": (c_int, [_P, _P, _I, _I, _I, _I, _F, _P, _P]),
     "rave_weight_to_tapmajor_bf16": (c_int, [_P, _P, _I, _I, _I, _I, _I, _P]),
+    "rave_prior_latent_classes": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "rave_prior_embed_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_prior_embed_wgrad": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_gate_fwd": (c_int, [_P, _P, _I, _I, _I, _I, _P]),
+    "rave_gate_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P]),
+    "rave_prior_head_ce_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_prior_head_ce_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
 }
 
 

@@ -213,3 +213,16 @@ def build_rave(name="v2", sampling_rate=48000, capacity=None, latent_size=None, 
             spectrogram=mel_spectrogram(sampling_rate) if hyb_enc is not None else None,
             input_mode="mel" if hyb_enc is not None else "pqmf")
     return model
+
+
+# configs/prior/prior_v1.gin (scripts/train_prior.py's default prior configuration)
+PRIOR_V1 = dict(resolution=32, res_size=512, skp_size=256, kernel_size=3, cycle_size=4, n_layers=10)
+
+
+def build_prior(rave_model, latent_size=None, fidelity=None, **overrides):
+    """`VariationalPrior(pretrained_vae=rave_model)` at the prior_v1.gin bindings (`sr` = the RAVE's sampling rate), as
+    `scripts/train_prior.py` builds it; `overrides` rebind any of them.  One of latent_size / fidelity is required."""
+    from .prior import VariationalPrior
+    kw = dict(PRIOR_V1, sr=rave_model.sr)
+    kw.update(overrides)
+    return VariationalPrior(pretrained_vae=rave_model, latent_size=latent_size, fidelity=fidelity, **kw)

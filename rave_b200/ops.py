@@ -1306,3 +1306,115 @@ def gru(x, rnn):
         h = GruLayerFn.apply(h, getattr(rnn, f"weight_ih_l{l}"), getattr(rnn, f"weight_hh_l{l}"),
                              getattr(rnn, f"bias_ih_l{l}"), getattr(rnn, f"bias_hh_l{l}"))
     return h.transpose(1, 2)
+
+
+# ----------------------------------------------------------------------------------------------
+# latent prior (csrc/prior.cu).  `cl` = True: channel-last streams with bf16 operands (wgmma engine); False: [B, C, T]
+# fp32 (parity path).
+# ----------------------------------------------------------------------------------------------
+
+def prior_latent_classes(z, eps, latent_mean, latent_pca, D, R):
+    """Encoder output z [B, 2L, T] and eps [B, L, T] -> int32 classes [B, T - D + 1, D] (include/rave_b200.h)."""
+    z, eps, latent_mean, latent_pca = _f32c(z), _f32c(eps), _f32c(latent_mean), _f32c(latent_pca)
+    B, L2, T = z.shape
+    cls = torch.empty(B, T - D + 1, D, dtype=torch.int32, device=z.device)
+    call("rave_prior_latent_classes", ptr(z), ptr(eps), ptr(latent_mean), ptr(latent_pca), ptr(cls), B, L2 // 2, T, D,
+         R, stream_ptr())
+    return cls
+
+
+def _stream_shape(B, T, C, cl):
+    return (B, T, C) if cl else (B, C, T)
+
+
+def prior_embed_fwd(cls, w, bias, cl, slope=0.2):
+    """pre_net + LeakyReLU on class indices: (fp32 stream, bf16 channel-last operand if cl else None)."""
+    B, Tp, D = cls.shape
+    Cout, R, K = w.shape
+    out = torch.empty(_stream_shape(B, Tp, Cout, cl), dtype=torch.float32, device=w.device)
+    op = torch.empty(B, Tp, Cout, dtype=torch.bfloat16, device=w.device) if cl else None
+    call("rave_prior_embed_fwd", ptr(cls), ptr(_f32c(w)), ptr(_f32c(bias)), ptr(out), ptr(op), B, Tp, D, R, Cout, K,
+         int(cl), float(slope), stream_ptr())
+    return out, op
+
+
+def prior_embed_wgrad(cls, dout, x, w_shape, cl, slope=0.2):
+    """(dw [Cout, R, K], dbias [Cout]) of prior_embed_fwd from the fp32 gradient of its output; x = its operand
+    (cl) or fp32 stream (LeakyReLU')."""
+    B, Tp, D = cls.shape
+    Cout, R, K = w_shape
+    dw = torch.empty(w_shape, dtype=torch.float32, device=dout.device)
+    db = torch.empty(Cout, dtype=torch.float32, device=dout.device)
+    call("rave_prior_embed_wgrad", ptr(cls), ptr(_f32c(dout)), ptr(x), ptr(dw), ptr(db), B, Tp, D, R, Cout, K, int(cl),
+         float(slope), stream_ptr())
+    return dw, db
+
+
+def _gate_dims(h, cl):
+    if cl:
+        B, T, C2 = h.shape
+    else:
+        B, C2, T = h.shape
+    return B, C2 // 2, T
+
+
+def gate_fwd(h, cl):
+    """sigmoid(h[:, :C]) * tanh(h[:, C:]) over the channel axis of h (bf16 channel-last if cl, else fp32 [B, 2C, T])."""
+    B, C, T = _gate_dims(h, cl)
+    g = torch.empty(_stream_shape(B, T, C, cl), dtype=h.dtype, device=h.device)
+    call("rave_gate_fwd", ptr(h), ptr(g), B, C, T, int(cl), stream_ptr())
+    return g
+
+
+def gate_bwd(dg, h, cl):
+    B, C, T = _gate_dims(h, cl)
+    dh = torch.empty_like(h)
+    call("rave_gate_bwd", ptr(_f32c(dg)), ptr(h), ptr(dh), B, C, T, int(cl), stream_ptr())
+    return dh
+
+
+class GateFn(torch.autograd.Function):
+    """The gated unit of the prior's ResidualBlock on [B, 2C, T] fp32 (dense Prior.forward)."""
+
+    @staticmethod
+    def forward(ctx, h):
+        h = _f32c(h)
+        ctx.save_for_backward(h)
+        return gate_fwd(h, False)
+
+    @staticmethod
+    def backward(ctx, dg):
+        (h,) = ctx.saved_tensors
+        return gate_bwd(dg, h, False)
+
+
+def gate(h):
+    return GateFn.apply(h)
+
+
+def _head_dims(x, cls, cl):
+    B, Tp, D = cls.shape
+    Cin = x.shape[2] if cl else x.shape[1]
+    return B, Tp, D, Cin
+
+
+def prior_head_ce_fwd(x, w, bias, cls, cl, slope=0.2):
+    """Mean cross-entropy of post_net.2 on LeakyReLU(x) against the next frame's classes (0-d fp32 tensor)."""
+    B, Tp, D, Cin = _head_dims(x, cls, cl)
+    R = w.shape[0] // D
+    loss = torch.empty((), dtype=torch.float32, device=x.device)
+    call("rave_prior_head_ce_fwd", ptr(x), ptr(_f32c(w)), ptr(_f32c(bias)), ptr(cls), ptr(loss), B, Tp, D, R, Cin,
+         int(cl), float(slope), stream_ptr())
+    return loss
+
+
+def prior_head_ce_bwd(x, w, bias, cls, gloss, cl, slope=0.2):
+    """(d loss / d x in x's dtype and layout, dw like w, dbias) times the device scalar gloss."""
+    B, Tp, D, Cin = _head_dims(x, cls, cl)
+    R = w.shape[0] // D
+    dx = torch.empty_like(x)
+    dw = torch.empty_like(w)
+    db = torch.empty(w.shape[0], dtype=torch.float32, device=x.device)
+    call("rave_prior_head_ce_bwd", ptr(x), ptr(_f32c(w)), ptr(_f32c(bias)), ptr(cls), ptr(_f32c(gloss)), ptr(dx),
+         ptr(dw), ptr(db), B, Tp, D, R, Cin, int(cl), float(slope), stream_ptr())
+    return dx, dw, db
