@@ -146,6 +146,13 @@ int rave_mmd_bwd(const float *z, const float *prior, const float *g, float *dz, 
 /* SphericalEncoder.reparametrize (rave/blocks.py:839-842): out = z / |z|_2 over C per (b, t) of z [B][C][L], norm [B][L];
  * bwd: dz = (g - out (out . g)) / norm */
 int rave_sphere_norm_fwd(const float *z, float *out, float *norm, int B, int C, int L, void *stream);
+/* Validation PCA (rave/model.py:464-488): accumulates the count, mean and centred scatter matrix of the rows
+ * x_(b,t) = z[b][0:D][t] of z [B][C][L] fp32 (D <= C: the posterior mean is the first half of the encoder output, read in
+ * place) into state = [n | mean[D] | M2[D*D]] (fp64, updated in place; all zero to start).  Per-block moments, then
+ * Chan's pairwise merge in block order.  Fixed-order sums: bit-identical across runs, no host read, graph-capturable.
+ * 1 <= D <= 256; `work` holds rave_latent_moments_workspace_bytes(B, L, D) bytes. */
+int  rave_latent_moments(const float *z, int B, int C, int L, int D, double *state, double *work, void *stream);
+long rave_latent_moments_workspace_bytes(int B, int L, int D);
 int rave_sphere_norm_bwd(const float *g, const float *out, const float *norm, float *dz, int B, int C, int L,
                          void *stream);
 
@@ -430,6 +437,10 @@ int rave_noise_fir_bwd(const float *h, const float *M, const float *noise, const
  * ------------------------------------------------------------------------------------------- */
 int rave_mel_log1p_fwd(const void *X_c64, const int *band, const float *weights, float *out, int N, int F, int bins,
                        int M, int nnz, float scale, void *stream);
+/* its gradient with respect to X: dX[n][f][k] = 2 scale X[n][f][k] sum_m w_m[k] dy[n][m][f] / (1 + mel[n][m][f]) for
+ * f < F - 1, zero for the dropped last frame; dy [N][M][F-1], dX [N][F][bins] complex64. */
+int rave_mel_log1p_bwd(const void *X_c64, const int *band, const float *weights, const float *dy, void *dX_c64, int N,
+                       int F, int bins, int M, int nnz, float scale, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
  * GRU layer (rave/blocks.py:295-319: nn.GRU, gate order r, z, n), fp32, H = 128, one persistent launch per layer:

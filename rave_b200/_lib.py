@@ -40,6 +40,8 @@ SIGNATURES = {
     "rave_mmd_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
     "rave_sphere_norm_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _P]),
     "rave_sphere_norm_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P]),
+    "rave_latent_moments": (c_int, [_P, _I, _I, _I, _I, _P, _P, _P]),
+    "rave_latent_moments_workspace_bytes": (c_long, [_I, _I, _I]),
     "rave_conv1d_tc_supported": (c_int, [_I, _I, _I, _I, _I]),
     "rave_dilated_unit_tc_supported": (c_int, [_I, _I]),
     "rave_dilated_unit_tc_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _F, _I, _F, _P]),
@@ -94,6 +96,7 @@ SIGNATURES = {
     "rave_stft_frames_valid_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "rave_rfft_bwd_scale": (c_int, [_P, _P, _L, _I, _I, _L, _L, _L, _P]),
     "rave_mel_log1p_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_mel_log1p_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _F, _P]),
     "rave_gru_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "rave_gru_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "rave_gemm_f32_splits": (c_int, [_I, _I, _I]),

@@ -226,11 +226,27 @@ class MelSpectrogram(nn.Module):
         from . import ops
         batch, channels, T = x.shape
         w = self.spectrogram.window
+        if x.requires_grad and torch.is_grad_enabled():
+            # differentiable path (the receptive-field probe): framing, rfft and the mel reduction each with their
+            # library backward; training never asks for the input gradient and keeps the no-grad path below
+            X = ops.rfft(ops.stft_frames(x.reshape(-1, T), w, self.n_fft, self.hop_length), self._rfft_bw())
+            band, wts = self.band_table()
+            return ops.MelLog1pFn.apply(X, band, wts, self.n_mels, 1.0 / float(self._win_energy()), batch, channels)
         with torch.no_grad():
             frames = ops.stft_frames(x.detach().reshape(-1, T), w, self.n_fft, self.hop_length)
             X = torch.fft.rfft(frames)
             band, wts = self.band_table()
             return ops.mel_log1p(X, band, wts, self.n_mels, 1.0 / float(self._win_energy()), batch, channels)
+
+    def _rfft_bw(self):
+        """Bin weights of ops.rfft's backward for n_fft (MultiScaleSTFT.rfft_bw_<n>), on the window's device."""
+        w = self.spectrogram.window
+        hit = self.__dict__.get("_rfft_bw_cache")
+        if hit is None or hit.device != w.device:
+            bw = torch.full((self.n_fft // 2 + 1,), 0.5 * self.n_fft)
+            bw[0] = bw[-1] = self.n_fft
+            hit = self.__dict__["_rfft_bw_cache"] = bw.to(w.device)
+        return hit
 
     def _win_energy(self):
         w = self.spectrogram.window
@@ -270,27 +286,81 @@ class AudioDistanceV1(nn.Module):
         return {"spectral_distance": distance}
 
 
+def _is_recurrent(module) -> bool:
+    """The modules rave/core.py:186-188 switches off for the probe (a recurrence makes the gradient's support unbounded)."""
+    return hasattr(module, "gru_state") or hasattr(module, "temporal")
+
+
 @torch.enable_grad()
 def get_rave_receptive_field(model, n_channels=1):
-    """rave/core.py:180-217: autograd probe of the input gradient's support."""
+    """rave/core.py:180-217: support of the input gradient of one output sample, doubling the probe length until both
+    ends of the gradient are zero.  Recurrent modules are disabled for the probe; the probe runs on the fp32 kernels and
+    the dense PQMF tables (exact non-zero counts, the reference's fp32 measurement) in eval mode.  The input gradient is taken with
+    torch.autograd.grad, so no parameter `.grad` is created or cleared.  Precision, training flag and the recurrent
+    modules are restored afterwards."""
+    from . import engine, pqmf
     N = 2 ** 15
-    model.eval()
     device = next(iter(model.parameters())).device
-    while True:
-        x = torch.randn(1, model.n_channels, N, requires_grad=True, device=device)
-        z = model.encode(x)
-        z = model.encoder.reparametrize(z)[0]
-        y = model.decode(z)
-        y[0, 0, N // 2].backward()
-        grad = x.grad.data.reshape(-1)
-        left_grad, right_grad = grad.chunk(2, 0)
-        if (left_grad[0] == 0) and right_grad[-1] == 0:
-            break
-        N *= 2
-    left_rf = len(left_grad[left_grad != 0])
-    right_rf = len(right_grad[right_grad != 0])
-    model.zero_grad()
+    was_training, precision = model.training, engine.precision()
+    recurrent = [m for m in model.modules() if _is_recurrent(m)]
+    banks = [m for m in model.modules() if isinstance(m, pqmf.PQMF)]
+    model.eval()
+    engine.set_precision("fp32")
+    for m in recurrent:
+        m.disable()
+    for m in banks:
+        m.exact_taps = True
+    try:
+        while True:
+            x = torch.randn(1, model.n_channels, N, requires_grad=True, device=device)
+            z = model.encode(x)
+            z = model.encoder.reparametrize(z)[0]
+            y = model.decode(z)
+            (grad,) = torch.autograd.grad(y[0, 0, N // 2], x, allow_unused=True)
+            if grad is None:
+                raise RuntimeError("get_rave_receptive_field: the output does not depend on the input (an encoder "
+                                   "that detaches its output, e.g. a VariationalEncoder in phase 2)")
+            left_grad, right_grad = grad.reshape(-1).chunk(2, 0)
+            if left_grad[0] == 0 and right_grad[-1] == 0:
+                break
+            N *= 2
+        left_rf = int((left_grad != 0).sum())
+        right_rf = int((right_grad != 0).sum())
+    finally:
+        for m in recurrent:
+            m.enable()
+        for m in banks:
+            m.exact_taps = False
+        engine.set_precision(precision)
+        model.train(was_training)
     return left_rf, right_rf
+
+
+def latent_analysis(means: Sequence[torch.Tensor], latent_size: int):
+    """The latent PCA of RAVE.validation_epoch_end (rave/model.py:464-488) over the posterior means [B, D, L] of an
+    epoch, taken in list order: (latent_mean [D], components [D, D] (rows), fidelity [D]), all fp32.
+
+    One rave_latent_moments per tensor accumulates the fp64 count, mean and centred scatter (Chan's merge: no
+    X^T X - n m m^T cancellation on channels whose mean is large against their spread); the covariance M2 / (n - 1) is
+    diagonalised once on the device in fp64.  Order and signs follow sklearn's PCA: eigenvalues descending, negatives
+    clipped to zero, each component flipped so that its largest-magnitude entry is positive."""
+    from . import ops
+    D = int(latent_size)
+    n = sum(int(m.shape[0]) * int(m.shape[-1]) for m in means)          # rows, from shapes: no device read
+    if n < D:
+        raise ValueError(f"latent_analysis: {n} latent rows for {D} components (PCA needs at least as many rows)")
+    state = torch.zeros(1 + D + D * D, dtype=torch.float64, device=means[0].device)
+    for m in means:
+        ops.latent_moments(m, D, state)
+    mean = state[1:1 + D]
+    cov = state[1 + D:].reshape(D, D) / (n - 1)
+    ev, vec = torch.linalg.eigh(cov)
+    ev = ev.flip(0).clamp_min(0)
+    comps = vec.flip(1).T.contiguous()
+    pivot = comps.gather(1, comps.abs().argmax(1, keepdim=True))
+    comps = comps * torch.where(pivot < 0, -1.0, 1.0)
+    fidelity = torch.cumsum(ev / ev.sum(), 0)
+    return mean.float(), comps.float(), fidelity.float()
 
 
 # ---------------------------------------------------------------------------------------------

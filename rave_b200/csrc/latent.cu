@@ -346,3 +346,160 @@ extern "C" int rave_sphere_norm_bwd(const float *g, const float *out, const floa
   RAVE_CHECK_LAUNCH("sphere_norm_bwd");
   return 0;
 }
+
+// ---------------------------------------------------------------------------------------------
+// Streaming latent moments for the validation PCA (rave/model.py:464-488): count, mean and centred scatter matrix of the
+// rows x_(b,t) = z[b][0:D][t] of z [B][C][L], accumulated in fp64 into state = [n | mean[D] | M2[D*D]].
+//   Pass 1: grid (row blocks, 64 x 64 tiles of M2).  CTA (k, tile) walks block k's rows twice in 32-row tiles staged in
+//           shared memory as fp64 (loads coalesced along t): first the per-channel sums of its channels (one thread per
+//           channel, rows in order), then the centred products of its M2 tile (4 x 4 entries per thread, rows in order).
+//           Every CTA that needs a channel's mean computes it with the same sequence of additions, so the copies agree
+//           bit for bit.  Results (n_k, m_k, M2_k) go to work.
+//   Pass 2: state <- state (+) block 0 (+) block 1 (+) ... with Chan's update, d = m_k - m, M2 += M2_k + d d^T n n_k / n';
+//           each CTA owns 256 entries of M2 and replays the same running-mean sequence.
+// Every sum is sequential in a fixed order: bit-identical across runs, no float atomics, no host read.
+// ---------------------------------------------------------------------------------------------
+namespace rave {
+
+constexpr int LM_THREADS = 256;
+constexpr int LM_TILE = 64;          // M2 tile edge (channels)
+constexpr int LM_ROWS = 32;          // rows staged per shared-memory tile
+constexpr int LM_MAX_D = 256;
+constexpr int LM_MIN_BLOCK = 256;    // rows per block at least ...
+constexpr int LM_MAX_BLOCKS = 132;   // ... and at most one block per SM
+
+__host__ __device__ inline long lm_rows_per_block(long N) {
+  long r = (N + LM_MAX_BLOCKS - 1) / LM_MAX_BLOCKS;
+  if (r < LM_MIN_BLOCK) r = LM_MIN_BLOCK;
+  return (r + LM_ROWS - 1) / LM_ROWS * LM_ROWS;
+}
+
+// Stage rows [g0, g0 + nr) of channels [c0, c0 + 64) into s[r][c] as fp64 minus `sub` (nullptr: raw); rows past nr and
+// channels past D are zero.
+__device__ __forceinline__ void lm_stage(double (*s)[LM_TILE + 1], const float *__restrict__ z, long g0, int nr, int c0,
+                                         int C, int L, int D, const double *sub) {
+#pragma unroll
+  for (int k = 0; k < LM_ROWS * LM_TILE / LM_THREADS; ++k) {
+    const int e = threadIdx.x + k * LM_THREADS, r = e % LM_ROWS, c = e / LM_ROWS, ch = c0 + c;
+    double v = 0.0;
+    if (r < nr && ch < D) {
+      const long g = g0 + r, b = g / L, t = g - b * L;
+      v = (double)z[((size_t)b * C + ch) * L + t];
+      if (sub) v -= sub[c];
+    }
+    s[r][c] = v;
+  }
+}
+
+__global__ void __launch_bounds__(LM_THREADS)
+latent_moments_block_kernel(const float *__restrict__ z, int C, int L, int D, long N, long rpb, int tiles,
+                            const double *__restrict__ state, double *__restrict__ work) {
+  __shared__ double sa[LM_ROWS][LM_TILE + 1], sb[LM_ROWS][LM_TILE + 1];
+  __shared__ double ma[LM_TILE], mb[LM_TILE];
+  const int tid = threadIdx.x, ty = tid >> 4, tx = tid & 15;
+  const int ti = blockIdx.y / tiles, tj = blockIdx.y % tiles, ca = ti * LM_TILE, cb = tj * LM_TILE;
+  const long r0 = blockIdx.x * rpb, r1 = min(N, r0 + rpb), nb = r1 - r0;
+  const size_t rec = 1 + (size_t)D + (size_t)D * D;
+  double *out = work + 1 + D + blockIdx.x * rec;
+  if (blockIdx.x == 0 && blockIdx.y == 0)                       // pass 2 reads the incoming (n, mean) from here
+    for (int i = tid; i < 1 + D; i += LM_THREADS) work[i] = state[i];
+  // block means of the channels of this tile's rows (ca..) and columns (cb..)
+  double s = 0.0;
+  for (long g0 = r0; g0 < r1; g0 += LM_ROWS) {
+    const int nr = (int)min((long)LM_ROWS, r1 - g0);
+    lm_stage(sa, z, g0, nr, ca, C, L, D, nullptr);
+    lm_stage(sb, z, g0, nr, cb, C, L, D, nullptr);
+    __syncthreads();
+    if (tid < 2 * LM_TILE)
+      for (int r = 0; r < nr; ++r) s += tid < LM_TILE ? sa[r][tid] : sb[r][tid - LM_TILE];
+    __syncthreads();
+  }
+  if (tid < LM_TILE) ma[tid] = s / (double)nb;
+  else if (tid < 2 * LM_TILE) mb[tid - LM_TILE] = s / (double)nb;
+  __syncthreads();
+  if (tj == 0 && tid < LM_TILE && ca + tid < D) out[1 + ca + tid] = ma[tid];
+  if (blockIdx.y == 0 && tid == 0) out[0] = (double)nb;
+  // centred scatter of the tile
+  double acc[4][4] = {};
+  for (long g0 = r0; g0 < r1; g0 += LM_ROWS) {
+    const int nr = (int)min((long)LM_ROWS, r1 - g0);
+    lm_stage(sa, z, g0, nr, ca, C, L, D, ma);
+    lm_stage(sb, z, g0, nr, cb, C, L, D, mb);
+    __syncthreads();
+    for (int r = 0; r < nr; ++r) {
+      double a[4], b[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        a[q] = sa[r][ty * 4 + q];
+        b[q] = sb[r][tx * 4 + q];
+      }
+#pragma unroll
+      for (int p = 0; p < 4; ++p)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[p][q] = fma(a[p], b[q], acc[p][q]);
+    }
+    __syncthreads();
+  }
+  double *M2 = out + 1 + D;
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+      const int i = ca + ty * 4 + p, j = cb + tx * 4 + q;
+      if (i < D && j < D) M2[(size_t)i * D + j] = acc[p][q];
+    }
+}
+
+__global__ void __launch_bounds__(LM_THREADS)
+latent_moments_merge_kernel(int D, int nblk, const double *__restrict__ work, double *__restrict__ state) {
+  __shared__ double mean[LM_MAX_D], dl[LM_MAX_D];
+  const int tid = threadIdx.x;
+  const long e = (long)blockIdx.x * LM_THREADS + tid, DD = (long)D * D;
+  const int i = (int)(e / D), j = (int)(e % D);
+  const size_t rec = 1 + (size_t)D + (size_t)D * D;
+  double n = work[0];
+  if (tid < D) mean[tid] = work[1 + tid];
+  double m2 = e < DD ? state[1 + D + e] : 0.0;
+  for (int k = 0; k < nblk; ++k) {
+    const double *blk = work + 1 + D + k * rec;
+    const double nk = blk[0], nn = n + nk, f = nk / nn, w = n * nk / nn;
+    __syncthreads();                                            // mean[] of the previous merge is final
+    if (tid < D) dl[tid] = blk[1 + tid] - mean[tid];
+    __syncthreads();
+    if (e < DD) m2 += blk[1 + D + e] + dl[i] * dl[j] * w;
+    if (tid < D) mean[tid] = fma(dl[tid], f, mean[tid]);
+    n = nn;
+  }
+  if (e < DD) state[1 + D + e] = m2;
+  __syncthreads();
+  if (blockIdx.x == 0) {
+    if (tid == 0) state[0] = n;
+    if (tid < D) state[1 + tid] = mean[tid];
+  }
+}
+
+}  // namespace rave
+
+extern "C" long rave_latent_moments_workspace_bytes(int B, int L, int D) {
+  using namespace rave;
+  if (B <= 0 || L <= 0 || D <= 0 || D > LM_MAX_D) return 0;
+  const long N = (long)B * L, nblk = (N + lm_rows_per_block(N) - 1) / lm_rows_per_block(N);
+  return (long)sizeof(double) * (1 + D + nblk * (1 + D + (long)D * D));
+}
+
+extern "C" int rave_latent_moments(const float *z, int B, int C, int L, int D, double *state, double *work,
+                                   void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(z && state && work, "latent_moments: null pointer");
+  RAVE_CHECK_ARG(B > 0 && L > 0 && C > 0, "latent_moments: bad shape [%d][%d][%d]", B, C, L);
+  RAVE_CHECK_ARG(D >= 1 && D <= LM_MAX_D && D <= C, "latent_moments: latent size %d outside 1..min(%d, C = %d)", D,
+                 LM_MAX_D, C);
+  const long N = (long)B * L, rpb = lm_rows_per_block(N);
+  const int nblk = (int)((N + rpb - 1) / rpb), tiles = ceil_div(D, LM_TILE);
+  const cudaStream_t s = (cudaStream_t)stream;
+  latent_moments_block_kernel<<<dim3(nblk, tiles * tiles), LM_THREADS, 0, s>>>(z, C, L, D, N, rpb, tiles, state, work);
+  RAVE_CHECK_LAUNCH("latent_moments_block");
+  latent_moments_merge_kernel<<<ceil_div(D * D, LM_THREADS), LM_THREADS, 0, s>>>(D, nblk, work, state);
+  RAVE_CHECK_LAUNCH("latent_moments_merge");
+  return 0;
+}

@@ -325,6 +325,58 @@ mel_log1p_kernel(const float2 *__restrict__ X, const int *__restrict__ band, con
   }
 }
 
+// Gradient of mel_log1p_kernel with respect to X (the receptive-field probe of a mel-input model differentiates through
+// the front end):  dX[n][f][k] = 2 scale X[n][f][k] sum_m w_m[k] dy[n][m][f] / (1 + mel[n][m][f]), zero for the dropped
+// last frame.  Same tiling as the forward: the band sums are recomputed from |X|^2 in shared memory, then one thread per
+// (frame, bin) adds the bands covering bin k in band order.
+__global__ void __launch_bounds__(256)
+mel_log1p_bwd_kernel(const float2 *__restrict__ X, const int *__restrict__ band, const float *__restrict__ wts,
+                     const float *__restrict__ dy, float2 *__restrict__ dX, int F, int bins, int M, int nnz, float scale) {
+  extern __shared__ float sm[];
+  float *P = sm;                          // [MEL_FT][bins]
+  float *W = P + MEL_FT * bins;           // [nnz]
+  float *G = W + nnz;                     // [M][MEL_FT]: dy / (1 + mel)
+  int *bd = reinterpret_cast<int *>(G + M * MEL_FT);
+  const int n = blockIdx.y, f0 = blockIdx.x * MEL_FT;
+  const int Fo = F - 1;
+  const int nf = min(MEL_FT, F - f0);     // frames of this CTA, the dropped one included
+  const int nv = min(MEL_FT, Fo - f0);    // frames with an output
+  const float2 *Xn = X + ((size_t)n * F + f0) * bins;
+  float2 *dXn = dX + ((size_t)n * F + f0) * bins;
+  for (int i = threadIdx.x; i < nf * bins; i += blockDim.x) {
+    const float2 v = Xn[i];
+    P[i] = fmaf(v.x, v.x, v.y * v.y);
+  }
+  for (int i = threadIdx.x; i < nnz; i += blockDim.x) W[i] = wts[i];
+  for (int i = threadIdx.x; i < 3 * M; i += blockDim.x) bd[i] = band[i];
+  __syncthreads();
+  for (int o = threadIdx.x; o < M * MEL_FT; o += blockDim.x) {
+    const int m = o / MEL_FT, f = o % MEL_FT;
+    float g = 0.f;
+    if (f < nv) {
+      const int lo = bd[3 * m], hi = bd[3 * m + 1], off = bd[3 * m + 2];
+      const float *p = P + f * bins;
+      float acc = 0.f;
+      for (int k = lo; k < hi; ++k) acc = fmaf(W[off + k - lo], p[k], acc);
+      g = dy[((size_t)n * M + m) * Fo + f0 + f] / (1.f + scale * acc);
+    }
+    G[o] = g;
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < nf * bins; i += blockDim.x) {
+    const int f = i / bins, k = i % bins;
+    float s = 0.f;
+    if (f < nv)
+      for (int m = 0; m < M; ++m) {
+        const int lo = bd[3 * m], hi = bd[3 * m + 1];
+        if (k >= lo && k < hi) s = fmaf(W[bd[3 * m + 2] + k - lo], G[m * MEL_FT + f], s);
+      }
+    const float2 v = Xn[i];
+    const float c = 2.f * scale * s;
+    dXn[i] = make_float2(c * v.x, c * v.y);
+  }
+}
+
 }  // namespace rave
 
 extern "C" int rave_mel_log1p_fwd(const void *X_c64, const int *band, const float *weights, float *out, int N, int F,
@@ -339,6 +391,21 @@ extern "C" int rave_mel_log1p_fwd(const void *X_c64, const int *band, const floa
   mel_log1p_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>((const float2 *)X_c64, band, weights, out, F, bins, M, nnz,
                                                              scale);
   RAVE_CHECK_LAUNCH("mel_log1p_fwd");
+  return 0;
+}
+
+extern "C" int rave_mel_log1p_bwd(const void *X_c64, const int *band, const float *weights, const float *dy, void *dX_c64,
+                                  int N, int F, int bins, int M, int nnz, float scale, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(X_c64 && band && weights && dy && dX_c64 && N > 0 && F > 1 && bins > 0 && M > 0 && nnz > 0 &&
+                 N <= 65535, "mel_log1p_bwd: bad argument");
+  const size_t smem = ((size_t)MEL_FT * bins + nnz + (size_t)M * MEL_FT + 3 * M) * 4;
+  RAVE_CHECK_ARG(smem <= 48 * 1024, "mel_log1p_bwd: %d bins / %d filter weights / %d bands need %zu bytes of shared memory "
+                 "(at most 48 KB)", bins, nnz, M, smem);
+  dim3 grid(ceil_div(F, MEL_FT), N);
+  mel_log1p_bwd_kernel<<<grid, 256, smem, (cudaStream_t)stream>>>((const float2 *)X_c64, band, weights, dy,
+                                                                 (float2 *)dX_c64, F, bins, M, nnz, scale);
+  RAVE_CHECK_LAUNCH("mel_log1p_bwd");
   return 0;
 }
 

@@ -8,7 +8,8 @@ Replay-safe because train_body has no host-side decisions or syncs, the optimise
 every buffer the library kernels see is allocated from the graph's private pool (tensor maps bake the
 addresses at capture).  Host-side scalars that a schedule may move are read from device memory:
 `beta_factor` (BetaWarmupCallback) lives in `model._beta_dev`, refreshed before every replay; the loss
-weights (`model.weights`) are constants of the captured graph -- changing them needs a new GraphedTrainer.
+weights (`model.weights`) and the valid-signal crop (`model.receptive_field`) are constants of the captured graph --
+changing them needs a new GraphedTrainer.
 
 The eager warm-up the capture needs (lazy state, cuFFT plans, kernel attributes) performs real optimiser
 updates; parameters, buffers and optimiser state are snapshotted before it and restored afterwards, so
@@ -49,6 +50,8 @@ class GraphedTrainer:
         self.phase2 = bool(model.warmed_up)
         kinds = (True, False) if self.phase2 else (False,)
         self._weights_at_capture = dict(model.weights)
+        # the valid-signal crop of the multiband loss is baked in at capture too (validation_epoch_end sets it once)
+        self._receptive_field_at_capture = model._receptive_field_host()
         model._beta_dev = torch.tensor(float(model.beta_factor), dtype=torch.float32, device=example_batch.device)
         gen_opt, dis_opt = model.optimizers()
         # the discriminator only changes in D-steps: its prepared weights become persistent buffers, rewritten in place
@@ -125,6 +128,9 @@ class GraphedTrainer:
         if self.model.weights != self._weights_at_capture:
             raise RuntimeError("GraphedTrainer: model.weights changed after capture (the loss weights are constants of "
                                "the captured graphs); build a new GraphedTrainer")
+        if self.model._receptive_field_host() != self._receptive_field_at_capture:
+            raise RuntimeError("GraphedTrainer: model.receptive_field changed after capture (the valid-signal crop is a "
+                               "constant of the captured graphs); build a new GraphedTrainer")
         self.model._beta_dev.fill_(float(self.model.beta_factor))
         self.x_static.copy_(batch, non_blocking=True)
         self.graphs[is_dis].replay()

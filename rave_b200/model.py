@@ -506,3 +506,39 @@ class RAVE(nn.Module):
             self.log("pred_fake", aux["pred_fake"].mean())
         self.log_dict(loss_gen)
         return self.logged
+
+    # ------------------------------------------------------------------ validation
+    def validation_step(self, x, batch_idx, eps: Optional[torch.Tensor] = None):
+        """rave/model.py:426-444: reconstruct one validation batch and log `validation`, the full-band spectral
+        distance (the fused spectral kernels).  Returns (cat([x, y], -1), posterior mean [B, D, L] or None), the
+        mean for a VariationalEncoder only.  `eps` injects the reparametrisation noise as in training_step."""
+        with torch.no_grad():
+            z = self.encode(x)
+            if isinstance(self.encoder, blocks.VariationalEncoder):
+                mean = torch.split(z, z.shape[1] // 2, 1)[0]
+            else:
+                mean = None
+            z = (self.encoder.reparametrize(z, eps) if eps is not None else self.encoder.reparametrize(z))[0]
+            y = self.decode(z)
+            distance = self.audio_distance(x, y)
+            self.log("validation", sum(distance.values()))
+            return torch.cat([x, y], -1), mean
+
+    def validation_epoch_end(self, out):
+        """rave/model.py:446-495 without the audio logging: probe the receptive field once (it turns on the
+        valid-signal crop of training_step), then, in phase 1 of a VariationalEncoder model, fit the latent PCA
+        (`latent_mean`, `latent_pca`, `fidelity`, read by the prior) on this epoch's posterior means and log
+        fidelity_{0.8,0.9,0.95,0.99}.  Other encoders only get the receptive field, as in the reference."""
+        if not sum(self._receptive_field_host()):
+            self.set_receptive_field(*core.get_rave_receptive_field(self, n_channels=self.n_channels))
+        if not len(out):
+            return
+        if not self.warmed_up and isinstance(self.encoder, blocks.VariationalEncoder):
+            latent_mean, components, fidelity = core.latent_analysis([mean for _, mean in out], self.latent_size)
+            with torch.no_grad():
+                self.latent_mean.copy_(latent_mean)
+                self.latent_pca.copy_(components)
+                self.fidelity.copy_(fidelity)
+            for p in (.8, .9, .95, .99):
+                self.log(f"fidelity_{p}", (fidelity > p).to(torch.uint8).argmax().float())
+        self.eval_number += 1

@@ -346,6 +346,26 @@ def sphere_norm(z):
     return SphereNormFn.apply(z)
 
 
+def latent_moments(z, D, state):
+    """Accumulates the rows z[b, :D, t] of z [B, C, L] (fp32, C >= D) into state = [n | mean[D] | M2[D*D]] (fp64, in
+    place) with rave_latent_moments; the only allocation is the kernel's workspace."""
+    B, C, L = z.shape
+    if not (z.dtype == torch.float32 and z.stride(2) == 1 and z.stride(1) == L and (B == 1 or z.stride(0) >= C * L)
+            and z.stride(0) % L == 0):
+        z = _f32c(z)
+    elif B > 1:
+        C = z.stride(0) // L            # a channel slice of a [B, C', L] buffer (the mean half of the encoder output)
+    if state.dtype != torch.float64 or state.numel() != 1 + D + D * D or not state.is_contiguous():
+        raise _lib.RaveB200Error(f"latent_moments: state must be a contiguous fp64 tensor of 1 + D + D^2 = "
+                                 f"{1 + D + D * D} elements")
+    nbytes = int(_lib.load().rave_latent_moments_workspace_bytes(B, L, D))
+    work = torch.empty(max(nbytes, 8) // 8, dtype=torch.float64, device=z.device)
+    if not z.is_cuda:
+        raise _lib.RaveB200Error("rave_b200 ops need CUDA tensors (there is no CPU path)")
+    call("rave_latent_moments", z.data_ptr(), B, C, L, D, ptr(state), ptr(work), stream_ptr())
+    return state
+
+
 def am_tanh(x):
     """tanh(x[:, :C] * sigmoid(x[:, C:])) -- GeneratorV2 tail, rave/blocks.py:704-711."""
     return AmTanhFn.apply(x)
@@ -1237,6 +1257,28 @@ def mel_log1p(X, band, weights, n_mels, scale, batch, channels):
     call("rave_mel_log1p_fwd", ptr(torch.view_as_real(X)), ptr(band), ptr(weights), ptr(out), N, F, bins, n_mels,
          weights.numel(), float(scale), stream_ptr())
     return out
+
+
+class MelLog1pFn(torch.autograd.Function):
+    """mel_log1p with a gradient with respect to X (rave_mel_log1p_bwd): the receptive-field probe of a mel-input model
+    differentiates through the front end."""
+
+    @staticmethod
+    def forward(ctx, X, band, weights, n_mels, scale, batch, channels):
+        X = X.contiguous()
+        ctx.save_for_backward(X, band, weights)
+        ctx.dims = (n_mels, float(scale))
+        return mel_log1p(X, band, weights, n_mels, scale, batch, channels)
+
+    @staticmethod
+    def backward(ctx, dy):
+        X, band, weights = ctx.saved_tensors
+        n_mels, scale = ctx.dims
+        N, F, bins = X.shape
+        dX = torch.empty_like(X)
+        call("rave_mel_log1p_bwd", ptr(torch.view_as_real(X)), ptr(band), ptr(weights), ptr(_f32c(dy)),
+             ptr(torch.view_as_real(dX)), N, F, bins, n_mels, weights.numel(), scale, stream_ptr())
+        return dX, None, None, None, None, None, None
 
 
 def _dptr(t, offset=0):
