@@ -20,7 +20,7 @@ each a stride-1 conv over the taps of that phase (no zero-insertion, no wasted M
 """
 from dataclasses import dataclass, field
 from functools import partial
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, NamedTuple, Optional, Tuple
 
 import torch
 import torch.nn as nn
@@ -282,55 +282,67 @@ def _wide_wgrad_taps(K: int, stride: int, pad: int):
     return max(js) - jmin + 1, -jmin, slots
 
 
+class ConvLaunch(NamedTuple):
+    """One ops.conv1d_tc launch of a prepared layer: the tap-major weight and the geometry it is read with.  phases > 1:
+    the launch is the `phases` interleaved phases of a transposed map side by side, output row q holding positions
+    q*phases .. q*phases + phases-1 (weight [J][phases*C][C'], see _fused_phase_taps)."""
+    w: Optional[torch.Tensor]
+    stride: int
+    dil: int
+    pad: Tuple[int, int]      # as conv1d_tc takes it: (left, right)
+    phases: int = 1
+
+
 class _PreparedWeights:
-    """Effective weight of one layer in every tap-major bf16 layout the kernels need.  `plan()` decides
-    which layouts / tap orders are required; `prepare_layers()` produces them for a whole chain with ONE
-    multi-tensor launch pair (row norms + re-layout): rave_weight_prep_tc_multi."""
+    """Effective weight of one layer in every tap-major bf16 layout the kernels need, and the launch (`fwd`, `dgrad`:
+    ConvLaunch) each layout is read by.  `prepare_layers()` produces the layouts for a whole chain with ONE multi-tensor
+    launch pair (row norms + re-layout): rave_weight_prep_tc_multi."""
 
     def __init__(self, spec: LayerSpec, need_dgrad: bool, need_fwd: bool):
         self.spec = spec
-        K, s = spec.K, spec.stride
+        K, s, dil, pad_l = spec.K, spec.stride, spec.dil, spec.pad[0]
         if spec.kind == "conv":
             self.C0p, self.C1p = spec.Cout + spec.cout_pad, spec.Cin + spec.cin_pad
         else:
             self.C0p, self.C1p = spec.Cin + spec.cin_pad, spec.Cout + spec.cout_pad
         self.norm = None
-        self.fwd = None           # conv: [K][Cout][Cin]
-        self.fwd_fused = None     # convT: all output phases as one conv, wt [J][stride*Cout][Cin] (see
-        self.dgrad = None         #   _fused_phase_taps); stride-1 conv: flipped taps [K][Cin][Cout]; convT: [K][Cin][Cout]
-        self.dgrad_fused = None   # strided conv: all input phases as one conv, wt [J][stride*Cin][Cout]
-        self.fused_J = self.fused_pad = 0
-        self.need_dgrad = need_dgrad
-        self.need_fwd = need_fwd
         self.raw = None           # (norm, outA, outB) as produced by the prep kernel (refresh_static_prep rewrites them)
+        # tapsA feeds the launch without phases (conv forward, convT dgrad: [K][C0][C1]), tapsB the transposed one
+        # (stride-1 conv dgrad: flipped taps [K][C1][C0]; strided conv dgrad, convT forward: all phases in one launch)
+        self.fwd = self.dgrad = None
         if spec.kind == "conv":
             self.tapsA = list(range(K)) if need_fwd else []
+            self.fwd = ConvLaunch(None, s, dil, spec.pad) if need_fwd else None
             if not need_dgrad:
                 self.tapsB = []
             elif s == 1:
                 self.tapsB = list(range(K - 1, -1, -1))
+                self.dgrad = ConvLaunch(None, 1, dil, ((K - 1) * dil - pad_l, 0))
             else:
-                self.tapsB, self.fused_J, self.fused_pad = _fused_phase_taps(K, s, spec.pad[0])
+                self.tapsB, _, fused_pad = _fused_phase_taps(K, s, pad_l)
+                self.dgrad = ConvLaunch(None, 1, 1, (fused_pad, 0), s)
         else:
-            self.tapsB, self.fused_J, self.fused_pad = _fused_phase_taps(K, s, spec.pad[0])
+            self.tapsB, _, fused_pad = _fused_phase_taps(K, s, pad_l)
+            self.fwd = ConvLaunch(None, 1, 1, (fused_pad, 0), s)
             self.tapsA = list(range(K)) if need_dgrad else []
+            if need_dgrad:
+                self.dgrad = ConvLaunch(None, s, 1, (pad_l, 0))
         if len(self.tapsB) > 32:
             raise _lib.RaveB200Error(f"phase-fused layout of K={K}, stride={s} needs {len(self.tapsB)} > 32 slabs")
 
-    def finalize(self, norm, outA, outB, parts: int = 1):
-        """parts = 2: split-operand layouts, [all hi slabs | all lo slabs] along the leading axis."""
-        spec = self.spec
+    def finalize(self, norm, outA, outB):
+        """Attach the prep kernel's layouts to the launches (split-operand layouts, [all hi slabs | all lo slabs] along
+        the leading axis, keep that order in the phase-wide view)."""
         self.norm = norm
-        if spec.kind == "conv":
-            self.fwd = outA
-            if self.need_dgrad:
-                if spec.stride == 1:
-                    self.dgrad = outB
-                else:       # [J*stride][Cin_p][Cout_p] -> [J][stride*Cin_p][Cout_p]
-                    self.dgrad_fused = outB.view(parts * self.fused_J, spec.stride * self.C1p, self.C0p)
-        else:               # [J*stride][Cout_p][Cin_p] -> [J][stride*Cout_p][Cin_p]
-            self.fwd_fused = outB.view(parts * self.fused_J, spec.stride * self.C1p, self.C0p)
-            self.dgrad = outA
+
+        def attach(launch, w):
+            if launch is None:
+                return None
+            if launch.phases > 1:       # [J*phases][C1p][C0p] -> [J][phases*C1p][C0p]
+                w = w.view(-1, launch.phases * self.C1p, self.C0p)
+            return launch._replace(w=w)
+        fwd_w, dgrad_w = (outA, outB) if self.spec.kind == "conv" else (outB, outA)
+        self.fwd, self.dgrad = attach(self.fwd, fwd_w), attach(self.dgrad, dgrad_w)
         return self
 
 
@@ -468,7 +480,7 @@ def prepare_layers(jobs, x3: bool = False):
     if work:
         res = ops.weight_prep_tc_multi([(v, g, pw.tapsA, pw.tapsB, pw.C0p, pw.C1p) for (pw, v, g) in work], x3=x3)
         for (pw, _, _), raw in zip(work, res):
-            pw.finalize(*raw, 2 if x3 else 1)
+            pw.finalize(*raw)
             pw.raw = raw
     for (i, skey, key, capturing, pw, v, g) in misses:
         out[i] = pw
@@ -510,6 +522,49 @@ def _zero_rows(tensors, lo: int, hi: int) -> None:
         for t in tensors:
             if t is not None:
                 t[:, lo:hi].zero_()
+
+
+def _conv(launch: ConvLaunch, x, Lin: int, Lout: int, pitch: int, act: int, slope: float, out_f32=None, out_act=None,
+          bias=None, res=None, res_act=None, res_slope: float = 0.2, res_bf16=None, dact_src=None, fm_d=None,
+          fm_partner=None, x3: bool = False) -> None:
+    """ops.conv1d_tc of a prepared launch writing positions [0, Lout) of the [B][pitch][C] outputs.  A phase-fused launch
+    sees every per-position tensor (outputs, residuals, dact_src, fm_partner) with `phases` positions per row -- the
+    same bytes -- and computes every row: the caller zeroes the slack rows after it."""
+    q = launch.phases
+    act_cs = 0
+    if q > 1:
+        if pitch % q:
+            raise _lib.RaveB200Error("phase-fused conv: the row pitch must be a multiple of the stride")
+        pitch = Lout = pitch // q
+
+        def wide(t):
+            return t.view(t.shape[0], pitch, q * t.shape[2]) if t is not None else None
+        out_f32, out_act, res, res_act, res_bf16, dact_src, fm_partner = (
+            wide(t) for t in (out_f32, out_act, res, res_act, res_bf16, dact_src, fm_partner))
+        if bias is not None:
+            bias = bias.detach().repeat(q)
+        if x3:                    # [hi | lo] pairs per position, not per row
+            act_cs = launch.w.shape[1] // q
+    ops.conv1d_tc(x, launch.w, bias, res, launch.stride, launch.dil, launch.pad, act, slope, want_f32=False,
+                  want_act=False, out_f32=out_f32, out_act=out_act, out_rows=pitch, Lout=Lout, Lin=Lin,
+                  res_bf16=res_bf16, dact_src=dact_src, res_act=res_act, res_slope=res_slope, fm_d=fm_d,
+                  fm_partner=fm_partner, x3=x3, act_cs=act_cs)
+
+
+def _fused_unit(specs: List[LayerSpec], flat, lens: List[int], i: int, in_pitch: int) -> bool:
+    """True when layers i, i+1 are a Residual(DilatedUnit) -- act -> conv3(dil) -> act -> conv1x1 -> + x -- that one
+    ops.dilated_unit_tc launch (csrc/unit_tc.cu) can run: LeakyReLU, no bias, equal widths it supports, a length the
+    unit keeps and an operand pitch equal to the output's (`in_pitch`)."""
+    if i + 1 >= len(specs):
+        return False
+    s, s1 = specs[i], specs[i + 1]
+    s2 = specs[i + 2] if i + 2 < len(specs) else None
+    return (s.kind == "conv" and s1.kind == "conv" and s.K == 3 and s1.K == 1 and s.stride == 1 and s1.stride == 1
+            and s.pre_act == ops.ACT_LEAKY and s1.pre_act == ops.ACT_LEAKY and s1.res_opnd == i
+            and s.res_src is None and s.res_opnd is None and flat[3 * i + 2] is None and flat[3 * i + 5] is None
+            and s.Cin == s.Cout == s1.Cin == s1.Cout and not (s.cin_pad or s.cout_pad or s1.cin_pad or s1.cout_pad)
+            and lens[i] == lens[i + 1] == lens[i + 2] and ops.dilated_unit_tc_supported(s.Cin, lens[i])
+            and _pitch(lens[i + 1], s2) == in_pitch)
 
 
 class RawFirstLayer:
@@ -569,11 +624,10 @@ class RawFirstLayer:
         im2col = ops.im2col_c1 if a.dim() == 2 else ops.im2col_cin         # mono rows [Bs, T] / [Bs, Cin, T]
         self.X = im2col(a, self.Lin, self.Lout, self.Xp, s.K, s.stride, s.pad[0], self.period, self.pool)
         w_fwd, self.w_dgrad, bias_g = self.weights()
+        # positions Lout .. Xp-1 of the last group see zero taps but get the bias: the caller zeroes them
         ops.conv1d_tc(self._rows(self.X), w_fwd, bias_g, None, 1, 1, (0, 0), act_code, act_slope, want_f32=False,
                       want_act=False, out_f32=self._rows(out_f32), out_act=self._rows(out_act), Lout=rows, Lin=rows,
                       out_rows=self.pitch // self.G)
-        # positions Lout .. Xp-1 of the last group saw zero taps but got the bias
-        _zero_rows((out_f32, out_act), self.Lout, self.Xp)
 
     def wgrad(self, g, db):
         """Weight gradient partials [1][K][Cout][Cin] from the output gradient g [B][pitch][Cout_p]; the bias gradient
@@ -642,6 +696,7 @@ class TcChainFn(torch.autograd.Function):
         if alpha_idx and (x3 or fm):
             raise _lib.RaveB200Error("Snake chains run in the plain bf16 mode only (no split operands, no fused fm)")
         hraw: Dict[int, torch.Tensor] = {}     # raw (pre-Snake) bf16 input stream of layer i
+        lens = [L0] + chain_lengths(specs, L0)
         raw: Optional[RawFirstLayer] = None
         period = 1
         if x_in.dim() == 2 or src is not None:         # raw fp32 signal, read in place by the first layer
@@ -650,9 +705,8 @@ class TcChainFn(torch.autograd.Function):
             if not raw_input_ok(specs[0], cin):
                 raise _lib.RaveB200Error("raw fp32 rows are only accepted by a first conv with Cin = the signal's "
                                          "channels, Cin * K <= 32 and no dilation")
-            Lout0 = _out_len(specs[0], L0)
-            raw = RawFirstLayer(specs[0], cin, period, pool, x_in.shape, _pitch(Lout0, specs[1] if n > 1 else None),
-                                L0, Lout0)
+            raw = RawFirstLayer(specs[0], cin, period, pool, x_in.shape, _pitch(lens[1], specs[1] if n > 1 else None),
+                                L0, lens[1])
         B = x_in.shape[0] * period
         ctx.B = B
         # backward on the fake half only (see backward): always available to the fused feature-matching chains, and to
@@ -664,8 +718,6 @@ class TcChainFn(torch.autograd.Function):
         a = x_in
         f32: Dict[int, torch.Tensor] = {}
         acts: List[torch.Tensor] = []                 # operand consumed by layer i
-        prepared: List[_PreparedWeights] = []
-        lens = [L0]
         outputs = []
         stats = torch.zeros(max(n - 1, 1), 2, dtype=torch.float32, device=dev) if fm else None
         jobs = []
@@ -674,50 +726,19 @@ class TcChainFn(torch.autograd.Function):
             jobs.append((s, flat[3 * i].detach(), flat[3 * i + 1].detach() if flat[3 * i + 1] is not None else None,
                          need_dgrad and not own, not own))
         prepared = prepare_layers(jobs, x3=x3)
-        fused_second = False
-        for i, s in enumerate(specs):
-            if fused_second:           # the 1x1 conv of a unit the previous iteration ran as one fused launch
-                fused_second = False
-                continue
-            v, g, bias = flat[3 * i], flat[3 * i + 1], flat[3 * i + 2]
-            use_raw = raw is not None and i == 0
-            pw = prepared[i]
-            Lin = lens[-1]
-            Lout = _out_len(s, Lin)
-            s1 = specs[i + 1] if i + 1 < n else None
-            if (FUSE_UNITS and not x3 and not fm and not use_raw and s1 is not None and ACT_DTYPE == torch.bfloat16
-                    and s.kind == "conv" and s1.kind == "conv" and s.K == 3 and s1.K == 1 and s.stride == 1
-                    and s1.stride == 1 and s.pre_act == ops.ACT_LEAKY and s1.pre_act == ops.ACT_LEAKY
-                    and s1.res_opnd == i and s.res_src is None and s.res_opnd is None and bias is None
-                    and flat[3 * i + 5] is None and s.Cin == s.Cout == s1.Cin == s1.Cout
-                    and not (s.cin_pad or s.cout_pad or s1.cin_pad or s1.cout_pad) and Lout == Lin
-                    and ops.dilated_unit_tc_supported(s.Cin, Lin)):
-                # Residual(DilatedUnit) = act -> conv3(dil) -> act -> conv1x1 -> + x in ONE kernel: the intermediate
-                # operand stays in shared memory (written to HBM only when a backward will need it)
-                s2 = specs[i + 2] if i + 2 < n else None
-                pitch = _pitch(Lout, s2)
-                if pitch == a.shape[1]:
-                    want_f32 = s1.want_f32
-                    out_f32 = torch.empty(B, pitch, s.Cout, dtype=torch.float32, device=dev) if want_f32 else None
-                    out_act = torch.empty(B, pitch, s.Cout, dtype=ACT_DTYPE, device=dev) if s2 is not None else None
-                    _zero_rows((out_f32, out_act), Lout, pitch)
-                    a1, _, _ = ops.dilated_unit_tc(a, pw.fwd, prepared[i + 1].fwd, s.dil, s.pad[0], s.pre_slope,
-                                                   s1.pre_slope, s2.pre_act if s2 is not None else ops.ACT_NONE,
-                                                   s2.pre_slope if s2 is not None else 0.0, L=Lout, want_a1=need_dgrad,
-                                                   out_f32=out_f32, out_act=out_act)
-                    acts.append(a)
-                    acts.append(a1)
-                    lens.append(Lout)
-                    lens.append(Lout)
-                    if want_f32:
-                        f32[i + 1] = out_f32
-                    if s1.is_output:
-                        outputs.append(out_f32)
-                    a = out_act
-                    fused_second = True
-                    continue
-            lens.append(Lout)
-            nxt = specs[i + 1] if i + 1 < n else None
+        # one step per launch, (first layer, last layer): a Residual(DilatedUnit) runs as ONE kernel where it can (the
+        # intermediate operand stays in shared memory, written to HBM only when a backward will need it)
+        fuse = FUSE_UNITS and not x3 and not fm and ACT_DTYPE == torch.bfloat16
+        steps, i = [], 0
+        while i < n:
+            in_pitch = x_in.shape[1] if i == 0 else _pitch(lens[i], specs[i])
+            j = i + 1 if fuse and (raw is None or i > 0) and _fused_unit(specs, flat, lens, i, in_pitch) else i
+            steps.append((i, j))
+            i = j + 1
+        for i, j in steps:
+            s = specs[j]                # the layer whose output this step writes
+            Lout = lens[j + 1]
+            nxt = specs[j + 1] if j + 1 < n else None
             want_act = nxt is not None
             act_code = nxt.pre_act if nxt is not None else ops.ACT_NONE
             act_slope = nxt.pre_slope if nxt is not None else 0.0
@@ -727,50 +748,43 @@ class TcChainFn(torch.autograd.Function):
             want_f32 = s.want_f32 and not (fm and nxt is not None)
             pitch = _pitch(Lout, nxt)
             cout_p = s.Cout + s.cout_pad
-            bias_p = bias
-            if bias is not None and s.cout_pad:
-                bias_p = nn.functional.pad(bias.detach(), (0, s.cout_pad))
-            res = res_act = res_b16 = None
-            res_slope = 0.2
-            if s.res_opnd is not None:
-                res_act, res_slope = acts[s.res_opnd], specs[s.res_opnd].pre_slope
-            elif s.res_raw is not None:
-                res_b16 = hraw[s.res_raw]
-            elif s.res_src is not None:
-                res = f32[s.res_src]
             out_f32 = torch.empty(B, pitch, cout_p, dtype=torch.float32, device=dev) if want_f32 else None
             out_act = torch.empty(B, pitch, AW * cout_p, dtype=ACT_DTYPE, device=dev) if want_act else None
-            _zero_rows((out_f32, out_act), Lout, pitch)
             acts.append(a)
-            if use_raw:
+            if j > i:
+                unit = prepared[i].fwd
+                a1, _, _ = ops.dilated_unit_tc(a, unit.w, prepared[j].fwd.w, unit.dil, unit.pad[0], specs[i].pre_slope,
+                                               s.pre_slope, act_code, act_slope, L=Lout, want_a1=need_dgrad,
+                                               out_f32=out_f32, out_act=out_act)
+                acts.append(a1)
+            elif raw is not None and i == 0:
                 raw.forward(a, out_f32, out_act, act_code, act_slope)
-            elif s.kind == "conv":
-                ops.conv1d_tc(a, pw.fwd, bias_p, res, s.stride, s.dil, s.pad, act_code, act_slope,
-                              want_f32=False, want_act=False, out_f32=out_f32, out_act=out_act, Lout=Lout,
-                              Lin=Lin, out_rows=pitch, res_act=res_act, res_slope=res_slope, x3=x3, res_bf16=res_b16)
             else:
-                # transposed conv: the `stride` output phases side by side in one stride-1 conv (output row q =
-                # positions q*stride .. q*stride + stride-1: the same bytes as the [B][pitch][Cout] tensor)
-                st = s.stride
-                if pitch % st:
-                    raise _lib.RaveB200Error("transposed conv: the output pitch must be a multiple of the stride")
-                rows_q = pitch // st
-                bias_f = bias_p.detach().repeat(st) if bias_p is not None else None
-                ops.conv1d_tc(a, pw.fwd_fused, bias_f, None, 1, 1, (pw.fused_pad, 0), act_code, act_slope,
-                              want_f32=False, want_act=False,
-                              out_f32=out_f32.view(B, rows_q, st * cout_p) if out_f32 is not None else None,
-                              out_act=out_act.view(B, rows_q, st * AW * cout_p) if out_act is not None else None,
-                              out_rows=rows_q, Lout=rows_q, Lin=Lin, x3=x3, act_cs=cout_p if x3 else 0)
-                _zero_rows((out_f32, out_act), Lout, pitch)     # positions beyond the true length were computed too
+                bias = flat[3 * i + 2]
+                if bias is not None and s.cout_pad:
+                    bias = nn.functional.pad(bias.detach(), (0, s.cout_pad))
+                res = res_act = res_b16 = None
+                res_slope = 0.2
+                if s.res_opnd is not None:
+                    res_act, res_slope = acts[s.res_opnd], specs[s.res_opnd].pre_slope
+                elif s.res_raw is not None:
+                    res_b16 = hraw[s.res_raw]
+                elif s.res_src is not None:
+                    res = f32[s.res_src]
+                _conv(prepared[i].fwd, a, lens[i], Lout, pitch, act_code, act_slope, out_f32=out_f32, out_act=out_act,
+                      bias=bias, res=res, res_act=res_act, res_slope=res_slope, res_bf16=res_b16, x3=x3)
+            # positions past the true length: rows a launch did not write, or computed from zero taps (phase-fused
+            # launches, the last group of a raw first layer)
+            _zero_rows((out_f32, out_act), Lout, pitch)
             if snake_next:
-                hraw[i + 1] = out_act
-                out_act = ops.snake_cl_fwd(out_act, flat[alpha_idx[i + 1]])
+                hraw[j + 1] = out_act
+                out_act = ops.snake_cl_fwd(out_act, flat[alpha_idx[j + 1]])
             if fm and nxt is not None:
                 if act_code != ops.ACT_LEAKY or s.cout_pad:
                     raise _lib.RaveB200Error("feature-matching mode needs LeakyReLU between the layers")
-                ops.fm_stats(out_act, stats[i], Lout, act_slope)
+                ops.fm_stats(out_act, stats[j], Lout, act_slope)
             if want_f32:
-                f32[i] = out_f32
+                f32[j] = out_f32
             if (s.is_output and not fm) or (fm and nxt is None):
                 outputs.append(out_f32)
             a = out_act
@@ -832,7 +846,6 @@ class TcChainFn(torch.autograd.Function):
         g_cur: Optional[torch.Tensor] = None   # gradient (h-space) of layer i's output
         grads = [None] * len(flat)
         gx = None
-        gx_full = None
         wn_jobs = []       # (layer, dwt partials, v, g, norm): one multi-tensor launch at the end
         # bias gradients accumulated by the wgrad kernels: ONE zero-filled buffer for the whole chain
         db_off, db_total = {}, 0
@@ -916,59 +929,27 @@ class TcChainFn(torch.autograd.Function):
             if fo and i == 0:
                 # fake-rows-only backward: the chain's input gradient is [zeros; gx_fake] -- the last dgrad writes its
                 # rows straight into the second half of the full buffer (no zeros + copy pass afterwards)
-                gx_full = torch.empty(ctx.B, in_pitch, cin_p, dtype=ACT_DTYPE, device=g.device)
-                gx_full[:Bh].zero_()
-                gp = gx_full[Bh:]
+                gx = torch.empty(ctx.B, in_pitch, cin_p, dtype=ACT_DTYPE, device=g.device)
+                gx[:Bh].zero_()
+                gp = gx[Bh:]
             else:
                 gp = torch.empty(B, in_pitch, cin_p, dtype=ACT_DTYPE, device=g.device)
+            _conv(pw.dgrad, g, Lout, Lin, in_pitch, ops.ACT_NONE, s.pre_slope, out_act=gp, res_bf16=add_conv,
+                  dact_src=dact, fm_d=fm_d, fm_partner=fm_partner)
             _zero_rows((gp,), Lin, in_pitch)
-            if s.kind == "conv":
-                if s.stride == 1:
-                    padp = (s.K - 1) * s.dil - s.pad[0]
-                    ops.conv1d_tc(g, pw.dgrad, None, None, 1, s.dil, (padp, 0), ops.ACT_NONE, s.pre_slope,
-                                  want_f32=False, want_act=False, out_act=gp, Lout=Lin, Lin=Lout,
-                                  out_rows=in_pitch, res_bf16=add_conv, dact_src=dact, fm_d=fm_d,
-                                  fm_partner=fm_partner)
-                else:
-                    # strided conv: the `stride` input phases side by side in one stride-1 conv over g (row q of the
-                    # result = input positions q*stride .. +stride-1); g rows are fetched once, not once per phase
-                    st = s.stride
-                    if in_pitch % st:
-                        raise _lib.RaveB200Error("strided conv dgrad: the operand pitch must be a multiple of the stride")
-                    rows_q = in_pitch // st
-                    wide = st * cin_p
-
-                    def v4(t):
-                        return t.view(B, rows_q, wide) if t is not None else None
-                    ops.conv1d_tc(g, pw.dgrad_fused, None, None, 1, 1, (pw.fused_pad, 0), ops.ACT_NONE, s.pre_slope,
-                                  want_f32=False, want_act=False, out_act=v4(gp), out_rows=rows_q, Lout=rows_q,
-                                  Lin=Lout, res_bf16=v4(add_conv), dact_src=v4(dact), fm_d=fm_d,
-                                  fm_partner=v4(fm_partner))
-                    _zero_rows((gp,), Lin, in_pitch)
-            else:
-                ops.conv1d_tc(g, pw.dgrad, None, None, s.stride, 1, (s.pad[0], 0), ops.ACT_NONE, s.pre_slope,
-                              want_f32=False, want_act=False, out_act=gp, Lout=Lin, Lin=Lout, out_rows=in_pitch,
-                              res_bf16=add_conv, dact_src=dact, fm_d=fm_d, fm_partner=fm_partner)
             if snake_here:
                 al = flat[ctx.alpha_idx[i]]
                 gp, dal = ops.snake_cl_bwd(gp, ctx.hraw[i], al, add, want_dalpha=bool(al.requires_grad))
                 if dal is not None:
                     grads[ctx.alpha_idx[i]] = dal.reshape(al.shape)
             g_cur = gp
-            if i == 0:
+            if i == 0 and not fo:       # (fake rows only: no Snake, gp is the second half of gx)
                 gx = gp
         if wn_jobs:
             res = ops.weight_norm_bwd_multi([job[1:] for job in wn_jobs])
             for job, (dv, dg) in zip(wn_jobs, res):
                 i = job[0]
                 grads[3 * i], grads[3 * i + 1] = dv, dg
-        if fo and gx is not None and ctx.raw is None and gx.shape[0] == Bh:
-            if gx_full is not None and gx.data_ptr() == gx_full[Bh:].data_ptr() and gx.shape == gx_full[Bh:].shape:
-                gx = gx_full                 # the real rows' gradient is identically unused: zeros
-            else:
-                full = torch.zeros((ctx.B,) + tuple(gx.shape[1:]), dtype=gx.dtype, device=gx.device)
-                full[Bh:] = gx
-                gx = full
         return (gx, None, None, None, None, None, None) + tuple(grads)
 
 
