@@ -499,6 +499,30 @@ int rave_prior_head_ce_bwd(const void *x, const float *w, const float *bias, con
                            void *dx, float *dw, float *dbias, int B, int Tp, int D, int R, int Cin, int cl_bf16,
                            float slope, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Sampling from the latent prior (Prior.generate / validation_epoch_end), fp32 CUDA-core arithmetic, fixed-order sums.
+ *   prior_sample:   `params` = host array of the 2 + 6 n_layers + 4 device pointers of Prior._trained_parameters()
+ *                   (pre_net.0 w/b, per block dconv w/b, rconv w/b, sconv w/b, post_net.0 w/b, post_net.2 w/b); block i
+ *                   has dilation 2^(i mod cycle_size).  prefix [B][P][D] int32, uniform [B][T][D] (frames < P unused;
+ *                   may be NULL with argmax), classes [B][T][D] int32 out (frames < P copied from the prefix), logits
+ *                   [B][T-1][D][R] out or NULL.  Step i consumes frame i and produces frame i + 1 (the prefix's while
+ *                   i + 1 < P); a class is the first argmax, or the first r whose running softmax probability exceeds u
+ *                   (the last r of non-zero probability if none does).  State lives in `work`
+ *                   (rave_prior_sample_workspace_bytes, -1 for a bad shape) and is reset by every call.  The call
+ *                   captures and replays its own CUDA graph, so it refuses to run inside a stream capture.
+ *                   1 <= B <= 64, D divides res_size and skp_size, K <= 8, R <= 1024, 1 <= P <= T.
+ *   classes_to_latent: classes [B][T][D], dither [B][T][D], noise [B][L-D][T-D+1] (NULL when L = D), latent_pca [L][L],
+ *                   latent_mean [L] -> z [B][L][T-D+1] = latent_pca^T [y ; noise] + latent_mean, y[d][t] =
+ *                   clamp(erfinv(2 x - 1) sqrt 2, -4, 4) of x = k / R + dither / R, k = classes[b][t + d][d]
+ *                   (QuantizedNormal.decode, DiagonalShift.inverse, VariationalPrior.pre_process_latent)
+ * ------------------------------------------------------------------------------------------- */
+long rave_prior_sample_workspace_bytes(int B, int n_layers, int cycle_size, int res_size, int skp_size, int K, int D);
+int rave_prior_sample(const float *const *params, int n_layers, int cycle_size, int res_size, int skp_size, int K, int R,
+                      int D, const int *prefix, int P, const float *uniform, int T, int B, int argmax, int *classes,
+                      float *logits, void *work, long work_bytes, void *stream);
+int rave_prior_classes_to_latent(const int *classes, const float *dither, const float *noise, const float *latent_pca,
+                                 const float *latent_mean, float *z, int B, int T, int D, int L, int R, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

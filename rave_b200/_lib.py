@@ -117,6 +117,9 @@ SIGNATURES = {
     "rave_gate_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P]),
     "rave_prior_head_ce_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
     "rave_prior_head_ce_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
+    "rave_prior_sample_workspace_bytes": (c_long, [_I, _I, _I, _I, _I, _I, _I]),
+    "rave_prior_sample": (c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _I, _I, _I, _P, _P, _P, _L, _P]),
+    "rave_prior_classes_to_latent": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
 }
 
 

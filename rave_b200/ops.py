@@ -1460,3 +1460,44 @@ def prior_head_ce_bwd(x, w, bias, cls, gloss, cl, slope=0.2):
     call("rave_prior_head_ce_bwd", ptr(x), ptr(_f32c(w)), ptr(_f32c(bias)), ptr(cls), ptr(_f32c(gloss)), ptr(dx),
          ptr(dw), ptr(db), B, Tp, D, R, Cin, int(cl), float(slope), stream_ptr())
     return dx, dw, db
+
+
+def prior_sample(params, dilation_cycle, prefix, uniform, n_frames, R, argmax, return_logits):
+    """Cached sampling of the prior (csrc/prior_sample.cu) from its trained parameters (Prior._trained_parameters order):
+    int32 prefix [B, P, D], fp32 uniform [B, n_frames, D] (None with argmax) -> (classes [B, n_frames, D] int32,
+    logits [B, n_frames - 1, D, R] or None)."""
+    import ctypes
+    n_layers = (len(params) - 6) // 6
+    C, _, K = params[0].shape
+    Sk = params[-4].shape[0]
+    B, P, D = prefix.shape
+    prefix = prefix.contiguous()
+    if prefix.dtype != torch.int32:
+        raise _lib.RaveB200Error(f"prior_sample: prefix must be int32, got {prefix.dtype}")
+    ps = [_f32c(p) for p in params]
+    arr = (ctypes.c_void_p * len(ps))(*[ptr(p) for p in ps])
+    nbytes = int(_lib.load().rave_prior_sample_workspace_bytes(B, n_layers, dilation_cycle, C, Sk, K, D))
+    if nbytes < 0:
+        raise _lib.RaveB200Error(f"prior_sample: bad shape (B {B}, {n_layers} layers, C {C}, Sk {Sk}, K {K}, D {D})")
+    work = torch.empty(nbytes, dtype=torch.uint8, device=prefix.device)
+    cls = torch.empty(B, n_frames, D, dtype=torch.int32, device=prefix.device)
+    logits = (torch.empty(B, max(n_frames - 1, 0), D, R, dtype=torch.float32, device=prefix.device)
+              if return_logits else None)
+    call("rave_prior_sample", arr, n_layers, dilation_cycle, C, Sk, K, R, D, ptr(prefix), P,
+         ptr(None if uniform is None else _f32c(uniform)), n_frames, B, int(argmax), ptr(cls), ptr(logits), ptr(work),
+         nbytes, stream_ptr())
+    return cls, logits
+
+
+def prior_classes_to_latent(classes, dither, noise, latent_pca, latent_mean, R):
+    """int32 classes [B, T, D], dither [B, T, D], noise [B, L - D, T - D + 1] -> RAVE latent z [B, L, T - D + 1]
+    (QuantizedNormal.decode, DiagonalShift.inverse and VariationalPrior.pre_process_latent in one kernel)."""
+    B, T, D = classes.shape
+    L = latent_pca.shape[0]
+    if classes.dtype != torch.int32:
+        raise _lib.RaveB200Error(f"prior_classes_to_latent: classes must be int32, got {classes.dtype}")
+    z = torch.empty(B, L, T - D + 1, dtype=torch.float32, device=classes.device)
+    call("rave_prior_classes_to_latent", ptr(classes.contiguous()), ptr(_f32c(dither)),
+         ptr(None if noise is None or L == D else _f32c(noise)), ptr(_f32c(latent_pca)), ptr(_f32c(latent_mean)),
+         ptr(z), B, T, D, L, R, stream_ptr())
+    return z

@@ -10,6 +10,9 @@ Training step (`training_step`), with D = latent_size, R = resolution, T' = T - 
      against the next frame's classes (ops.prior_head_ce_fwd); the backward runs the same plan in reverse.
 In bf16 mode (`rave_b200.set_precision("bf16")`) the convs are wgmma launches on channel-last bf16 operands with fp32
 residual and skip streams; in fp32 mode the same plan runs on the CUDA-core parity kernels in [B, C, T] fp32.
+Sampling (`sample`) is one library call (ops.prior_sample) with cached per-block state; `decode_classes` turns classes
+into audio through one kernel (ops.prior_classes_to_latent) and the RAVE decoder.  `generate` is the reference's dense
+loop.
 """
 import copy
 import math
@@ -183,6 +186,7 @@ class Prior(nn.Module):
 
         self.n_channels = n_channels
         self.val_idx = 0
+        self.cycle_size = cycle_size
         self.dilations = tuple(2**(i % cycle_size) for i in range(n_layers))
         rf = (kernel_size - 1) * sum(2**(np.arange(n_layers) % cycle_size)) + 1
         if pretrained_vae is not None:
@@ -255,6 +259,54 @@ class Prior(nn.Module):
             pred = self.post_process_prediction(pred, argmax=argmax)
             x[..., i + 1:i + 2] = pred
         return x
+
+    @torch.no_grad()
+    def sample(self, prefix, n_frames: int, argmax: bool = False, uniform=None, return_logits: bool = False):
+        """Cached autoregressive sampling: int32 classes [B, n_frames, D] that continue the int32 prefix [B, P, D]
+        (1 <= P <= n_frames, B <= 64), plus the logits [B, n_frames - 1, D, R] of every step if `return_logits`.
+
+        Step i reads frame i and writes frame i + 1 (the prefix's while i + 1 < P), like `generate`, but each step costs
+        one frame of work: every block keeps the inputs its dilated conv still needs, and the whole loop is one
+        library call (csrc/prior_sample.cu).  A class is the first argmax, or the first class whose running softmax
+        probability exceeds the uniform draw u = uniform[b, i + 1, d]: the same distribution as the reference's
+        `torch.multinomial`, whose draws cannot be reproduced bit for bit.  `uniform` [B, n_frames, D] injects the
+        draws (frames < P unused); by default they are `torch.rand` on the current CUDA generator.  fp32 kernels in
+        both precision modes."""
+        if not prefix.is_cuda:
+            raise _lib.RaveB200Error("the prior's sampler needs CUDA tensors (there is no CPU path)")
+        B, _, D = prefix.shape
+        if uniform is None and not argmax:
+            uniform = torch.rand(B, n_frames, D, device=prefix.device)
+        cls, logits = ops.prior_sample(self._trained_parameters(), self.cycle_size, prefix.to(torch.int32),
+                                       uniform, n_frames, self.quantized_normal.resolution, argmax, return_logits)
+        return (cls, logits) if return_logits else cls
+
+    @torch.no_grad()
+    def decode_classes(self, classes, dither=None, noise=None):
+        """Audio of int32 classes [B, T, D]: QuantizedNormal.decode, DiagonalShift.inverse and pre_process_latent in one
+        kernel (ops.prior_classes_to_latent), then synth.decode in eval mode.  `dither` [B, T, D] and `noise`
+        [B, L - D, T - D + 1] inject the draws; by default they are drawn as the reference draws them, in its order:
+        `torch.rand` on the classes' device, then `torch.randn` on the CPU."""
+        self.synth.eval()
+        B, T, D = classes.shape
+        L = self.synth.latent_pca.shape[0]
+        if dither is None:
+            dither = torch.rand(B, T, D, device=classes.device)
+        if noise is None:
+            noise = torch.randn(B, L - D, T - D + 1).to(classes.device)
+        z = ops.prior_classes_to_latent(classes.to(torch.int32), dither, noise, self.synth.latent_pca,
+                                        self.synth.latent_mean, self.quantized_normal.resolution)
+        return self.synth.decode(z)
+
+    @torch.no_grad()
+    def validation_epoch_end(self, out):
+        """The reference's generation: a random first frame (randn_like the encoded first validation batch, shifted and
+        quantised), `sample` over the shifted length, `decode_classes`; the audio goes to logged["generation"]."""
+        x = torch.randn_like(self.encode(out[0]))
+        cls = self.quantized_normal.classes(self.diagonal_shift(x)).permute(0, 2, 1).to(torch.int32)
+        cls = self.sample(cls[:, :1].contiguous(), cls.shape[1])
+        self.logged["generation"] = self.decode_classes(cls)
+        self.val_idx += 1
 
     def split_classes(self, x):
         # B x D*C x T
