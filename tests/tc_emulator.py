@@ -1,11 +1,45 @@
-"""TEST DOUBLE: torch-CPU emulation of the tensor-core entry points' documented semantics
-(include/rave_b200.h), used ONLY by tests/test_engine_cpu.py to exercise the host-side engine logic
-(planning, phase decomposition, pitches, the explicit backward) without a GPU.  Not part of the product."""
+"""TEST DOUBLE: torch emulation of the tensor-core entry points' documented semantics (include/rave_b200.h).  Not part
+of the product.  Two users:
+
+- tests/test_engine_cpu.py installs it in place of rave_b200.ops to exercise the host-side engine logic (planning, phase
+  decomposition, pitches, the explicit backward) without a GPU.  Default: fp32 arithmetic on the inputs' device.
+- tests/launch_checker.py evaluates it under `compute(torch.float64)` on the snapshotted operands of every launch the
+  engine issues on the GPU (tests/test_gpu_launch_replay.py), as the high-precision reference of each kernel.
+
+OPERAND_DTYPE is the type operands / bf16 outputs are rounded to; COMPUTE_DTYPE the type every sum is formed in.  Every
+entry point computes on its inputs' device."""
+import contextlib
+
 import torch
 import torch.nn.functional as F
 
 
 OPERAND_DTYPE = torch.bfloat16
+COMPUTE_DTYPE = torch.float32
+
+
+@contextlib.contextmanager
+def compute(dtype=torch.float64):
+    """Evaluate every entry point in `dtype` inside the block."""
+    global COMPUTE_DTYPE
+    saved = COMPUTE_DTYPE
+    COMPUTE_DTYPE = dtype
+    try:
+        yield
+    finally:
+        COMPUTE_DTYPE = saved
+
+
+def _c(t):
+    return t.to(COMPUTE_DTYPE)
+
+
+def _dev(t):
+    return t.device
+
+
+def _zeros(like, *shape):
+    return torch.zeros(*shape, dtype=COMPUTE_DTYPE, device=like.device)
 
 
 def _bf16(t):
@@ -18,15 +52,15 @@ def conv1d_tc(xa_cl, wt, bias=None, res_cl=None, stride=1, dil=1, pad=(0, 0), ac
               fm_d=None, fm_partner=None, x3=False, act_cs=0):
     if x3:
         return _conv1d_tc_x3(xa_cl, wt, bias, res_cl, stride, dil, pad, act, slope, out_f32, out_act, out_rows, Lout,
-                             Lin, res_act, res_slope, act_cs)
+                             Lin, res_act, res_slope, act_cs, out_row_stride, out_row_offset)
     B, in_pitch, Cin = xa_cl.shape
     Lin = in_pitch if Lin is None else Lin
     K, Cout, _ = wt.shape
     assert in_pitch >= -(-Lin // stride) * stride
     if in_pitch > Lin:
         assert float(xa_cl[:, Lin:].float().abs().max()) == 0.0, "slack rows must be zero"
-    x = xa_cl[:, :Lin].float().permute(0, 2, 1)                     # [B, Cin, Lin]
-    w = wt.float().permute(1, 2, 0)                                  # [Cout, Cin, K]
+    x = _c(xa_cl[:, :Lin]).permute(0, 2, 1)                         # [B, Cin, Lin]
+    w = _c(wt).permute(1, 2, 0)                                      # [Cout, Cin, K]
     if Lout is None:
         Lout = (Lin + pad[0] + pad[1] - dil * (K - 1) - 1) // stride + 1
     # rows l*stride + k*dil - pad_l, zero outside [0, Lin)
@@ -42,86 +76,90 @@ def conv1d_tc(xa_cl, wt, bias=None, res_cl=None, stride=1, dil=1, pad=(0, 0), ac
     y = F.conv1d(xp, w, None, stride, 0, dil)[..., :Lout]            # [B, Cout, Lout]
     v = y.permute(0, 2, 1)                                           # [B, Lout, Cout]
     if bias is not None:
-        v = v + bias
+        v = v + _c(bias)
     rows = out_rows if out_rows else Lout
-    ors = out_row_stride if out_row_stride else 1
-    idx = torch.arange(Lout) * ors + out_row_offset
+    idx = out_row_index(Lout, out_row_stride, out_row_offset, _dev(xa_cl))
     if dact_src is not None:
-        sgn = torch.signbit(dact_src[:, idx].float())
+        sgn = torch.signbit(_c(dact_src[:, idx]))
         v = torch.where(sgn, v * slope, v)
     if fm_d is not None and fm_partner is not None:      # fake half only: partner = the real rows
-        a = dact_src[:, idx].float()
-        ar = fm_partner[:, idx].float()
+        fd = _c(fm_d)
+        a = _c(dact_src[:, idx])
+        ar = _c(fm_partner[:, idx])
         hf, hr = torch.where(a > 0, a, a / slope), torch.where(ar > 0, ar, ar / slope)
-        v = v - fm_d[0] * torch.sign(hr - hf)
+        v = v - fd[0] * torch.sign(hr - hf)
     elif fm_d is not None:
-        a = dact_src[:, idx].float()
+        fd = _c(fm_d)
+        a = _c(dact_src[:, idx])
         h = torch.where(a > 0, a, a / slope)
         hr, hf = h[:B // 2], h[B // 2:]
         sd = torch.sign(hr - hf)
-        v = v + torch.cat([fm_d[0] * sd + fm_d[1] * torch.sign(hr), -fm_d[0] * sd], 0)
+        v = v + torch.cat([fd[0] * sd + fd[1] * torch.sign(hr), -fd[0] * sd], 0)
     if res_bf16 is not None:
-        v = v + res_bf16[:, idx].float()
+        v = v + _c(res_bf16[:, idx])
     if res_act is not None:
-        ra = res_act[:, idx].float()
+        ra = _c(res_act[:, idx])
         v = v + torch.where(ra > 0, ra, ra / res_slope)
     if res_cl is not None:
-        v = v + res_cl[:, idx]
+        v = v + _c(res_cl[:, idx])
     if want_f32 and out_f32 is None:
-        out_f32 = torch.zeros(B, rows, Cout)
+        out_f32 = _zeros(xa_cl, B, rows, Cout)
     if want_act and out_act is None:
-        out_act = torch.zeros(B, rows, Cout, dtype=OPERAND_DTYPE)
+        out_act = torch.zeros(B, rows, Cout, dtype=OPERAND_DTYPE, device=_dev(xa_cl))
     if out_f32 is not None:
-        out_f32[:, idx] = v
+        out_f32[:, idx] = v.to(out_f32.dtype)
     if out_act is not None:
         a = F.leaky_relu(v, slope) if act == 1 else v
-        out_act[:, idx] = _bf16(a)
+        out_act[:, idx] = _bf16(a).to(out_act.dtype)
     return out_f32, out_act
+
+
+def out_row_index(Lout, out_row_stride=0, out_row_offset=0, device=None):
+    """Rows of a [B][out_rows][C] output that positions 0 .. Lout-1 land in: l * out_row_stride + out_row_offset."""
+    return torch.arange(Lout, device=device) * (out_row_stride if out_row_stride else 1) + out_row_offset
 
 
 def _split(v):
     hi = v.to(torch.bfloat16)
-    lo = (v - hi.float()).to(torch.bfloat16)
+    lo = (v - hi.to(v.dtype)).to(torch.bfloat16)
     return hi, lo
 
 
 def _conv1d_tc_x3(xa_cl, wt, bias, res_cl, stride, dil, pad, act, slope, out_f32, out_act, out_rows, Lout, Lin, res_act,
-                  res_slope, act_cs):
+                  res_slope, act_cs, out_row_stride=0, out_row_offset=0):
     """Split-operand semantics of rave_conv1d_tc_fwd_x3 (include/rave_b200.h): rows [hi | lo], weights [2][K][Cout][Cin],
     hi*hi + lo*hi + hi*lo accumulated in fp32; out_act positions are [hi | lo] pairs of act_cs channels."""
     B, in_pitch, C2 = xa_cl.shape
     Cin = C2 // 2
     K = wt.shape[0] // 2
     Cout = wt.shape[1]
-    a_hi, a_lo = xa_cl[..., :Cin].float(), xa_cl[..., Cin:].float()
-    w_hi, w_lo = wt[:K].float(), wt[K:].float()
-    saved = OPERAND_DTYPE
+    a_hi, a_lo = xa_cl[..., :Cin], xa_cl[..., Cin:]
+    w_hi, w_lo = wt[:K], wt[K:]
 
     def run(a, w):
-        o, _ = conv1d_tc(a.to(torch.bfloat16), w.to(torch.bfloat16), None, None, stride, dil, pad, 0, slope,
-                         want_f32=True, want_act=False, out_rows=out_rows, Lout=Lout, Lin=Lin)
+        o, _ = conv1d_tc(a.contiguous(), w, None, None, stride, dil, pad, 0, slope, want_f32=True, want_act=False,
+                         Lout=Lout, Lin=Lin)
         return o
-    v = run(a_hi, w_hi) + run(a_lo, w_hi) + run(a_hi, w_lo)
-    rows = v.shape[1]
-    LoutE = Lout if Lout is not None else rows
+    v = run(a_hi, w_hi) + run(a_lo, w_hi) + run(a_hi, w_lo)          # [B, Lout, Cout]
+    LoutE = v.shape[1]
+    rows = out_rows if out_rows else LoutE
+    idx = out_row_index(LoutE, out_row_stride, out_row_offset, _dev(xa_cl))
     if bias is not None:
-        v[:, :LoutE] += bias
+        v = v + _c(bias)
     if res_act is not None:
-        ra = res_act[..., :Cout].float() + res_act[..., Cout:].float()
-        v[:, :LoutE] += torch.where(ra > 0, ra, ra / res_slope)[:, :LoutE]
+        ra = _c(res_act[:, idx, :Cout]) + _c(res_act[:, idx, Cout:])
+        v = v + torch.where(ra > 0, ra, ra / res_slope)
     if res_cl is not None:
-        v[:, :LoutE] += res_cl[:, :LoutE]
+        v = v + _c(res_cl[:, idx])
     if out_f32 is not None:
-        out_f32[:, :LoutE] = v[:, :LoutE]
-    else:
-        out_f32 = None
+        out_f32[:, idx] = v.to(out_f32.dtype)
     if out_act is not None:
         a = F.leaky_relu(v, slope) if act == 1 else v
         cs = act_cs if act_cs else Cout
         hi, lo = _split(a)
         q = Cout // cs
-        pair = torch.stack([hi.reshape(B, rows, q, cs), lo.reshape(B, rows, q, cs)], 3)      # [B, rows, q, 2, cs]
-        out_act[:, :LoutE] = pair.reshape(B, rows, 2 * Cout)[:, :LoutE]
+        pair = torch.stack([hi.reshape(B, LoutE, q, cs), lo.reshape(B, LoutE, q, cs)], 3)    # [B, Lout, q, 2, cs]
+        out_act[:, idx] = pair.reshape(B, LoutE, 2 * Cout).to(out_act.dtype)
     return out_f32, out_act
 
 
@@ -133,15 +171,29 @@ def dilated_unit_tc(xa_cl, w3t, w1t, dil, pad_l, slope_in, slope_mid, act_out, s
                     out_f32=None, out_act=None):
     """Semantics of rave_dilated_unit_tc_fwd: the two per-layer launches back to back, the intermediate rounded to the
     operand type exactly as the kernel rounds it before the second GEMM."""
+    L = xa_cl.shape[1] if L is None else L
+    a1 = unit_stage1(xa_cl, w3t, dil, pad_l, slope_mid, L)
+    unit_stage2(a1, xa_cl, w1t, slope_in, act_out, slope_out, L, out_f32, out_act)
+    return (a1 if want_a1 else None), out_f32, out_act
+
+
+def unit_stage1(xa_cl, w3t, dil, pad_l, slope_mid, L, out_act=None):
+    """a1 [B, pitch, C] = operand-type LeakyReLU(conv3(xa, dil)) over rows [0, L), zero slack rows."""
     B, pitch, C = xa_cl.shape
-    L = pitch if L is None else L
+    if out_act is None:
+        out_act = torch.zeros(B, pitch, C, dtype=OPERAND_DTYPE, device=_dev(xa_cl))
     _, a1 = conv1d_tc(xa_cl, w3t, None, None, 1, dil, (pad_l, 2 * dil - pad_l), 1, slope_mid, want_f32=False,
-                      want_act=True, out_rows=pitch, Lout=L, Lin=L)
+                      want_act=True, out_act=out_act, out_rows=pitch, Lout=L, Lin=L)
     if pitch > L:
         a1[:, L:] = 0
-    conv1d_tc(a1, w1t, None, None, 1, 1, (0, 0), act_out, slope_out, want_f32=False, want_act=False, out_f32=out_f32,
-              out_act=out_act, out_rows=pitch, Lout=L, Lin=L, res_act=xa_cl, res_slope=slope_in)
-    return (a1 if want_a1 else None), out_f32, out_act
+    return a1
+
+
+def unit_stage2(a1, xa_cl, w1t, slope_in, act_out, slope_out, L, out_f32=None, out_act=None):
+    """The unit's outputs from its intermediate a1: conv1x1(a1) + unleaky(xa) (the residual), rows [0, L)."""
+    return conv1d_tc(a1, w1t, None, None, 1, 1, (0, 0), act_out, slope_out, want_f32=False, want_act=False,
+                     out_f32=out_f32, out_act=out_act, out_rows=xa_cl.shape[1], Lout=L, Lin=L, res_act=xa_cl,
+                     res_slope=slope_in)
 
 
 def ncl_to_cl_x3(x):
@@ -155,15 +207,15 @@ def conv1d_tc_wgrad(P_cl, Q_cl, K, stride=1, dil=1, pad_l=0, Lp=None, Lq=None, d
     _, q_pitch, Cn = Q_cl.shape
     Lp = p_pitch if Lp is None else Lp
     Lq = q_pitch if Lq is None else Lq
-    P = P_cl[:, :Lp].float()
+    P = P_cl[:, :Lp].to(COMPUTE_DTYPE)
     if dbias is not None:
         dbias += P.sum((0, 1))
-    Q = Q_cl[:, :q_pitch].float()
+    Q = Q_cl[:, :q_pitch].to(COMPUTE_DTYPE)
     if q_pitch > Lq:
         assert float(Q[:, Lq:].abs().max()) == 0.0
     S = 2                                  # two "row slices": the batch halves
-    dwt = torch.zeros(S, K, Cm, Cn)
-    l = torch.arange(Lp)
+    dwt = _zeros(P, S, K, Cm, Cn)
+    l = torch.arange(Lp, device=P.device)
     half = (B + 1) // 2
     for k in range(K):
         r = l * stride + k * dil - pad_l
@@ -238,9 +290,9 @@ def conv1d_c1(x_rows, w, bias, Lin, stride, pad, act, slope, out_f32=None, out_a
 
 def conv1d_c1_wgrad(g_cl, x_rows, Cout, K, Lin, Lout, stride, pad_l):
     R = g_cl.shape[0]
-    g = g_cl[:, :Lout, :Cout].float()
-    dwt = torch.zeros(3, K, Cout, 1)                       # 3 "slices": rows split arbitrarily
-    l = torch.arange(Lout)
+    g = g_cl[:, :Lout, :Cout].to(COMPUTE_DTYPE)
+    dwt = _zeros(g, 3, K, Cout, 1)                         # 3 "slices": rows split arbitrarily
+    l = torch.arange(Lout, device=g.device)
     for k in range(K):
         pos = l * stride + k - pad_l
         ok = (pos >= 0) & (pos < Lin)
@@ -257,16 +309,16 @@ def conv1d_c1_dgrad(g_cl, w, x_pitch, Lin, Lout, stride, pad_l):
     R = g_cl.shape[0]
     Cout = w.shape[0]
     K = w.numel() // Cout
-    g = g_cl[:, :Lout, :Cout].float().permute(0, 2, 1)               # [R, Cout, Lout]
+    g = g_cl[:, :Lout, :Cout].to(COMPUTE_DTYPE).permute(0, 2, 1)               # [R, Cout, Lout]
     full = F.conv_transpose1d(g, w.reshape(Cout, 1, K), None, stride)  # [R, 1, (Lout-1)*s + K]
-    dx = torch.zeros(R, x_pitch)
+    dx = _zeros(g, R, x_pitch)
     seg = full[:, 0, pad_l:pad_l + Lin]
     dx[:, :seg.shape[1]] = seg
     return dx
 
 
 def colsum_bf16(g_cl, L, C):
-    return g_cl[:, :L, :C].float().sum((0, 1))
+    return g_cl[:, :L, :C].to(COMPUTE_DTYPE).sum((0, 1))
 
 
 def _c1_rows(src, Lin, period, pool):
@@ -282,10 +334,10 @@ def _c1_rows(src, Lin, period, pool):
 
 
 def im2col_c1(src, Lin, Lout, out_pitch, K, stride, pad_l, period=1, pool=1):
-    x_rows = _c1_rows(src.float(), Lin, period, pool)
+    x_rows = _c1_rows(src.to(COMPUTE_DTYPE), Lin, period, pool)
     R = x_rows.shape[0]
-    X = torch.zeros(R, out_pitch, 16)
-    l = torch.arange(Lout)
+    X = _zeros(x_rows, R, out_pitch, 16)
+    l = torch.arange(Lout, device=src.device)
     for k in range(K):
         pos = l * stride + k - pad_l
         ok = (pos >= 0) & (pos < Lin)
@@ -296,21 +348,38 @@ def im2col_c1(src, Lin, Lout, out_pitch, K, stride, pad_l, period=1, pool=1):
 def gather_c1(P_cl, src_shape, Lin, Lout, K, stride, pad_l, period=1, pool=1, batch0=0):
     if batch0:
         part = gather_c1(P_cl, (src_shape[0] - batch0, src_shape[1]), Lin, Lout, K, stride, pad_l, period, pool)
-        return torch.cat([torch.zeros(batch0, src_shape[1]), part], 0)
+        return torch.cat([_zeros(part, batch0, src_shape[1]), part], 0)
     R = P_cl.shape[0]
     Bs, T = src_shape
-    dx = torch.zeros(R, Lin)
-    t = torch.arange(Lin)
+    P = _c(P_cl)
+    dx = _zeros(P, R, Lin)
+    t = torch.arange(Lin, device=P.device)
     for k in range(K):
         q = t + pad_l - k
         ok = (q >= 0) & (q % stride == 0) & (q // stride < Lout)
-        dx[:, t[ok]] += P_cl[:, (q[ok] // stride), k]
+        dx[:, t[ok]] += P[:, (q[ok] // stride), k]
     # adjoint of _c1_rows
     with torch.enable_grad():
-        src = torch.zeros(Bs, T, requires_grad=True)
+        src = _zeros(P, Bs, T).requires_grad_(True)
         rows = _c1_rows(src, Lin, period, pool)
         (g,) = torch.autograd.grad(rows, src, dx)
     return g.detach()
+
+
+def im2col_cin(src, Lin, Lout, out_pitch, K, stride, pad_l, period=1, pool=1):
+    """im2col_c1 of each of the src [Bs, cin, T] channels side by side: X[r, l, c*K + k], zero up to W = 16 or 32."""
+    Bs, cin, T = src.shape
+    W = 16 if cin * K <= 16 else 32
+    X = torch.cat([im2col_c1(src[:, c], Lin, Lout, out_pitch, K, stride, pad_l, period, pool)[..., :K]
+                   for c in range(cin)], -1)
+    return F.pad(X, (0, W - cin * K))
+
+
+def gather_cin(P_cl, src_shape, Lin, Lout, K, stride, pad_l, period=1, pool=1, batch0=0):
+    """The adjoint of im2col_cin: dsrc [Bs, cin, T]."""
+    Bs, cin, T = src_shape
+    return torch.stack([gather_c1(P_cl[..., c * K:(c + 1) * K], (Bs, T), Lin, Lout, K, stride, pad_l, period, pool,
+                                  batch0) for c in range(cin)], 1)
 
 
 def _unleaky(a, slope):
@@ -319,7 +388,7 @@ def _unleaky(a, slope):
 
 def fm_stats(a_cl, stats_row, L, slope):
     B2 = a_cl.shape[0]
-    h = _unleaky(a_cl[:, :L].float(), slope)
+    h = _unleaky(a_cl[:, :L].to(COMPUTE_DTYPE), slope)
     hr, hf = h[:B2 // 2], h[B2 // 2:]
     stats_row[0] += (hr - hf).abs().sum()
     stats_row[1] += hr.abs().sum()
@@ -327,7 +396,7 @@ def fm_stats(a_cl, stats_row, L, slope):
 
 def fm_grad(a_cl, dstats_row, L, slope):
     B2 = a_cl.shape[0]
-    h = _unleaky(a_cl.float(), slope)
+    h = _unleaky(a_cl.to(COMPUTE_DTYPE), slope)
     hr, hf = h[:B2 // 2], h[B2 // 2:]
     sd = torch.sign(hr - hf)
     g = torch.cat([dstats_row[0] * sd + dstats_row[1] * torch.sign(hr), -dstats_row[0] * sd], 0)
@@ -337,7 +406,7 @@ def fm_grad(a_cl, dstats_row, L, slope):
 
 def score_stats(score_cl, stats6, L):
     B2 = score_cl.shape[0]
-    s = score_cl[:, :L, 0].float()
+    s = score_cl[:, :L, 0].to(COMPUTE_DTYPE)
     sr, sf = s[:B2 // 2], s[B2 // 2:]
     stats6.view(-1).add_(torch.stack([(sr - sf).abs().sum(), sr.abs().sum(), torch.relu(1 - sr).sum(),
                            torch.relu(1 + sf).sum(), sr.sum(), sf.sum()]))
@@ -345,13 +414,13 @@ def score_stats(score_cl, stats6, L):
 
 def score_grad(score_cl, dstats6, L):
     B2, pitch, C = score_cl.shape
-    s = score_cl[:, :L, 0].float()
+    s = score_cl[:, :L, 0].to(COMPUTE_DTYPE)
     sr, sf = s[:B2 // 2], s[B2 // 2:]
-    d = dstats6.float().reshape(-1)
+    d = dstats6.to(COMPUTE_DTYPE).reshape(-1)
     sd = torch.sign(sr - sf)
-    gr = d[0] * sd + d[1] * torch.sign(sr) - d[2] * (sr < 1).float() + d[4]
-    gf = -d[0] * sd + d[3] * (sf > -1).float() + d[5]
-    g = torch.zeros(B2, pitch, C, dtype=torch.float32)
+    gr = d[0] * sd + d[1] * torch.sign(sr) - d[2] * (sr < 1).to(COMPUTE_DTYPE) + d[4]
+    gf = -d[0] * sd + d[3] * (sf > -1).to(COMPUTE_DTYPE) + d[5]
+    g = torch.zeros(B2, pitch, C, dtype=torch.float32, device=score_cl.device)
     g[:B2 // 2, :L, 0] = gr
     g[B2 // 2:, :L, 0] = gf
     from rave_b200 import engine
@@ -375,7 +444,7 @@ def weight_prep_tc_multi(items, x3=False, into=None):
     try:
         for it in items:
             norm, A, Bm = weight_prep_tc(*it)
-            cat = lambda t: None if t is None else torch.cat(_split(t.float()), 0)
+            cat = lambda t: None if t is None else torch.cat(_split(t.to(COMPUTE_DTYPE)), 0)
             out.append((norm, cat(A), cat(Bm)))
     finally:
         globals()["OPERAND_DTYPE"] = saved
@@ -397,19 +466,19 @@ def weight_norm_bwd_multi(items):
 
 
 def snake_cl_fwd(h_cl, alpha):
-    al = alpha.detach().reshape(-1).float()
-    x = h_cl.float()
+    al = alpha.detach().reshape(-1).to(COMPUTE_DTYPE)
+    x = h_cl.to(COMPUTE_DTYPE)
     return _bf16(x + torch.sin(al * x) ** 2 / (al + 1e-9))
 
 
 def snake_cl_bwd(ga_cl, h_cl, alpha, add=None, want_dalpha=True):
-    al = alpha.detach().reshape(-1).float()
+    al = alpha.detach().reshape(-1).to(COMPUTE_DTYPE)
     ae = al + 1e-9
-    x, g = h_cl.float(), ga_cl.float()
+    x, g = h_cl.to(COMPUTE_DTYPE), ga_cl.to(COMPUTE_DTYPE)
     s2 = torch.sin(2 * al * x)
     gh = g * (1 + al * s2 / ae)
     if add is not None:
-        gh = gh + add.float()
+        gh = gh + add.to(COMPUTE_DTYPE)
     dal = (g * (x * s2 / ae - torch.sin(al * x) ** 2 / (ae * ae))).reshape(-1, x.shape[-1]).sum(0) if want_dalpha else None
     return _bf16(gh), dal
 
@@ -458,7 +527,8 @@ def stft_frames(x, window, n_fft, hop):
 def install(monkeypatch):
     from rave_b200 import ops
     for name in ("conv1d_tc", "conv1d_tc_wgrad", "weight_prep_tc", "weight_norm_bwd_tapmajor", "ncl_to_cl",
-                 "cl_to_ncl", "weight_norm_raw", "conv1d_c1", "conv1d_c1_wgrad", "fm_stats", "fm_grad", "conv1d_c1_dgrad", "colsum_bf16", "im2col_c1", "gather_c1", "weight_prep_tc_multi",
+                 "cl_to_ncl", "weight_norm_raw", "conv1d_c1", "conv1d_c1_wgrad", "fm_stats", "fm_grad", "conv1d_c1_dgrad", "colsum_bf16", "im2col_c1", "gather_c1", "im2col_cin", "gather_cin",
+                 "weight_prep_tc_multi",
                  "weight_norm_bwd_multi", "score_stats", "score_grad", "ncl_to_cl_x3", "dilated_unit_tc",
                  "dilated_unit_tc_supported", "snake_cl_fwd", "snake_cl_bwd", "activation", "leaky_fm", "time_stack_nhwc",
                  "leaky_fm_stack", "stft_frames"):
