@@ -279,6 +279,21 @@ int rave_leaky_fm_stack_dil_bwd(const float *a, const void *gxs_bf16, const floa
 int rave_snake_cl_fwd(const void *h_bf16, const float *alpha, void *a_bf16, long rows, int C, void *stream);
 int rave_snake_cl_bwd(const void *ga_bf16, const void *h_bf16, const float *alpha, const void *add_bf16, void *gh_bf16,
                       float *dalpha, long rows, int C, void *stream);
+/* AdaptiveInstanceNormalization (rave/blocks.py:863-926) in eval mode on a channel-last bf16 stream h [B][pitch][C]
+ * (csrc/adain.cu).  The statistics buffers are the module's own, fp32: mean_* / std_* [max_batch][C], learn_* and
+ * num_update_* [1]; every flag and counter is read on the device.
+ *   adain_cl_stats   : per (b, c), the mean and unbiased std of the L valid rows (fixed-order fp32 sums; NaN for L = 1);
+ *                      learn_y set -> mean_y / std_y += (stat - old) / (num_update_y + 1), num_update_y += 1 (learn_x
+ *                      ignored); else learn_x set -> the same on the x buffers.  Then scale / shift [B][C] of the
+ *                      transfer from the updated buffers: scale = std_y / (std_x + 1e-5), shift = mean_y - mean_x scale
+ *                      when learn_y is clear and both counters are non-zero, else exactly 1 / 0.  B <= max_batch.
+ *   adain_snake_cl_fwd: rows l < L: h = h scale + shift in place (the residual's skip stream), a = Snake(h) as the next
+ *                      conv's operand (rave_snake_cl_fwd's arithmetic); rows [L, pitch) of a are zeroed.  C % 8 == 0. */
+int rave_adain_cl_stats(const void *h_bf16, int B, int L, int pitch, int C, float *mean_x, float *std_x, float *mean_y,
+                        float *std_y, const float *learn_x, const float *learn_y, float *num_update_x,
+                        float *num_update_y, int max_batch, float *scale, float *shift, void *stream);
+int rave_adain_snake_cl_fwd(void *h_bf16, const float *alpha, const float *scale, const float *shift, void *a_bf16,
+                            int B, int L, int pitch, int C, void *stream);
 int rave_conv1d_tc_wgrad(const void *P_bf16, const void *Q_bf16, float *dwt, float *dbias, int B, int Cm, int Lp,
                          int p_pitch, int Cn, int Lq, int q_pitch, int K, int stride, int dil, int pad_l,
                          void *stream);

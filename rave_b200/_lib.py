@@ -73,6 +73,8 @@ SIGNATURES = {
     "rave_l1_grad_f32": (c_int, [_P, _P, _P, _P, _P, ctypes.c_long, _P]),
     "rave_snake_cl_fwd": (c_int, [_P, _P, _P, ctypes.c_long, _I, _P]),
     "rave_snake_cl_bwd": (c_int, [_P, _P, _P, _P, _P, _P, ctypes.c_long, _I, _P]),
+    "rave_adain_cl_stats": (c_int, [_P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P, _P, _P, _I, _P, _P, _P]),
+    "rave_adain_snake_cl_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "rave_weight_prep_tc": (c_int, [_P, _P, _P, _P, _P, _I, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "rave_weight_norm_bwd_tapmajor": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "rave_conv1d_c1_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _P]),

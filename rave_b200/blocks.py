@@ -92,8 +92,11 @@ def _default_activation(dim):
 
 
 class AdaptiveInstanceNormalization(nn.Module):
-    """Identity in training (rave/blocks.py:901-902); holds the reference's buffers so that v3
-    state_dicts load (the running statistics are only used by the export-time style transfer)."""
+    """Identity in training (rave/blocks.py:901-902).  In eval mode it learns the running mean / std of its input over
+    time as the target (`learn_y`) or source (`learn_x`) statistics, and once both were learned maps the stream from
+    source to target statistics: the style transfer, driven by `update_adain`.  `forward` is the reference's arithmetic
+    (the fp32 path); the v3 chains on the wgmma engine run it as two kernels per layer (engine.plan_sequential,
+    csrc/adain.cu) that read the same buffers and flags on the device."""
 
     def __init__(self, dim: int) -> None:
         super().__init__()
@@ -137,6 +140,30 @@ class AdaptiveInstanceNormalization(nn.Module):
         if self.num_update_x and self.num_update_y:
             x = self.transfer(x)
         return x
+
+
+def update_adain(root: nn.Module, learn_target: bool = False, learn_source: bool = False, reset_target: bool = False,
+                 reset_source: bool = False) -> int:
+    """Style-transfer controls of every AdaptiveInstanceNormalization under `root` (scripts/export.py:213-230,
+    `ScriptedRAVE.update_adain`): both learn flags are cleared, then set from `learn_target` (learn_y) and
+    `learn_source` (learn_x); then `reset_target` / `reset_source` restore the y / x statistics and counters.  Only
+    in-place device writes (no host sync, no host-to-device copy), so it may sit between the replays of a captured
+    CUDA graph.  Returns the number of AdaIN layers touched."""
+    n = 0
+    for m in root.modules():
+        if isinstance(m, AdaptiveInstanceNormalization):
+            m.learn_x.zero_()
+            m.learn_y.zero_()
+            if learn_target:
+                m.learn_y.add_(1)
+            if learn_source:
+                m.learn_x.add_(1)
+            if reset_target:
+                m.reset_y()
+            if reset_source:
+                m.reset_x()
+            n += 1
+    return n
 
 
 # ---------------------------------------------------------------------------------------------

@@ -217,6 +217,16 @@ class CachedSequential(nn.Sequential):
             cache[key] = specs
         return cache[key]
 
+    def _adain_ok(self, specs, x, x3: bool) -> bool:
+        """A plan with eval-mode AdaIN runs on the engine in the plain bf16 mode when no gradient is needed and the
+        batch fits the statistics buffers; otherwise the sequence runs module by module."""
+        ads = [s.adain for s in specs if s.adain is not None]
+        if not ads:
+            return True
+        if x3 or any(x.shape[0] > a.mean_x.shape[0] for a in ads):
+            return False
+        return not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())))
+
     def forward(self, x, res=None):
         from . import engine
         mode = engine.precision()
@@ -225,6 +235,8 @@ class CachedSequential(nn.Sequential):
             mode = "fp32"          # the split-operand mode is a forward path: gradients run on the fp32 kernels
         if res is None and mode in ("bf16", "bf16x3") and x.is_cuda and x.dim() == 3 and not self._cached:
             specs = self._tc_plan()
+            if specs is not None and not self._adain_ok(specs, x, x3):
+                specs = None
             if specs is not None and (specs[0].kind != "conv" or x.shape[-1] % specs[0].stride == 0):
                 lead = engine.split_recurrent(list(self))[0]
                 if lead is not None:

@@ -81,6 +81,8 @@ class LayerSpec:
                                    # residual stream: the skip is recovered from it (no fp32 copy of h_src)
     pre_mod: Optional[nn.Module] = None   # the Snake module (owner of alpha) when pre_act == ACT_SNAKE
     res_raw: Optional[int] = None  # Snake units: index of the layer whose raw (pre-Snake) bf16 input IS the skip stream
+    adain: Optional[nn.Module] = None     # eval-mode AdaptiveInstanceNormalization applied to this layer's raw input
+                                          # stream (before its Snake): the first conv of a Residual(DilatedUnit)
 
 
 def raw_input_ok(spec: LayerSpec, cin: int) -> bool:
@@ -118,6 +120,9 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
     Residual(DilatedUnit), AdaIN (identity in training).  Returns None if something is unsupported.
     Snake (v3): the producer writes its pre-activation as bf16, a channel-last Snake kernel turns it into the next conv's
     operand (and keeps the raw stream for the backward and for the unit's skip).
+    An eval-mode AdaIN in front of a Residual(DilatedUnit) of Snake units becomes `adain` of the unit's first conv: the
+    chain learns from / transfers the raw stream there (forward only, see TcChainFn).  In front of anything else (a
+    LeakyReLU unit) it is not run here.
     A leading GRU is not part of the plan (split_recurrent): the caller runs it first."""
     from . import blocks, cc
     mods = split_recurrent(list(mods))[1]
@@ -125,6 +130,7 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
     NONE = (ops.ACT_NONE, 0.0, None)
     pending = NONE
     last_idx = -1            # index of the layer producing the current stream (-1 = chain input)
+    adain = None             # eval-mode AdaIN waiting for the Residual(DilatedUnit) it feeds
 
     def act_of(m):
         if isinstance(m, nn.LeakyReLU):
@@ -152,9 +158,11 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
         return True
 
     for m in mods:
+        if adain is not None and not isinstance(m, blocks.Residual):
+            return None
         if isinstance(m, blocks.AdaptiveInstanceNormalization):
             if not m.training:
-                return None
+                adain = m
             continue
         a = act_of(m)
         if a is not None:
@@ -181,6 +189,10 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
             if not add_conv(c3):
                 return None
             c3_idx = last_idx
+            if adain is not None:
+                if acts[0][0] != ops.ACT_SNAKE:
+                    return None
+                specs[-1].adain, adain = adain, None
             pending = acts[1]
             if not add_conv(c1, res_src=src):
                 return None
@@ -190,7 +202,7 @@ def plan_sequential(mods: List[nn.Module]) -> Optional[List[LayerSpec]]:
                 specs[-1].res_raw = c3_idx        # Snake is not invertible: the raw bf16 input of conv3 is the skip
             continue
         return None
-    if pending[0] != ops.ACT_NONE or not specs:
+    if pending[0] != ops.ACT_NONE or adain is not None or not specs:
         return None
     if specs[0].pre_act != ops.ACT_NONE:
         # a chain's operands are activated by their PRODUCER's epilogue; the chain input has no producer, so a
@@ -682,6 +694,8 @@ class TcChainFn(torch.autograd.Function):
         n = len(specs)
         ctx.set_materialize_grads(False)
         need_dgrad = x_in.requires_grad or any(t is not None and t.requires_grad for t in flat)
+        if any(s.adain is not None for s in specs):
+            need_dgrad = False     # eval-mode AdaIN chains are forward only (run_chain refuses them under autograd)
         if x3:
             # split-operand mode: forward chains only (x_in rows are [hi | lo]); the caller keeps autograd away
             if fm or x_in.dim() == 2:
@@ -778,7 +792,15 @@ class TcChainFn(torch.autograd.Function):
             _zero_rows((out_f32, out_act), Lout, pitch)
             if snake_next:
                 hraw[j + 1] = out_act
-                out_act = ops.snake_cl_fwd(out_act, flat[alpha_idx[j + 1]])
+                ad = nxt.adain
+                if ad is None:
+                    out_act = ops.snake_cl_fwd(out_act, flat[alpha_idx[j + 1]])
+                else:
+                    # AdaIN on the raw stream: statistics / running update, then h <- h scale + shift in place (the
+                    # unit's skip reads hraw) and the Snake operand of the transformed stream
+                    scale, shift = ops.adain_cl_stats(out_act, Lout, ad.mean_x, ad.std_x, ad.mean_y, ad.std_y,
+                                                      ad.learn_x, ad.learn_y, ad.num_update_x, ad.num_update_y)
+                    out_act = ops.adain_snake_cl_fwd(out_act, flat[alpha_idx[j + 1]], scale, shift, Lout)
             if fm and nxt is not None:
                 if act_code != ops.ACT_LEAKY or s.cout_pad:
                     raise _lib.RaveB200Error("feature-matching mode needs LeakyReLU between the layers")
@@ -986,6 +1008,10 @@ def run_chain(x_cl_bf16: torch.Tensor, specs: List[LayerSpec], L0: Optional[int]
         v, g, b = _layer_params(s)
         flat += [v, g, b]
     flat += [s.pre_mod.alpha for s in specs if s.pre_act == ops.ACT_SNAKE]      # after the 3n weight entries
+    if any(s.adain is not None for s in specs) and torch.is_grad_enabled() and (
+            x_cl_bf16.requires_grad or any(t is not None and t.requires_grad for t in flat)):
+        raise _lib.RaveB200Error("a chain with eval-mode AdaIN runs without autograd only (no backward through the "
+                                 "style statistics)")
     if L0 is None:
         L0 = x_cl_bf16.shape[1]
     return TcChainFn.apply(x_cl_bf16, specs, L0, fm, src, fake_grad_only or _FAKE_ROWS_ONLY, x3, *flat)

@@ -237,6 +237,14 @@ class RAVE(nn.Module):
         z = self.encoder.reparametrize(z)[0]
         return self.decode(z)
 
+    def update_adain(self, learn_target: bool = False, learn_source: bool = False, reset_target: bool = False,
+                     reset_source: bool = False) -> int:
+        """Style transfer of a model with AdaIN layers (v3): learn the target statistics over target audio
+        (`learn_target=True`), then the source statistics (`learn_source=True`; the transfer already applies in those
+        calls), then `update_adain()` to transfer with the statistics frozen; `reset_*` forget them.  Eval mode only
+        (AdaIN is the identity in training).  Returns the number of AdaIN layers (0 without any): blocks.update_adain."""
+        return blocks.update_adain(self, learn_target, learn_source, reset_target, reset_source)
+
     def on_train_batch_end(self, outputs=None, batch=None, batch_idx=None) -> None:
         self.lr_schedulers().step()
 

@@ -777,6 +777,43 @@ def snake_cl_bwd(ga_cl, h_cl, alpha, add=None, want_dalpha=True):
     return gh, dal
 
 
+def _adain_buffer(t, C, rows=None):
+    if t.dtype != torch.float32 or not t.is_contiguous() or t.shape[1:] != ((C, 1) if rows is None else ()) \
+            or (rows is not None and t.numel() != rows):
+        raise _lib.RaveB200Error(f"adain: statistics buffer of shape {tuple(t.shape)} / {t.dtype} does not fit C = {C}")
+    return t
+
+
+def adain_cl_stats(h_cl, L, mean_x, std_x, mean_y, std_y, learn_x, learn_y, num_update_x, num_update_y):
+    """AdaptiveInstanceNormalization's eval-mode statistics on an engine stream h_cl [B, pitch, C] bf16 (first L rows
+    valid), written into the module's own buffers (mean_* / std_* [N, C, 1], learn_* / num_update_* [1], fp32; B <= N):
+    the learn_y / learn_x running update and counter step, all decided on the device.  Returns (scale, shift) [B, C]
+    fp32 of the transfer (exactly 1 / 0 where it does not apply).  Forward only: the buffers are not autograd inputs."""
+    B, pitch, C = h_cl.shape
+    stats = [_adain_buffer(t, C) for t in (mean_x, std_x, mean_y, std_y)]
+    flags = [_adain_buffer(t, C, rows=1) for t in (learn_x, learn_y, num_update_x, num_update_y)]
+    if h_cl.dtype != torch.bfloat16 or not (0 < L <= pitch):
+        raise _lib.RaveB200Error("adain_cl_stats: h must be a bf16 [B, pitch, C] stream with 0 < L <= pitch")
+    scale = torch.empty(B, C, dtype=torch.float32, device=h_cl.device)
+    shift = torch.empty_like(scale)
+    call("rave_adain_cl_stats", ptr(h_cl), B, int(L), pitch, C, *(ptr(t) for t in stats), *(ptr(t) for t in flags),
+         mean_x.shape[0], ptr(scale), ptr(shift), stream_ptr())
+    return scale, shift
+
+
+def adain_snake_cl_fwd(h_cl, alpha, scale, shift, L):
+    """h_cl [B, pitch, C] bf16 <- h scale + shift on rows < L (in place: the residual's skip stream); returns the Snake
+    operand a = Snake(h) [B, pitch, C] with zero rows [L, pitch)."""
+    B, pitch, C = h_cl.shape
+    if h_cl.dtype != torch.bfloat16 or scale.shape != (B, C) or shift.shape != (B, C) or not (0 < L <= pitch):
+        raise _lib.RaveB200Error("adain_snake_cl_fwd: h [B, pitch, C] bf16, scale / shift [B, C], 0 < L <= pitch")
+    a = torch.empty_like(h_cl)
+    al = _f32c(alpha.detach().reshape(-1))
+    call("rave_adain_snake_cl_fwd", ptr(h_cl), ptr(al), ptr(_f32c(scale)), ptr(_f32c(shift)), ptr(a), B, int(L), pitch,
+         C, stream_ptr())
+    return a
+
+
 def dilated_unit_tc_supported(C, L):
     return bool(_lib.load().rave_dilated_unit_tc_supported(C, L))
 
