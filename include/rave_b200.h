@@ -538,6 +538,19 @@ int rave_prior_sample(const float *const *params, int n_layers, int cycle_size, 
 int rave_prior_classes_to_latent(const int *classes, const float *dither, const float *noise, const float *latent_pca,
                                  const float *latent_mean, float *z, int B, int T, int D, int L, int R, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Training-batch transforms (get_dataset's transform list, rave/dataset.py:207-262), per example b of raw [B][C][L]
+ * (int16 when raw_int16, else float32; C channels share every draw) -> out [B][C][N] float32:
+ *   decode float32(int16) / 32767; crop [off, off + N); when apply, the allpass lfilter(b, a) of
+ *   pole_to_z_filter(omega, .99) from zero state, in float64; + U[0, 1) / 2^16; with normalize, normalize_signal over
+ *   the example; with derivative, lfilter([.5, -.5], [1]); times keep; float32.
+ *   draws [B][4] float64 = (off, apply, omega, keep), off clamped to [0, L - N]; key [2] int64 = (Philox seed,
+ *   counter offset) of the dequantisation uniforms, keyed by (b, c, n); noise [B][C][N] float64 replaces them (or
+ *   NULL).  One launch, two with normalize; graph-capturable (stream-ordered workspace, no host synchronisation).
+ * ------------------------------------------------------------------------------------------- */
+int rave_augment(const void *raw, int raw_int16, int B, int C, int L, int N, const double *draws, const long long *key,
+                 const double *noise, float *out, int normalize, int derivative, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -122,6 +122,7 @@ SIGNATURES = {
     "rave_prior_sample_workspace_bytes": (c_long, [_I, _I, _I, _I, _I, _I, _I]),
     "rave_prior_sample": (c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _I, _I, _I, _P, _P, _P, _L, _P]),
     "rave_prior_classes_to_latent": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "rave_augment": (c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
 }
 
 

@@ -1538,3 +1538,16 @@ def prior_classes_to_latent(classes, dither, noise, latent_pca, latent_mean, R):
          ptr(None if noise is None or L == D else _f32c(noise)), ptr(_f32c(latent_pca)), ptr(_f32c(latent_mean)),
          ptr(z), B, T, D, L, R, stream_ptr())
     return z
+
+
+# ----------------------------------------------------------------------------------------------
+# Training-batch transforms (rave_b200/transforms.py)
+# ----------------------------------------------------------------------------------------------
+
+def augment(raw, draws, key, out, noise=None, normalize=False, derivative=False):
+    """raw [B, C, L] int16 / fp32 -> out [B, C, N] fp32 with rave_augment (include/rave_b200.h): draws [B, 4] fp64,
+    key [2] int64, noise [B, C, N] fp64 or None.  Shapes and dtypes are the caller's to check."""
+    B, C, L = raw.shape
+    call("rave_augment", ptr(raw), int(raw.dtype == torch.int16), B, C, L, out.shape[-1], ptr(draws), ptr(key),
+         ptr(noise), ptr(out), int(normalize), int(derivative), stream_ptr())
+    return out
