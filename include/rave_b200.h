@@ -551,6 +551,20 @@ int rave_prior_classes_to_latent(const int *classes, const float *dither, const 
 int rave_augment(const void *raw, int raw_int16, int B, int C, int L, int N, const double *draws, const long long *key,
                  const double *noise, float *out, int normalize, int derivative, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Exponential moving average of parameters (the reference's EMA callback, scripts/train.py:81-119), multi-tensor.
+ *   table [4T + 1] int64 = [ p[T] | ema[T] | numel[T] | chunk0[T + 1] ]: float32 pointers, element counts and the
+ *   prefix sum of each tensor's chunk count, ceil(numel / rave_ema_chunk_elems()); n_chunks = chunk0[T].
+ *   update: ema = rn(rn(ema * factor) + rn(p * one_minus_factor)) element by element (no FMA: torch's float32
+ *   `w * factor + p * (1 - factor)` bit for bit), or ema = p for a tensor t whose state[t] is 0; the launch then sets
+ *   state[0 .. T) to 1.  state [T + 1] int32 = [ initialised flags | completion ticket, 0 between launches ].
+ *   swap: exchange p and ema in place.  One launch each, graph-capturable.
+ * ------------------------------------------------------------------------------------------- */
+long long rave_ema_chunk_elems(void);
+int rave_ema_update(const long long *table, int n_tensors, long long n_chunks, int *state, float factor,
+                    float one_minus_factor, void *stream);
+int rave_ema_swap(const long long *table, int n_tensors, long long n_chunks, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,7 +6,7 @@ computation of the hot path goes through one of these entry points.  There is NO
 """
 import ctypes
 import os
-from ctypes import c_float, c_int, c_long, c_size_t, c_ulonglong, c_void_p, c_char_p
+from ctypes import c_float, c_int, c_long, c_longlong, c_size_t, c_ulonglong, c_void_p, c_char_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "csrc", "librave_b200.so")
@@ -123,6 +123,9 @@ SIGNATURES = {
     "rave_prior_sample": (c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _I, _I, _I, _P, _P, _P, _L, _P]),
     "rave_prior_classes_to_latent": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_augment": (c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
+    "rave_ema_chunk_elems": (c_longlong, []),
+    "rave_ema_update": (c_int, [_P, _I, c_longlong, _P, _F, _F, _P]),
+    "rave_ema_swap": (c_int, [_P, _I, c_longlong, _P]),
 }
 
 

@@ -11,9 +11,12 @@ addresses at capture).  Host-side scalars that a schedule may move are read from
 weights (`model.weights`) and the valid-signal crop (`model.receptive_field`) are constants of the captured graph --
 changing them needs a new GraphedTrainer.
 
+With `ema=` (an `ema.EMA`), the averages' update launch ends the G-step graph and the D-step graph, after the optimiser
+step: one library launch more per replay.  The flat buffer of averages and its flags are allocated before capture.
+
 The eager warm-up the capture needs (lazy state, cuFFT plans, kernel attributes) performs real optimiser
 updates; parameters, buffers and optimiser state are snapshotted before it and restored afterwards, so
-constructing a GraphedTrainer does not move the model.
+constructing a GraphedTrainer does not move the model (nor the averages of an `ema`).
 """
 import copy
 from typing import Dict, Optional
@@ -39,7 +42,7 @@ def _refresh_static_after_load(m, keys):
 
 
 class GraphedTrainer:
-    def __init__(self, model, example_batch: torch.Tensor, grad_hook=None, warmup_steps: int = 3):
+    def __init__(self, model, example_batch: torch.Tensor, grad_hook=None, warmup_steps: int = 3, ema=None):
         if not example_batch.is_cuda:
             raise RuntimeError("GraphedTrainer needs a CUDA batch")
         self.model = model
@@ -68,7 +71,13 @@ class GraphedTrainer:
                 model._static_enc_prep = True
             if not getattr(model, "_static_prep_hook", None):
                 model._static_prep_hook = model.register_load_state_dict_post_hook(_refresh_static_after_load)
-        snap_tensors = [(t, t.detach().clone()) for t in list(model.parameters()) + list(model.buffers())]
+        self.ema = ema
+        ema_tensors = []
+        if ema is not None:
+            ema._bind(model)
+            ema._graphed = True
+            ema_tensors = [ema.flat, ema._state]
+        snap_tensors = [(t, t.detach().clone()) for t in list(model.parameters()) + list(model.buffers()) + ema_tensors]
         snap_opt = [(o, copy.deepcopy(o.state_dict())) for o in (gen_opt, dis_opt)]
         self.graphs: Dict[bool, torch.cuda.CUDAGraph] = {}
         self.outputs: Dict[bool, Dict[str, torch.Tensor]] = {}
@@ -81,6 +90,8 @@ class GraphedTrainer:
             for i in range(warmup_steps):
                 for is_dis in kinds:
                     model.train_body(self.x_static, is_dis, None, grad_hook)
+                    if ema is not None:
+                        ema._launch_update()
         torch.cuda.current_stream().wait_stream(side)
         torch.cuda.synchronize()
         pool = None
@@ -91,6 +102,8 @@ class GraphedTrainer:
             with torch.cuda.graph(g, pool=pool, capture_error_mode="thread_local"):
                 logs = model.train_body(self.x_static, is_dis, None, grad_hook)
                 out = {k: (v.clone() if torch.is_tensor(v) else v) for k, v in logs.items()}
+                if ema is not None:
+                    ema._launch_update()
             pool = g.pool()
             self.launches[is_dis] = _lib.launch_count() - n0
             self.graphs[is_dis] = g

@@ -1551,3 +1551,24 @@ def augment(raw, draws, key, out, noise=None, normalize=False, derivative=False)
     call("rave_augment", ptr(raw), int(raw.dtype == torch.int16), B, C, L, out.shape[-1], ptr(draws), ptr(key),
          ptr(noise), ptr(out), int(normalize), int(derivative), stream_ptr())
     return out
+
+
+# ----------------------------------------------------------------------------------------------
+# Exponential moving average of parameters (rave_b200/ema.py)
+# ----------------------------------------------------------------------------------------------
+
+def ema_chunk_elems() -> int:
+    """Elements per chunk of the EMA table's chunk prefix (include/rave_b200.h)."""
+    return int(_lib.load().rave_ema_chunk_elems())
+
+
+def ema_update(table, n_tensors, n_chunks, state, factor):
+    """rave_ema_update over the tensors of `table` [4T + 1] int64: ema = ema * factor + p * (1 - factor) in float32,
+    1 - factor in double as Python computes it; a tensor whose state flag is 0 is copied instead."""
+    call("rave_ema_update", ptr(table), int(n_tensors), int(n_chunks), ptr(state), float(factor), 1.0 - float(factor),
+         stream_ptr())
+
+
+def ema_swap(table, n_tensors, n_chunks):
+    """rave_ema_swap: exchange the parameters and the averages of `table` in place."""
+    call("rave_ema_swap", ptr(table), int(n_tensors), int(n_chunks), stream_ptr())
