@@ -226,8 +226,11 @@ int rave_conv1d_tc_fwd_x3(const void *xa_bf16, const void *wt_bf16, const float 
  * the slices are summed, in order, by rave_weight_norm_bwd_tapmajor / rave_tapmajor_to_weight_f32).
  * For ConvTranspose1d swap the roles (P = activated input, Q = dy).  Cm, Cn multiples of 8.
  * dbias [Cm] fp32, pre-zeroed, or NULL: += sum_{b,l} P[b][l][m] (the conv bias gradient when P = dy), reduced by the
- * tap-0 CTAs from the tiles they stream anyway (fp32 atomics across row slices). */
+ * tap-0 CTAs from the tiles they stream anyway (one partial per row slice, added in slice order). */
 int rave_conv1d_tc_wgrad_splits(int B, int Cm, int Lp, int Cn, int K);
+/* tile of that launch: BLOCK_N | BLOCK_M << 8 | ring stages << 16; it runs K * splits * ceil(Cm / BLOCK_M) *
+ * ceil(Cn / BLOCK_N) CTAs of one tile each (scripts/profile_layers.py labels the wgrad launches with it) */
+int rave_conv1d_tc_wgrad_plan(int B, int Cm, int Lp, int Cn, int K);
 /* Operand of a (kt, kf) Conv2d evaluated as a conv along frequency (Descript MRD, rave/descript_discriminator.py:118-184):
  * x [B][C][T][F] fp32 -> out [(b,t)][Fp][Cp] bf16 with out[.][f][dt*C + c] = x[b][c][t + dt - pt][f] (zero elsewhere), and
  * the adjoint gx [B][C][T][F] += (written once) from g [(b,t)][Fp][Cp]. */

@@ -57,6 +57,7 @@ SIGNATURES = {
     "rave_conv1d_tc_wgrad": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_tapmajor_to_weight_f32": (c_int, [_P, _P, _I, _I, _I, _I, _I, _P]),
     "rave_conv1d_tc_wgrad_splits": (c_int, [_I, _I, _I, _I, _I]),
+    "rave_conv1d_tc_wgrad_plan": (c_int, [_I, _I, _I, _I, _I]),
     "rave_time_stack_cl": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_time_stack_cl_bwd": (c_int, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "rave_time_stack_nhwc": (c_int, [_P, _P, _I, _I, _I, _I, ctypes.c_long, ctypes.c_long, _I, _I, _I, _I, _P]),

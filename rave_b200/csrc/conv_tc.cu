@@ -1187,9 +1187,13 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmap_p, const __grid_constan
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
-  // tile / slice owned by this CTA
-  const int split = blockIdx.x % p.splits;
-  int t = blockIdx.x / p.splits;
+  // tile / slice owned by this CTA.  The slice is the slowest index: the CTAs of one slice stream the same P and Q rows
+  // (every tap, m-tile and n-tile of those rows) and run side by side, so each row comes from HBM about once and the
+  // other tiles find it in L2.  With the slice fastest, a slice's tiles fell into different waves and every wave
+  // re-read the rows.
+  const int tiles = p.K * p.n_mt * p.n_nt;
+  const int split = blockIdx.x / tiles;
+  int t = blockIdx.x % tiles;
   const int nt = t % p.n_nt; t /= p.n_nt;
   const int mt = t % p.n_mt; t /= p.n_mt;
   const int k = t;
@@ -1382,6 +1386,16 @@ extern "C" int rave_conv1d_tc_wgrad_splits(int B, int Cm, int Lp, int Cn, int K)
   int BL, n_lt, n_bg, n_mt, BN, n_nt, splits;
   rave::tc::wg_geometry(B, Cm, Lp, Cn, K, &BL, &n_lt, &n_bg, &n_mt, &BN, &n_nt, &splits);
   return splits;
+}
+
+// Tile rave_conv1d_tc_wgrad runs for a shape: BLOCK_N | BLOCK_M << 8 | ring stages << 16; the launch has
+// K * splits * ceil(Cm / BLOCK_M) * ceil(Cn / BLOCK_N) CTAs (one tile each).
+extern "C" int rave_conv1d_tc_wgrad_plan(int B, int Cm, int Lp, int Cn, int K) {
+  using namespace rave::tc;
+  int BL, n_lt, n_bg, n_mt, BN, n_nt, splits;
+  wg_geometry(B, Cm, Lp, Cn, K, &BL, &n_lt, &n_bg, &n_mt, &BN, &n_nt, &splits);
+  const int stages = BN == 64 ? WgSmem<64>::STAGES : WgSmem<128>::STAGES;
+  return BN | 128 << 8 | stages << 16;
 }
 
 extern "C" int rave_conv1d_tc_wgrad(const void *P, const void *Q, float *dwt, float *dbias, int B, int Cm, int Lp,

@@ -96,7 +96,8 @@ def wgrad_runner(torch, ops, ints, ptrs):
 
 
 def instance(lib, name, ints, ptrs):
-    """Kernel of a launch; conv launches the ping-pong kernel takes are marked ` pp` and its ring stages."""
+    """Kernel of a launch; conv launches the ping-pong kernel takes are marked ` pp` and its ring stages, weight-gradient
+    launches carry their tile (rows of Cm x columns of Cn), split-K slices, CTAs and waves of 132 SMs."""
     if name == "rave_conv1d_tc_fwd":
         B, Cin, Cout, Lout, K, act = ints[0], ints[1], ints[4], ints[5], ints[6], ints[10]
         v = lib.rave_conv1d_tc_plan(B, Cin, Cout, Lout, K)
@@ -110,8 +111,12 @@ def instance(lib, name, ints, ptrs):
         return f"conv<{v & 0xfff},{(v >> 12) & 0xfff}>" + (f" pp{stages}" if stages else "")
     if name == "rave_conv1d_tc_wgrad":
         Bc, Cm, Lp, pp, Cn = ints[:5]
-        s = lib.rave_conv1d_tc_wgrad_splits(Bc, Cm, Lp, Cn, ints[7])
-        return f"wgrad<{64 if Cn <= 64 else 128}> x{s}"
+        K = ints[7]
+        s = lib.rave_conv1d_tc_wgrad_splits(Bc, Cm, Lp, Cn, K)
+        v = lib.rave_conv1d_tc_wgrad_plan(Bc, Cm, Lp, Cn, K)
+        bn, bm = v & 0xff, (v >> 8) & 0xff
+        items = K * s * math.ceil(Cm / bm) * math.ceil(Cn / bn)
+        return f"wgrad<{bn}> {bm}x{bn} x{s} {items}/{math.ceil(items / 132)}w"
     return name
 
 
