@@ -203,6 +203,10 @@ int rave_conv1d_tc_pp_stages(int B, int Cin, int Cout, int Lout, int K, int fm, 
 /* ring stages of the ping-pong kernel for a forward launch of this shape (bias and / or LeakyReLU, bf16 output only:
  * no res, res_bf16, res_act, dact_src or out_f32); 0 = the launch runs the single-warpgroup kernel */
 int rave_conv1d_tc_pp_fwd_stages(int B, int Cin, int Cout, int Lout, int K);
+/* ring stages of the wide kernel (128 x 192 tiles, two MMA warpgroups per tile) for a forward launch of this shape
+ * (the operand set of rave_conv1d_tc_pp_fwd_stages, Cout a multiple of 192, many k-blocks per tile); 0 = the launch
+ * does not run it.  Where it is > 0 it takes precedence over the two queries above. */
+int rave_conv1d_tc_wide_stages(int B, int Cin, int Cout, int Lout, int K);
 int rave_conv1d_tc_fwd(const void *xa_bf16, const void *wt_bf16, const float *bias, const float *res,
                        const void *res_bf16, const void *dact_src_bf16, const void *res_act_bf16, float res_slope,
                        float *out_f32, void *out_act_bf16,

@@ -48,6 +48,7 @@ SIGNATURES = {
     "rave_conv1d_tc_plan": (c_int, [_I, _I, _I, _I, _I]),
     "rave_conv1d_tc_pp_stages": (c_int, [_I, _I, _I, _I, _I, _I, _I]),
     "rave_conv1d_tc_pp_fwd_stages": (c_int, [_I, _I, _I, _I, _I]),
+    "rave_conv1d_tc_wide_stages": (c_int, [_I, _I, _I, _I, _I]),
     "rave_conv1d_tc_fwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _F, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I,
                                    _F, _I, _I, _I, _P, _I, _P]),
     "rave_conv1d_tc_fwd_x3": (c_int, [_P, _P, _P, _P, _P, _F, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _F, _I,

@@ -15,7 +15,9 @@
 // epilogue thread writes out with TMA tensor stores.
 // Warp roles: 0-3 = MMA warpgroup, 4 = TMA producer, 5-8 = epilogue.  The input-gradient launches (LeakyReLU' mask,
 // bf16 out only) and the forward launches with bias / LeakyReLU and a bf16 output only run the ping-pong kernel instead
-// (conv_tc_pp_kernel, conv_tc_pp_fwd_kernel): two MMA warpgroups on alternate tiles, epilogue from registers.
+// (conv_tc_pp_kernel, conv_tc_pp_fwd_kernel): two MMA warpgroups on alternate tiles, epilogue from registers.  The
+// long-k forward launches of that operand set with Cout % 192 == 0 run conv_tc_wide_kernel: two MMA warpgroups on the
+// two m64 halves of one 128 x 192 tile.
 //
 // Replaces: cc.Conv1d.forward = F.pad + F.conv1d -> cuDNN (reference call sites rave/blocks.py:96-108,
 // 538-592, 637-692; rave/discriminator.py:99-111), the preceding activation module and the residual add.
@@ -340,9 +342,10 @@ __device__ __forceinline__ void produce_kblock(uint8_t *smem, Ring &r, const CUt
 }
 
 // The wgmma of k-block kb of a tile from the ring slot at shared address sa, as one committed group: BLOCK_K / 16 steps
-// of the two m64 halves (x3: plus lo*hi and hi*lo).  The first step of a tile overwrites the accumulators.
-template <int BLOCK_N, int BLOCK_K, bool X3>
-__device__ __forceinline__ void mma_kblock(float (*d)[BLOCK_N / 2], uint32_t sa, int kb) {
+// of the two m64 halves (x3: plus lo*hi and hi*lo).  The first step of a tile overwrites the accumulators.  NH = 1: the
+// warpgroup issues half h0 alone into d[0] (conv_tc_wide_kernel: the other half is the other warpgroup's).
+template <int BLOCK_N, int BLOCK_K, bool X3, int NH = 2>
+__device__ __forceinline__ void mma_kblock(float (*d)[BLOCK_N / 2], uint32_t sa, int kb, int h0 = 0) {
   using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
   constexpr int SWZ = BLOCK_K * 2;
   // rows 64 h .. 64 h + 63 of an operand tile start 64 swizzle spans further: + (64 * SWZ) >> 4 in the address field
@@ -354,8 +357,8 @@ __device__ __forceinline__ void mma_kblock(float (*d)[BLOCK_N / 2], uint32_t sa,
   for (int kk = 0; kk < BLOCK_K / 16; ++kk) {
     // advance 16 bf16 = 32 bytes inside the swizzle span: +2 in the (addr >> 4) field
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
-      Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + h * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
+    for (int h = 0; h < NH; ++h)
+      Wgmma<BLOCK_N, 0, 0>::mma(d[h], adesc + (h0 + h) * A_HALF + 2 * kk, bdesc + 2 * kk, (kb > 0 || kk > 0) ? 1u : 0u);
   }
   if (X3) {        // a*w ~ a_hi*w_hi + a_lo*w_hi + a_hi*w_lo (the lo*lo term is below fp32 accumulation noise)
     const uint64_t adesc_lo = make_kmajor_desc(sa + L::A_PART, SWZ);
@@ -375,15 +378,15 @@ __device__ __forceinline__ void mma_kblock(float (*d)[BLOCK_N / 2], uint32_t sa,
 // Main loop of one tile (MMA warpgroup): its kblocks k-blocks from the ring.  One wgmma group stays in flight: k-block kb
 // is issued before the group of kb - 1 is waited for, so the tensor pipe does not drain between k-blocks; a slot is
 // released (one arrival per warp) once the group that reads it has completed.  Returns the slot of the last group, which
-// is still in flight (mma_drain).
-template <int BLOCK_N, int BLOCK_K, bool X3>
+// is still in flight (mma_drain).  NH, h0: the m64 halves the warpgroup issues (mma_kblock).
+template <int BLOCK_N, int BLOCK_K, bool X3, int NH = 2>
 __device__ __forceinline__ int mma_mainloop(float (*d)[BLOCK_N / 2], uint32_t smem_base, Ring &r, int kblocks,
-                                            int lane) {
+                                            int lane, int h0 = 0) {
   using L = SmemLayout<BLOCK_N, BLOCK_K, X3>;
   int prev = 0;
   for (int kb = 0; kb < kblocks; ++kb) {
     mbar_wait(&r.full[r.stage], r.phase);
-    mma_kblock<BLOCK_N, BLOCK_K, X3>(d, smem_base + r.stage * L::STAGE_BYTES, kb);
+    mma_kblock<BLOCK_N, BLOCK_K, X3, NH>(d, smem_base + r.stage * L::STAGE_BYTES, kb, h0);
     wgmma_wait<1>();                                         // the group of k-block kb - 1 has completed
     if (kb > 0) {
       __syncwarp();
@@ -396,11 +399,11 @@ __device__ __forceinline__ int mma_mainloop(float (*d)[BLOCK_N / 2], uint32_t sm
 }
 
 // End of a tile's main loop: wait for its last wgmma group, then release that group's slot
-template <int BLOCK_N>
+template <int BLOCK_N, int NH = 2>
 __device__ __forceinline__ void mma_drain(float (*d)[BLOCK_N / 2], const Ring &r, int prev, int lane) {
   wgmma_wait<0>();
-  wgmma_fence_regs<BLOCK_N / 2>(d[0]);
-  wgmma_fence_regs<BLOCK_N / 2>(d[1]);
+#pragma unroll
+  for (int h = 0; h < NH; ++h) wgmma_fence_regs<BLOCK_N / 2>(d[h]);
   __syncwarp();
   if (lane == 0) mbar_arrive(&r.empty[prev]);
 }
@@ -575,10 +578,11 @@ __device__ __forceinline__ void pp_epilogue(float (*d)[BLOCK_N / 2], uint8_t *sl
 
 // Forward epilogue of one tile from the accumulator registers into the output slot (the boxes and fragment mapping of
 // pp_epilogue).  Per element the fp32 sequence of tc_epi_chunk: + bias[co], max(v, slope v) for LeakyReLU, one rounding
-// to bf16.  Column pair j outermost: one bias load per pair serves the thread's four rows.
-template <int BLOCK_N, int BOXC, bool BIAS, bool LEAKY>
+// to bf16.  Column pair j outermost: one bias load per pair serves the thread's four rows.  NH, h0: the m64 halves the
+// warpgroup holds (mma_kblock); with NH = 1 a thread has two rows.
+template <int BLOCK_N, int BOXC, bool BIAS, bool LEAKY, int NH = 2>
 __device__ __forceinline__ void pp_fwd_epilogue(float (*d)[BLOCK_N / 2], uint8_t *slot, const TcParams &p, int w,
-                                                int lane, int n0) {
+                                                int lane, int n0, int h0 = 0) {
   constexpr int SPAN = BOXC * 2, JB = BOXC / 8;
   const uint32_t base = stg_offset<BOXC>(16 * w + (lane >> 2), 0) + 4 * (lane & 3);
   const uint32_t sslot = smem_u32(slot);
@@ -588,7 +592,7 @@ __device__ __forceinline__ void pp_fwd_epilogue(float (*d)[BLOCK_N / 2], uint8_t
     const float2 bb = BIAS ? __ldg(bias + 4 * j) : make_float2(0.f, 0.f);
     const uint32_t col = (base ^ (uint32_t)((j % JB) << 4)) + (j / JB) * (BLOCK_M * SPAN);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int h = 0; h < NH; ++h) {
 #pragma unroll
       for (int r = 0; r < 2; ++r) {
         float v0 = d[h][4 * j + 2 * r], v1 = d[h][4 * j + 2 * r + 1];
@@ -603,7 +607,7 @@ __device__ __forceinline__ void pp_fwd_epilogue(float (*d)[BLOCK_N / 2], uint8_t
         __nv_bfloat162 o = __floats2bfloat162_rn(v0, v1);
         // volatile: each store stays next to its arithmetic (with plain stores ptxas ran all of a tile's arithmetic
         // ahead of the stores and spilled tile-loop invariants at BLOCK_N = 128)
-        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sslot + col + (64 * h + 8 * r) * SPAN),
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(sslot + col + (64 * (h0 + h) + 8 * r) * SPAN),
                      "r"(*reinterpret_cast<uint32_t *>(&o))
                      : "memory");
       }
@@ -770,6 +774,107 @@ conv_tc_pp_fwd_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
       &tmap_a, &tmap_b, nullptr, nullptr, nullptr, &tmap_o, p);
 }
 
+// =============================================================================================
+// Wide forward kernel.  The long-k forward launches of the PP_FWD operand set whose Cout is a multiple of 192 (the
+// discriminators' layers 2-4) run 128 x 192 tiles: warpgroups 1 and 2 both work on every tile, warpgroup 1 on rows
+// 0-63 and warpgroup 2 on rows 64-127, each issuing m64n192k16 from the same ring stage.  An activation tile is then
+// loaded once per 192 output channels instead of once per 96 or 128, and each stage's weight tile feeds two m64 blocks
+// per k16 step as in conv_tc_kernel, so shared memory serves fewer operand bytes per MMA.  Each output element gets
+// conv_tc_kernel's k16 steps in the same order; the epilogue is pp_fwd_epilogue's, so the bf16 output is the same.
+// Warp roles as in conv_tc_pp_body: warpgroup 0 = TMA producer (warp 0), warpgroups 1 and 2 = MMA + epilogue.  The ring
+// (produce_kblock, mma_mainloop) is shared: a stage is free once all 8 MMA warps have released it.  Both warpgroups
+// write their rows into one bf16 output slot (128 x 192, 48 KB); after a named barrier one thread stores it by TMA.
+// Before the next tile's epilogue that thread waits until the stores have read the slot and arms oempty, which both
+// warpgroups wait on before they write the slot again.  The epilogue does not overlap the MMAs of the CTA, so the
+// kernel only takes launches with many k-blocks per tile (wide_stages).
+// =============================================================================================
+constexpr int WIDE_N = 192;
+
+template <int BLOCK_K, bool BIAS, bool LEAKY>
+__global__ void __launch_bounds__(PP_THREADS, 1)
+conv_tc_wide_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+                    const __grid_constant__ CUtensorMap tmap_o, const TcParams p) {
+  constexpr int BLOCK_N = WIDE_N;
+  using L = SmemLayout<BLOCK_N, BLOCK_K, false>;
+  constexpr int BOXC = L::OUT_BOXC;
+  constexpr int BOX_BYTES = BLOCK_M * L::OUT_SPAN;
+  const int STAGES = p.stages;
+
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t *full_bar = reinterpret_cast<uint64_t *>(smem + p.bar_off);
+  uint64_t *empty_bar = full_bar + STAGES;
+  uint64_t *oempty_bar = empty_bar + STAGES;     // store issuer -> both warpgroups: the tensor stores have read the slot
+
+  const int wg = threadIdx.x >> 7;
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_tiles = p.n_lt * p.n_bg * p.n_nt;
+  const int kblocks = p.K * p.num_kb;
+
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmap_a);
+    tma_prefetch_desc(&tmap_b);
+    tma_prefetch_desc(&tmap_o);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full_bar[s], 1);
+      mbar_init(&empty_bar[s], 8);               // one arrival per MMA warp of both warpgroups
+    }
+    mbar_init(oempty_bar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+  griddep_launch_dependents();
+  griddep_wait();
+
+  Ring ring{full_bar, empty_bar, STAGES, 0, 0};
+  if (wg == 0) {
+    // =========================== TMA producer (warp-uniform loop, elected lane issues) ===========================
+    warpgroup_reg_dealloc<56>();
+    if (warp != 0) return;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
+      for (int k = 0; k < p.K; ++k) {
+        const TapOrigin o = tap_origin(k, p.dil, p.pad_l, p.stride);
+        for (int kb = 0; kb < p.num_kb; ++kb)
+          produce_kblock<BLOCK_N, BLOCK_K, false>(smem, ring, &tmap_a, &tmap_b, p, t, o, k, kb);
+      }
+    }
+  } else {
+    // =========================== MMA + epilogue warpgroups 1, 2: rows 64 h .. 64 h + 63 ===========================
+    warpgroup_reg_alloc<224>();
+    const int h = wg - 1;
+    const int w = warp & 3;
+    const bool issuer = threadIdx.x == 128;
+    const uint32_t smem_base = smem_u32(smem);
+    uint8_t *slot = smem + p.ops_off;
+    float d[1][BLOCK_N / 2];
+    int u = 0;                                     // tiles this CTA has run
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++u) {
+      const int prev = mma_mainloop<BLOCK_N, BLOCK_K, false, 1>(d, smem_base, ring, kblocks, lane, h);
+      mma_drain<BLOCK_N, 1>(d, ring, prev, lane);
+      const TileCoord t = tile_coord<BLOCK_N>(tile, p);
+      // the tensor stores of the previous tile have read the slot (they ran during this tile's main loop)
+      if (issuer && u > 0) {
+        bulk_wait_read<0>();
+        mbar_arrive(oempty_bar);
+      }
+      mbar_wait(oempty_bar, (u & 1) ^ 1);
+      pp_fwd_epilogue<BLOCK_N, BOXC, BIAS, LEAKY, 1>(d, slot, p, w, lane, t.n0, h);
+      // rows past Lout and batches past B fall outside the tensor map and are not written
+      fence_proxy_async();
+      named_bar_sync(1, 256);
+      if (issuer) {
+#pragma unroll
+        for (int cb = 0; cb < BLOCK_N / BOXC; ++cb)
+          tma_store_3d(&tmap_o, slot + cb * BOX_BYTES, t.n0 + cb * BOXC, t.l0, t.b0);
+        bulk_commit();
+      }
+    }
+    if (issuer) bulk_wait_all();
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
@@ -897,6 +1002,47 @@ static int pp_fwd_stages(int kblocks) {
   return s >= q.stages && (BN == 128 || kblocks <= 24) ? s : 0;
 }
 
+// Wide forward kernel (conv_tc_wide_kernel): BLOCK_K of a launch of Cin input channels, and its ring stages next to the
+// 48 KB output slot (4 at BLOCK_K = 64, 8 at BLOCK_K = 32).
+static int wide_block_k(int Cin) { return pick_block_k(Cin); }
+template <int BK>
+constexpr int wide_ring_stages() {
+  using L = SmemLayout<WIDE_N, BK, false>;
+  const int s = (SMEM_MAX - L::FIXED - L::STG_BYTES) / L::STAGE_BYTES;
+  return s > 8 ? 8 : s;
+}
+// Fewest k-blocks per tile for which a forward launch (bias / LeakyReLU -> bf16 only) with Cout % 192 == 0 runs the wide
+// kernel: its epilogue does not overlap the CTA's MMAs, so the short-k launches stay on the ping-pong kernel.  Measured
+// (DESIGN section 5.6): every v2 launch of 15-90 k-blocks per tile took 5-30 % less time than on the ping-pong kernel or
+// conv_tc_kernel; one of 12 k-blocks broke even.
+constexpr int WIDE_MIN_KBLOCKS = 12;
+// Instances: BLOCK_K = 64 and 32 (Cin a multiple of 32).
+static int wide_stages(int Cin, int Cout, int K) {
+  const int BK = wide_block_k(Cin);
+  if (BK < 32 || Cout % WIDE_N || K * ceil_div(Cin, BK) < WIDE_MIN_KBLOCKS) return 0;
+  return BK == 64 ? wide_ring_stages<64>() : wide_ring_stages<32>();
+}
+
+template <int BK>
+static int launch_wide(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, int stages, cudaStream_t stream) {
+  using L = SmemLayout<WIDE_N, BK, false>;
+  p.stages = stages;
+  p.ops_bytes = L::STG_BYTES;
+  p.ops_off = p.stages * L::STAGE_BYTES;
+  p.bar_off = p.ops_off + p.ops_bytes;
+  const int grid = persistent_grid(p.n_lt * p.n_bg * p.n_nt), smem = p.bar_off + L::FIXED;
+  CUtensorMap to;
+  if (encode_rows_map<WIDE_N>(&to, p.out_act, p, p.BB)) return 1;
+  const auto go = [&](auto bias, auto leaky) {
+    return launch_tc<conv_tc_wide_kernel<BK, decltype(bias)::value, decltype(leaky)::value>>(
+        "conv1d_tc", grid, PP_THREADS, smem, stream, ta, tb, to, p);
+  };
+  const std::true_type y;
+  const std::false_type n;
+  const bool leaky = p.act == RAVE_ACT_LEAKY;
+  return p.bias ? (leaky ? go(y, y) : go(y, n)) : (leaky ? go(n, y) : go(n, n));
+}
+
 // FWD: a forward launch (bias / LeakyReLU; the slot holds the output tile alone), else an input-gradient launch
 template <int BN, int BK, bool FWD>
 static int launch_pp(const CUtensorMap &ta, const CUtensorMap &tb, TcParams p, int stages, cudaStream_t stream) {
@@ -1004,6 +1150,16 @@ extern "C" int rave_conv1d_tc_pp_fwd_stages(int B, int Cin, int Cout, int Lout, 
   });
 }
 
+// Ring stages of the wide kernel (128 x 192 tiles, two MMA warpgroups per tile) for a forward launch of this shape (bias
+// and / or LeakyReLU, bf16 output only); 0 = the launch does not run it.  A launch the wide kernel takes runs neither
+// conv_tc_kernel nor the ping-pong kernel, whatever rave_conv1d_tc_plan and rave_conv1d_tc_pp_fwd_stages report for it.
+extern "C" int rave_conv1d_tc_wide_stages(int B, int Cin, int Cout, int Lout, int K) {
+  using namespace rave::tc;
+  const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
+  if (!g.BK || !g.BN) return 0;
+  return wide_stages(Cin, Cout, K);
+}
+
 static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias, const float *res,
                               const void *res_bf16, const void *dact_src, const void *res_act, float res_slope,
                               float *out_f32, void *out_act,
@@ -1036,7 +1192,14 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
 
   const TcGeometry g = tc_geometry(B, Cin, Cout, Lout);
   RAVE_CHECK_ARG(g.BN > 0, "conv1d_tc: no BLOCK_N for Cout=%d", Cout);
-  const int BK = g.BK, BN = g.BN;
+  // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only) and
+  // forward launches (bias and / or LeakyReLU, bf16 out only): the ping-pong kernel where pp_stages / pp_fwd_stages
+  // give it the launch; long-k forward launches with Cout % 192 == 0 the wide kernel (wide_stages)
+  const bool bf16_only = out_act && !res && !res_act && !out_f32;
+  const bool pp_dgrad = bf16_only && dact_src && !bias && act == RAVE_ACT_NONE;
+  const bool pp_fwd = bf16_only && !dact_src && !res_bf16 && !fm_d;
+  const int wide = !x3 && pp_fwd ? wide_stages(Cin, Cout, K) : 0;
+  const int BK = wide ? wide_block_k(Cin) : g.BK, BN = wide ? WIDE_N : g.BN;
   // 256-byte L2 promotion over-fetches when a TMA row is a 64-byte (or shorter) span of a 192-byte channel row
   // (measured on the Cin = 96 layers: 209.6 -> 184.7 us); neutral to slightly positive for 128-byte spans.
   const CUtensorMapL2promotion promo = BK == 64 ? CU_TENSOR_MAP_L2_PROMOTION_L2_256B : CU_TENSOR_MAP_L2_PROMOTION_NONE;
@@ -1062,7 +1225,9 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
                  "conv1d_tc(x3): %d channels per position do not tile the %d-column rows in 16-column chunks", p.act_cs,
                  Cout);
   RAVE_CHECK_ARG(!x3 || !res_act || p.act_cs == Cout, "conv1d_tc(x3): res_act needs one position per row");
-  p.BL = g.BL; p.BB = g.BB; p.n_lt = g.n_lt; p.n_bg = g.n_bg; p.n_nt = g.n_nt; p.num_kb = g.num_kb;
+  p.BL = g.BL; p.BB = g.BB; p.n_lt = g.n_lt; p.n_bg = g.n_bg;
+  p.n_nt = Cout / BN;
+  p.num_kb = ceil_div(Cin, BK);
 
   // A: channel-last activations viewed as (c, phase, l/stride, b)
   CUtensorMap ta, tb;
@@ -1083,12 +1248,7 @@ static int conv1d_tc_fwd_impl(const void *xa, const void *wt, const float *bias,
   }
   cudaStream_t s = (cudaStream_t)stream;
   if (x3) return conv_tc_dispatch_x3(BK, BN, ta, tb, p, s);
-  // input-gradient launches (LeakyReLU' mask, optional feature-matching term and gradient skip, bf16 out only) and
-  // forward launches (bias and / or LeakyReLU, bf16 out only): the ping-pong kernel where pp_stages / pp_fwd_stages
-  // give it the launch
-  const bool bf16_only = out_act && !res && !res_act && !out_f32;
-  const bool pp_dgrad = bf16_only && dact_src && !bias && act == RAVE_ACT_NONE;
-  const bool pp_fwd = bf16_only && !dact_src && !res_bf16 && !fm_d;
+  if (wide) return BK == 64 ? launch_wide<64>(ta, tb, p, wide, s) : launch_wide<32>(ta, tb, p, wide, s);
   const int nops = 1 + (fm_d ? 1 : 0) + (res_bf16 ? 1 : 0);
   return visit_tile(BK, BN, [&](auto bk, auto bn) {
     constexpr int BK_ = decltype(bk)::value, BN_ = decltype(bn)::value;

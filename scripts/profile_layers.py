@@ -96,8 +96,9 @@ def wgrad_runner(torch, ops, ints, ptrs):
 
 
 def instance(lib, name, ints, ptrs):
-    """Kernel of a launch; conv launches the ping-pong kernel takes are marked ` pp` and its ring stages, weight-gradient
-    launches carry their tile (rows of Cm x columns of Cn), split-K slices, CTAs and waves of 132 SMs."""
+    """Kernel of a launch; conv launches the ping-pong kernel takes are marked ` pp` and its ring stages, those the wide
+    kernel (128 x 192 tiles) takes `wide<192,BLOCK_K> s` and its ring stages, weight-gradient launches carry their tile
+    (rows of Cm x columns of Cn), split-K slices, CTAs and waves of 132 SMs."""
     if name == "rave_conv1d_tc_fwd":
         B, Cin, Cout, Lout, K, act = ints[0], ints[1], ints[4], ints[5], ints[6], ints[10]
         v = lib.rave_conv1d_tc_plan(B, Cin, Cout, Lout, K)
@@ -107,6 +108,9 @@ def instance(lib, name, ints, ptrs):
             if dact and not bias and act == 0:
                 stages = lib.rave_conv1d_tc_pp_stages(B, Cin, Cout, Lout, K, int(fm), int(res_bf16))
             elif not (dact or res_bf16 or fm):
+                wide = lib.rave_conv1d_tc_wide_stages(B, Cin, Cout, Lout, K)
+                if wide:
+                    return f"wide<192,{64 if Cin % 64 == 0 else 32}> s{wide}"
                 stages = lib.rave_conv1d_tc_pp_fwd_stages(B, Cin, Cout, Lout, K)
         return f"conv<{v & 0xfff},{(v >> 12) & 0xfff}>" + (f" pp{stages}" if stages else "")
     if name == "rave_conv1d_tc_wgrad":
