@@ -572,6 +572,34 @@ int rave_ema_update(const long long *table, int n_tensors, long long n_chunks, i
                     float one_minus_factor, void *stream);
 int rave_ema_swap(const long long *table, int n_tensors, long long n_chunks, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * The exported model's compact latent (scripts/export.py:351-408: the post / pre-processing of the four ScriptedRAVE
+ * subclasses), fp32, fixed-order sums, one thread per output unless stated.
+ *   latent_project:   z [B][2L][T] encoder output (mean | scale), eps [B][L][T] -> out [B][l][T] =
+ *                     latent_pca[:l] (eps (softplus(scale) + 1e-4) + mean - latent_mean), latent_pca [L][L], l <= L
+ *   latent_unproject: z [B][l][T], noise [B][L-l][T] (NULL when l = L) -> out [B][L][T] =
+ *                     latent_pca^T [z ; noise] + latent_mean
+ *   rvq_encode:       x [B][D][T], codebooks [Q][K][D] (16-byte aligned) -> codes [B][Q][T] int32: Q residual stages,
+ *                     code = argmin_k |r|^2 - 2 r.c_k + |c_k|^2 (ties: lowest k), r -= c_code; norms [Q][K] is a
+ *                     workspace that receives |c_k|^2.  Two launches (norms, then all Q stages); D % 4 == 0, D <= 256
+ *   rvq_decode:       codes [B][Q][T] float -> out [B][D + n_noise][T]: rows [0, D) = sum_q codebooks[q][k_q] added in q
+ *                     order, k_q = trunc(clamp(code, 0, K - 1)) (NaN -> 0); rows [D, D + n_noise) = noise [B][n_noise][T]
+ *                     (NULL when n_noise = 0)
+ *   sphere_to_angles: x [B][L][T] -> angles [B][L-1][T] (unit_norm_vector_to_angles, one thread per frame; the arccos
+ *                     argument is clamped to [-1, 1], NaN kept)
+ *   angles_to_sphere: angles [B][L-1][T] -> x [B][L][T] (angles_to_unit_norm_vector, floor modulo, one thread per frame)
+ * ------------------------------------------------------------------------------------------- */
+int rave_latent_project(const float *z, const float *eps, const float *latent_mean, const float *latent_pca, float *out,
+                        int B, int L, int T, int l, void *stream);
+int rave_latent_unproject(const float *z, const float *noise, const float *latent_mean, const float *latent_pca,
+                          float *out, int B, int L, int T, int l, void *stream);
+int rave_rvq_encode(const float *x, const float *codebooks, float *norms, int *codes, int B, int D, int T, int Q, int K,
+                    void *stream);
+int rave_rvq_decode(const float *codes, const float *codebooks, const float *noise, float *out, int B, int Q, int T,
+                    int K, int D, int n_noise, void *stream);
+int rave_sphere_to_angles(const float *x, float *angles, int B, int L, int T, void *stream);
+int rave_angles_to_sphere(const float *angles, float *x, int B, int L, int T, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -128,6 +128,12 @@ SIGNATURES = {
     "rave_ema_chunk_elems": (c_longlong, []),
     "rave_ema_update": (c_int, [_P, _I, c_longlong, _P, _F, _F, _P]),
     "rave_ema_swap": (c_int, [_P, _I, c_longlong, _P]),
+    "rave_latent_project": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "rave_latent_unproject": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "rave_rvq_encode": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "rave_rvq_decode": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
+    "rave_sphere_to_angles": (c_int, [_P, _P, _I, _I, _I, _P]),
+    "rave_angles_to_sphere": (c_int, [_P, _P, _I, _I, _I, _P]),
 }
 
 

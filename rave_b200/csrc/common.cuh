@@ -93,6 +93,14 @@ __device__ __forceinline__ bool block_sum_finish(const BlockSum &s, float *out) 
   return true;
 }
 
+// VariationalEncoder.reparametrize's sample minus the latent mean: eps (softplus(scale) + 1e-4) + mean - latent_mean,
+// torch's softplus (threshold 20), every step rounded on its own (no FMA contraction).  Shared by the prior's latent
+// classes and the exported model's latent projection, so both see the same bits.
+__device__ __forceinline__ float centred_sample(float mean, float scale, float eps, float latent_mean) {
+  const float sd = __fadd_rn(scale > 20.f ? scale : log1pf(expf(scale)), 1e-4f);
+  return __fsub_rn(__fadd_rn(__fmul_rn(eps, sd), mean), latent_mean);
+}
+
 // activation(dim) of rave/blocks.py: LeakyReLU(slope) / Snake(alpha)
 __device__ __forceinline__ float act_apply(float x, int act, float slope, float alpha) {
   if (act == RAVE_ACT_LEAKY) return x > 0.f ? x : x * slope;

@@ -43,9 +43,7 @@ prior_latent_classes_kernel(const float *__restrict__ z, const float *__restrict
   const float *zm = z + (size_t)b * 2 * L * T + t, *zs = zm + (size_t)L * T, *ep = eps + (size_t)b * L * T + t;
   float acc = 0.f;
   for (int c = 0; c < L; ++c) {
-    const float sc = zs[(size_t)c * T];
-    const float sd = __fadd_rn(sc > 20.f ? sc : log1pf(expf(sc)), 1e-4f);      // softplus (threshold 20) + 1e-4
-    const float s = __fsub_rn(__fadd_rn(__fmul_rn(ep[(size_t)c * T], sd), zm[(size_t)c * T]), lmean[c]);
+    const float s = centred_sample(zm[(size_t)c * T], zs[(size_t)c * T], ep[(size_t)c * T], lmean[c]);
     acc = fmaf(pca[(size_t)d * L + c], s, acc);
   }
   const float u = 0.5f * (1.f + erff(acc / 1.41421356237309515f));

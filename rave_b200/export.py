@@ -1,0 +1,176 @@
+"""`ExportedRAVE`: the compact latent interface of a trained model, as the reference's export exposes it
+(`ScriptedRAVE` and its four subclasses, scripts/export.py:75-409), without TorchScript, nn~ registration or resampling.
+
+`encode` returns the compact latent and `decode` takes one:
+  * VariationalEncoder: the posterior sample, centred on `latent_mean`, projected onto the first `latent_size` PCA rows;
+    decode fills the dropped dimensions with standard normal noise and inverts the projection;
+  * DiscreteEncoder: the residual-VQ codes as floats; decode clamps them, sums the codebook rows and appends the
+    `noise_augmentation` noise channels;
+  * WasserteinEncoder: encode is the identity; decode appends the noise channels;
+  * SphericalEncoder: the `latent_size - 1` hyperspherical angles in [-1, 1) of the raw encoder output; decode maps them
+    back to unit vectors.
+The latent arithmetic runs on csrc/export.cu.  Neither call synchronises with the host, so `encode` -> `decode` can be
+captured in a CUDA graph.
+
+Random draws (the posterior's eps, the decode noise) come from the current CUDA generator on the model's device unless
+`eps` / `noise` inject them.  The reference draws the decode noise on the CPU: same distribution, different stream (as in
+`Prior.decode_classes`).
+
+`set_stereo_mode` is not provided: its batch folding only makes sense inside nn~, which passes the two channels of a
+stereo stream as two batch rows.
+"""
+import math
+from typing import Optional
+
+import numpy as np
+import torch
+import torch.nn as nn
+
+from . import blocks, ops
+
+
+def _kind(encoder) -> str:
+    if isinstance(encoder, blocks.VariationalEncoder):
+        return "variational"
+    if isinstance(encoder, blocks.DiscreteEncoder):
+        return "discrete"
+    if isinstance(encoder, blocks.WasserteinEncoder):
+        return "wasserstein"
+    if isinstance(encoder, blocks.SphericalEncoder):
+        return "spherical"
+    raise ValueError(f"Encoder type {encoder.__class__.__name__} not supported")
+
+
+def variational_latent_size(fidelity: torch.Tensor, f: float) -> int:
+    """scripts/export.py:120-122: the first index whose cumulative explained variance exceeds f (at least 1), rounded
+    up to a power of two.  argmax of an all-False mask is 0, so an untrained model (fidelity all zero) gives 1."""
+    size = max(int(np.argmax(fidelity.detach().cpu().numpy() > f)), 1)
+    return 2 ** math.ceil(math.log2(size))
+
+
+class ExportedRAVE(nn.Module):
+    """The exported model's encode / decode / forward around a trained `RAVE` (put in eval mode, as the export does).
+
+    `channels`: number of output channels of decode (default: the model's).  More than the model has: every example is
+    decoded ceil(channels / n_channels) times, each time with its own noise, and the decodes are stacked along the
+    channel axis (the reference does this for one example; with a larger batch it slices the batch instead).  Fewer:
+    the first channels are kept.  `fidelity`: explained variance that sets `latent_size` of a variational model.
+
+    Style transfer of a model with AdaIN layers: set `learn_target`, `learn_source`, `reset_target`, `reset_source`;
+    they are applied through `RAVE.update_adain` before `encode` and before a `decode` that `forward` did not call, and
+    the two resets clear after each application (scripts/export.py:213-230)."""
+
+    def __init__(self, model, channels: Optional[int] = None, fidelity: float = .95):
+        super().__init__()
+        model.eval()
+        self.model = model
+        self.kind = _kind(model.encoder)
+        self.n_channels = model.n_channels
+        self.target_channels = channels or self.n_channels
+        self.full_latent_size = model.latent_size
+        self.is_using_adain = any(isinstance(m, blocks.AdaptiveInstanceNormalization) for m in model.modules())
+        if self.is_using_adain and self.n_channels != self.target_channels:
+            raise ValueError("AdaIN requires the original number of channels")
+        self.learn_target = False
+        self.learn_source = False
+        self.reset_target = False
+        self.reset_source = False
+
+        enc = model.encoder
+        if self.kind == "variational":
+            self.latent_size = variational_latent_size(model.fidelity, fidelity)
+            if self.latent_size > self.full_latent_size:
+                raise ValueError(f"fidelity {fidelity} gives {self.latent_size} latent dimensions, more than the "
+                                 f"model's {self.full_latent_size}")
+        elif self.kind == "discrete":
+            self.latent_size = enc.num_quantizers
+            if any(not isinstance(vq.project_in, nn.Identity) for vq in enc.rvq.layers):
+                raise ValueError("the residual VQ's codebook dimension must equal the latent size")
+        elif self.kind == "wasserstein":
+            self.latent_size = self.full_latent_size
+        else:
+            self.latent_size = self.full_latent_size - 1
+        self.n_noise = getattr(enc, "noise_augmentation", 0) if self.kind in ("discrete", "wasserstein") else 0
+
+        dev = model.latent_pca.device
+        x_len = 2 ** 14
+        z = self.encode(torch.zeros(1, self.n_channels, x_len, device=dev))
+        self.encode_ratio = x_len // z.shape[-1]
+
+    # ------------------------------------------------------------------ latent arithmetic
+    def _codebooks(self):
+        return torch.stack([vq.codebook for vq in self.model.encoder.rvq.layers]).float()
+
+    def post_process_latent(self, z, eps=None):
+        z = z.float()
+        if self.kind == "variational":
+            B, L2, T = z.shape
+            eps = self._draw(eps, (B, L2 // 2, T), z.device, "eps")
+            return ops.latent_project(z, eps, self.model.latent_mean.float(), self.model.latent_pca.float(),
+                                      self.latent_size)
+        if self.kind == "discrete":
+            return ops.rvq_encode(z, self._codebooks()).float()
+        if self.kind == "wasserstein":
+            return z
+        return ops.sphere_to_angles(z)
+
+    def pre_process_latent(self, z, noise=None):
+        z = z.float()
+        B, _, T = z.shape
+        if self.kind == "variational":
+            noise = self._draw(noise, (B, self.full_latent_size - z.shape[1], T), z.device, "noise")
+            return ops.latent_unproject(z, noise, self.model.latent_mean.float(), self.model.latent_pca.float())
+        if self.kind == "spherical":
+            return ops.angles_to_sphere(z)
+        noise = self._draw(noise, (B, self.n_noise, T), z.device, "noise") if self.n_noise else None
+        if self.kind == "discrete":
+            return ops.rvq_decode(z, self._codebooks(), noise)
+        return z if noise is None else torch.cat([z, noise], 1)
+
+    @staticmethod
+    def _draw(given, shape, device, name):
+        if given is None:
+            return torch.randn(shape, device=device)
+        if tuple(given.shape) != tuple(shape):
+            raise ValueError(f"{name} has shape {tuple(given.shape)}, expected {tuple(shape)}")
+        return given.to(device=device, dtype=torch.float32)
+
+    # ------------------------------------------------------------------ style transfer flags
+    def _update_adain(self):
+        self.model.update_adain(self.learn_target, self.learn_source, self.reset_target, self.reset_source)
+        self.reset_source = False
+        self.reset_target = False
+
+    # ------------------------------------------------------------------ interface
+    @torch.no_grad()
+    def encode(self, x, eps: Optional[torch.Tensor] = None):
+        """x [B, n_channels, N] -> compact latent [B, latent_size, N / encode_ratio].  `eps` [B, L, T]: the posterior's
+        standard normal draw of a variational model."""
+        if self.is_using_adain:
+            self._update_adain()
+        return self.post_process_latent(self.model.encode(x), eps)
+
+    @torch.no_grad()
+    def decode(self, z, noise: Optional[torch.Tensor] = None):
+        """Compact latent [B, latent_size, T] -> audio [B, target_channels, T * encode_ratio].  `noise`: the draw of
+        pre_process_latent for the ceil(target_channels / n_channels) B decoded rows (row b r + i is decode i of
+        example b): [B r, L - latent_size, T] (variational) or [B r, noise_augmentation, T]."""
+        return self._decode(z, noise, from_forward=False)
+
+    @torch.no_grad()
+    def forward(self, x, eps: Optional[torch.Tensor] = None, noise: Optional[torch.Tensor] = None):
+        return self._decode(self.encode(x, eps), noise, from_forward=True)
+
+    def _decode(self, z, noise, from_forward: bool):
+        if self.is_using_adain and not from_forward:
+            self._update_adain()
+        B, T = z.shape[0], z.shape[-1]
+        reps = math.ceil(self.target_channels / self.n_channels) if self.target_channels > self.n_channels else 1
+        if reps > 1:
+            z = z.repeat_interleave(reps, 0)
+        y = self.model.decode(self.pre_process_latent(z, noise))
+        if y.shape[-1] > T * self.encode_ratio:
+            y = y[..., :T * self.encode_ratio]
+        if reps > 1:
+            y = y.reshape(B, reps * self.n_channels, y.shape[-1])
+        return y[:, :self.target_channels] if self.target_channels != y.shape[1] else y

@@ -1541,6 +1541,73 @@ def prior_classes_to_latent(classes, dither, noise, latent_pca, latent_mean, R):
 
 
 # ----------------------------------------------------------------------------------------------
+# The exported model's compact latent (csrc/export.cu, rave_b200/export.py)
+# ----------------------------------------------------------------------------------------------
+
+def latent_project(z, eps, latent_mean, latent_pca, l):
+    """Encoder output z [B, 2L, T] and eps [B, L, T] -> the first l PCA coordinates of the centred sample [B, l, T]."""
+    z, eps, latent_mean, latent_pca = _f32c(z), _f32c(eps), _f32c(latent_mean), _f32c(latent_pca)
+    B, L2, T = z.shape
+    out = torch.empty(B, l, T, dtype=torch.float32, device=z.device)
+    call("rave_latent_project", ptr(z), ptr(eps), ptr(latent_mean), ptr(latent_pca), ptr(out), B, L2 // 2, T, int(l),
+         stream_ptr())
+    return out
+
+
+def latent_unproject(z, noise, latent_mean, latent_pca):
+    """z [B, l, T] and noise [B, L - l, T] -> latent_pca.T @ [z; noise] + latent_mean, [B, L, T]."""
+    z, latent_mean, latent_pca = _f32c(z), _f32c(latent_mean), _f32c(latent_pca)
+    B, l, T = z.shape
+    L = latent_pca.shape[0]
+    out = torch.empty(B, L, T, dtype=torch.float32, device=z.device)
+    call("rave_latent_unproject", ptr(z), ptr(None if l == L else _f32c(noise)), ptr(latent_mean), ptr(latent_pca),
+         ptr(out), B, L, T, l, stream_ptr())
+    return out
+
+
+def rvq_encode(x, codebooks):
+    """x [B, D, T], codebooks [Q, K, D] -> int32 residual-VQ codes [B, Q, T] (all Q stages in one launch)."""
+    x, codebooks = _f32c(x), _f32c(codebooks)
+    B, D, T = x.shape
+    Q, K, _ = codebooks.shape
+    norms = torch.empty(Q, K, dtype=torch.float32, device=x.device)
+    codes = torch.empty(B, Q, T, dtype=torch.int32, device=x.device)
+    call("rave_rvq_encode", ptr(x), ptr(codebooks), ptr(norms), ptr(codes), B, D, T, Q, K, stream_ptr())
+    return codes
+
+
+def rvq_decode(codes, codebooks, noise=None):
+    """Float codes [B, Q, T] (clamped to [0, K - 1], truncated) -> sum of the codebook rows [B, D, T], followed by the
+    channels of noise [B, N, T] when given: [B, D + N, T]."""
+    codes, codebooks = _f32c(codes), _f32c(codebooks)
+    B, Q, T = codes.shape
+    _, K, D = codebooks.shape
+    n_noise = 0 if noise is None else noise.shape[1]
+    out = torch.empty(B, D + n_noise, T, dtype=torch.float32, device=codes.device)
+    call("rave_rvq_decode", ptr(codes), ptr(codebooks), ptr(_f32c(noise)), ptr(out), B, Q, T, K, D, n_noise,
+         stream_ptr())
+    return out
+
+
+def sphere_to_angles(x):
+    """x [B, L, T] -> the L - 1 hyperspherical angles of each frame in [-1, 1), [B, L - 1, T]."""
+    x = _f32c(x)
+    B, L, T = x.shape
+    out = torch.empty(B, L - 1, T, dtype=torch.float32, device=x.device)
+    call("rave_sphere_to_angles", ptr(x), ptr(out), B, L, T, stream_ptr())
+    return out
+
+
+def angles_to_sphere(angles):
+    """angles [B, L - 1, T] -> unit vectors [B, L, T]."""
+    angles = _f32c(angles)
+    B, L1, T = angles.shape
+    out = torch.empty(B, L1 + 1, T, dtype=torch.float32, device=angles.device)
+    call("rave_angles_to_sphere", ptr(angles), ptr(out), B, L1 + 1, T, stream_ptr())
+    return out
+
+
+# ----------------------------------------------------------------------------------------------
 # Training-batch transforms (rave_b200/transforms.py)
 # ----------------------------------------------------------------------------------------------
 
