@@ -600,6 +600,16 @@ int rave_rvq_decode(const float *codes, const float *codebooks, const float *noi
 int rave_sphere_to_angles(const float *x, float *angles, int B, int L, int T, void *stream);
 int rave_angles_to_sphere(const float *angles, float *x, int B, int L, int T, void *stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * The export's resampler (rave/resampler.py), one phase-bank FIR per row of x [rows][L_in]:
+ *   y[r][i P + p] = sum_{k < K} w[p][k] x[r][i S + k - pad] (x = 0 outside [0, L_in)), i < n_pos, p < P,
+ * y [rows][n_pos P], w [P][K].  Down (to_model_sampling_rate): P = 1, S = ratio; up (from_model_sampling_rate):
+ * P = ratio, S = 1, written interleaved.  Each output is a chain of float32 FMAs over k in increasing order.
+ * 1 <= P, S <= 8, 1 <= K <= 64; one launch, no atomics.
+ * ------------------------------------------------------------------------------------------- */
+int rave_resample(const float *x, const float *w, float *y, long long rows, int L_in, int n_pos, int P, int S, int K,
+                  int pad, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -134,6 +134,7 @@ SIGNATURES = {
     "rave_rvq_decode": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]),
     "rave_sphere_to_angles": (c_int, [_P, _P, _I, _I, _I, _P]),
     "rave_angles_to_sphere": (c_int, [_P, _P, _I, _I, _I, _P]),
+    "rave_resample": (c_int, [_P, _P, _P, c_longlong, _I, _I, _I, _I, _I, _I, _P]),
 }
 
 

@@ -1,5 +1,5 @@
 """`ExportedRAVE`: the compact latent interface of a trained model, as the reference's export exposes it
-(`ScriptedRAVE` and its four subclasses, scripts/export.py:75-409), without TorchScript, nn~ registration or resampling.
+(`ScriptedRAVE` and its four subclasses, scripts/export.py:75-409), without TorchScript or nn~ registration.
 
 `encode` returns the compact latent and `decode` takes one:
   * VariationalEncoder: the posterior sample, centred on `latent_mean`, projected onto the first `latent_size` PCA rows;
@@ -9,8 +9,10 @@
   * WasserteinEncoder: encode is the identity; decode appends the noise channels;
   * SphericalEncoder: the `latent_size - 1` hyperspherical angles in [-1, 1) of the raw encoder output; decode maps them
     back to unit vectors.
-The latent arithmetic runs on csrc/export.cu.  Neither call synchronises with the host, so `encode` -> `decode` can be
-captured in a CUDA graph.
+The latent arithmetic runs on csrc/export.cu.  With `target_sr` (the export's `--sr`), the model runs in a host at
+`target_sr = ratio * sr`: encode resamples its input down to the model's rate first, decode resamples the model's output
+up before the crop (rave_b200/resampler.py, csrc/resample.cu).  Neither call synchronises with the host, so
+`encode` -> `decode` can be captured in a CUDA graph.
 
 Random draws (the posterior's eps, the decode noise) come from the current CUDA generator on the model's device unless
 `eps` / `noise` inject them.  The reference draws the decode noise on the CPU: same distribution, different stream (as in
@@ -27,6 +29,7 @@ import torch
 import torch.nn as nn
 
 from . import blocks, ops
+from .resampler import Resampler
 
 
 def _kind(encoder) -> str:
@@ -55,15 +58,22 @@ class ExportedRAVE(nn.Module):
     decoded ceil(channels / n_channels) times, each time with its own noise, and the decodes are stacked along the
     channel axis (the reference does this for one example; with a larger batch it slices the batch instead).  Fewer:
     the first channels are kept.  `fidelity`: explained variance that sets `latent_size` of a variational model.
+    `target_sr`: the host's sample rate, a multiple of the model's `sr` (ratios 2 and 3 can be built); `sr` becomes
+    `target_sr` and `encode_ratio` counts samples at that rate.
 
     Style transfer of a model with AdaIN layers: set `learn_target`, `learn_source`, `reset_target`, `reset_source`;
     they are applied through `RAVE.update_adain` before `encode` and before a `decode` that `forward` did not call, and
     the two resets clear after each application (scripts/export.py:213-230)."""
 
-    def __init__(self, model, channels: Optional[int] = None, fidelity: float = .95):
+    def __init__(self, model, channels: Optional[int] = None, fidelity: float = .95, target_sr: Optional[int] = None):
         super().__init__()
         model.eval()
         self.model = model
+        self.resampler = None
+        if target_sr is not None and target_sr != model.sr:
+            if target_sr % model.sr:
+                raise ValueError(f"target_sr {target_sr} is not a multiple of the model's sampling rate {model.sr}")
+            self.resampler = Resampler(target_sr, model.sr).to(model.latent_pca.device)
         self.kind = _kind(model.encoder)
         self.n_channels = model.n_channels
         self.target_channels = channels or self.n_channels
@@ -96,6 +106,11 @@ class ExportedRAVE(nn.Module):
         x_len = 2 ** 14
         z = self.encode(torch.zeros(1, self.n_channels, x_len, device=dev))
         self.encode_ratio = x_len // z.shape[-1]
+
+    @property
+    def sr(self) -> int:
+        """The sampling rate encode takes and decode returns: target_sr with a resampler, else the model's."""
+        return self.resampler.target_sr if self.resampler is not None else self.model.sr
 
     # ------------------------------------------------------------------ latent arithmetic
     def _codebooks(self):
@@ -148,6 +163,8 @@ class ExportedRAVE(nn.Module):
         standard normal draw of a variational model."""
         if self.is_using_adain:
             self._update_adain()
+        if self.resampler is not None:
+            x = self.resampler.to_model_sampling_rate(x.float())
         return self.post_process_latent(self.model.encode(x), eps)
 
     @torch.no_grad()
@@ -169,6 +186,8 @@ class ExportedRAVE(nn.Module):
         if reps > 1:
             z = z.repeat_interleave(reps, 0)
         y = self.model.decode(self.pre_process_latent(z, noise))
+        if self.resampler is not None:
+            y = self.resampler.from_model_sampling_rate(y.float())
         if y.shape[-1] > T * self.encode_ratio:
             y = y[..., :T * self.encode_ratio]
         if reps > 1:

@@ -1608,6 +1608,22 @@ def angles_to_sphere(angles):
 
 
 # ----------------------------------------------------------------------------------------------
+# The export's resampler (csrc/resample.cu, rave_b200/resampler.py)
+# ----------------------------------------------------------------------------------------------
+
+def resample(x, w, stride: int, pad: Tuple[int, int]):
+    """Phase-bank FIR over every row of x [..., L]: w [P, K], y[..., i P + p] = sum_k w[p, k] x[..., i stride + k - pad[0]]
+    (zero outside the row), n = (L + pad[0] + pad[1] - K) // stride + 1 positions i -> y [..., n P].  One launch."""
+    x, w = _f32c(x), _f32c(w)
+    L = x.shape[-1]
+    P, K = w.shape
+    n = (L + pad[0] + pad[1] - K) // stride + 1
+    y = torch.empty(*x.shape[:-1], n * P, dtype=torch.float32, device=x.device)
+    call("rave_resample", ptr(x), ptr(w), ptr(y), x.numel() // L, L, n, P, stride, K, pad[0], stream_ptr())
+    return y
+
+
+# ----------------------------------------------------------------------------------------------
 # Training-batch transforms (rave_b200/transforms.py)
 # ----------------------------------------------------------------------------------------------
 
