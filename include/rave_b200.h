@@ -546,6 +546,33 @@ int rave_prior_classes_to_latent(const int *classes, const float *dither, const 
                                  const float *latent_mean, float *z, int B, int T, int D, int L, int R, void *stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Streaming generation from the latent prior (the exported model's `prior(temp)`, scripts/export.py TraceModel), the
+ * sampler's kernels with state kept from call to call.  The caller owns `work` (rave_prior_stream_workspace_bytes, -1
+ * for a bad shape); no call but reset clears it.  It holds the frame counter, the class ring, the per-block rings, the
+ * row temperatures and the diagonal cache of decoded values.
+ *   prior_stream_create:  checks the shape as prior_sample does (B <= 64 rows), copies the parameter pointers and
+ *                         captures one frame's launches into a CUDA graph, kept until destroy.  The parameters are read
+ *                         through those pointers at every replay; re-create when they move.  Does not touch `work`.
+ *   prior_stream_reset:   the initial state: frame 0 of class R / 2 in every dim (QuantizedNormal.encode(0)), zero conv
+ *                         history, a diagonal cache of 0.0.
+ *   prior_stream:         T >= 1 frames: one prologue launch (row temperature softplus(mean_t temp[b][0][t]) / ln 2 in
+ *                         float32, the call's frame base and tensors) and T replays of the frame graph.  Frame n + 1's
+ *                         class in dim d is the inverse CDF at uniform[b][i][d] of the softmax of logits / temperature
+ *                         (i the frame's index in the call); its decode with dither[b][i][d] enters the cache, and
+ *                         out[b][d][i] is the decoded dim d of frame n + 1 - (D - 1 - d) (0.0 before the first).
+ *                         temp [B][1][T], uniform / dither [B][T][D], out [B][D][T], float32.  Refuses to run inside a
+ *                         stream capture.
+ *   prior_stream_destroy: frees the graph (not `work`).
+ * ------------------------------------------------------------------------------------------- */
+long rave_prior_stream_workspace_bytes(int B, int n_layers, int cycle_size, int res_size, int skp_size, int K, int D);
+int rave_prior_stream_create(const float *const *params, int n_layers, int cycle_size, int res_size, int skp_size,
+                             int K, int R, int D, int B, void *work, long work_bytes, void **state);
+int rave_prior_stream_reset(void *state, void *stream);
+int rave_prior_stream(void *state, const float *temp, const float *uniform, const float *dither, float *out, int T,
+                      void *stream);
+int rave_prior_stream_destroy(void *state);
+
+/* ---------------------------------------------------------------------------------------------
  * Training-batch transforms (get_dataset's transform list, rave/dataset.py:207-262), per example b of raw [B][C][L]
  * (int16 when raw_int16, else float32; C channels share every draw) -> out [B][C][N] float32:
  *   decode float32(int16) / 32767; crop [off, off + N); when apply, the allpass lfilter(b, a) of

@@ -124,6 +124,11 @@ SIGNATURES = {
     "rave_prior_sample_workspace_bytes": (c_long, [_I, _I, _I, _I, _I, _I, _I]),
     "rave_prior_sample": (c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _P, _I, _P, _I, _I, _I, _P, _P, _P, _L, _P]),
     "rave_prior_classes_to_latent": (c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "rave_prior_stream_workspace_bytes": (c_long, [_I, _I, _I, _I, _I, _I, _I]),
+    "rave_prior_stream_create": (c_int, [_P, _I, _I, _I, _I, _I, _I, _I, _I, _P, _L, _P]),
+    "rave_prior_stream_reset": (c_int, [_P, _P]),
+    "rave_prior_stream": (c_int, [_P, _P, _P, _P, _P, _I, _P]),
+    "rave_prior_stream_destroy": (c_int, [_P]),
     "rave_augment": (c_int, [_P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _I, _P]),
     "rave_ema_chunk_elems": (c_longlong, []),
     "rave_ema_update": (c_int, [_P, _I, c_longlong, _P, _F, _F, _P]),

@@ -12,10 +12,16 @@
 //                                     first argmax, or the inverse CDF of the softmax at an explicit uniform
 //                           One frame's launches are captured once into a CUDA graph and replayed T - 1 times; the frame
 //                           index lives in the workspace and the head advances it.
+//   prior_stream          : the exported model's prior(temp) (scripts/export.py TraceModel): the same frame stages on a
+//                           state the caller keeps from call to call; the frame graph is captured once per state and
+//                           replayed once per frame, and the head also divides the logits by the row's temperature,
+//                           decodes the class and writes the diagonally shifted output.
 //   prior_classes_to_latent: QuantizedNormal.decode (dither given), DiagonalShift.inverse and
 //                           VariationalPrior.pre_process_latent (noise given) in one pass.
 // fp32 CUDA-core arithmetic.  Every dot product is added in one fixed order per output (lane-strided partials, then a
 // fixed xor tree), which depends on neither B nor the other rows; no float atomics.
+#include <vector>
+
 #include "common.cuh"
 
 namespace rave {
@@ -35,6 +41,11 @@ enum { MODE_GATE = 0, MODE_RES_SKIP = 1, MODE_POST = 2 };
 struct Ctl {
   int step;            // frame consumed by the current step
   unsigned ticket;     // head CTAs done with the current step
+  // prior_stream only (zero in prior_sample): the call's first produced frame, its length and its tensors, written by
+  // the call's prologue so that the one captured frame graph serves calls of any length
+  int base, T;
+  const float *uniform, *dither;   // [B][T][D]
+  float *out;                      // [B][D][T]
 };
 
 // Workspace: control word, class ring [B][K][D], per block the ring of dconv inputs [B][S_l][C] with
@@ -42,6 +53,7 @@ struct Ctl {
 struct Layout {
   size_t cls, ring[64], g, skp, p, total;
   int S[64];
+  size_t temp, diag;   // prior_stream only
 };
 
 inline size_t up256(size_t x) { return (x + 255) & ~(size_t)255; }
@@ -64,6 +76,23 @@ Layout layout(int B, int n_layers, int cycle, int C, int Sk, int K, int D) {
   o += up256((size_t)B * Sk * sizeof(float));
   L.total = o;
   return L;
+}
+
+// prior_stream: the sampler's layout, then the row temperatures temp [B] and the diagonal cache [B][D][D]: the decoded
+// value of dim d of produced frame n in slot [b][d][n mod D]
+Layout stream_layout(int B, int n_layers, int cycle, int C, int Sk, int K, int D) {
+  Layout L = layout(B, n_layers, cycle, C, Sk, K, D);
+  L.temp = L.total;
+  L.diag = L.temp + up256((size_t)B * sizeof(float));
+  L.total = L.diag + up256((size_t)B * D * D * sizeof(float));
+  return L;
+}
+
+// QuantizedNormal.decode of class k with its dither: clamp(erfinv(2 x - 1) sqrt 2, -4, 4), x = k / R + dither / R
+__device__ __forceinline__ float class_to_normal(int k, float dither, float rf) {
+  const float x = __fadd_rn(__fdiv_rn((float)k, rf), __fdiv_rn(dither, rf));
+  const float y = __fmul_rn(erfinvf(__fsub_rn(__fmul_rn(2.f, x), 1.f)), 1.41421356237309515f);
+  return fminf(fmaxf(y, -4.f), 4.f);
 }
 
 __device__ __forceinline__ int wrap(int t, int S) {
@@ -250,11 +279,15 @@ __global__ void __launch_bounds__(PS_THREADS) ps_rows_kernel(const RowsArgs a) {
 // t + 1: prefix[b][t + 1][d] while t + 1 < P, else the first argmax, else the inverse CDF: the first r whose running sum
 // of softmax probabilities (max subtracted, classes 0..R-1 in order) exceeds u = uniform[b][t + 1][d], or the last r of
 // non-zero probability if rounding leaves none.  The last CTA to finish advances the frame index.
+// prior_stream (diag non-null): the logits are divided by the row's temperature temp[b] first, the uniform is
+// ctl->uniform[b][f][d] with f = t + 1 - ctl->base the frame's index in the call, and the CTA then decodes its class with
+// ctl->dither[b][f][d] into diag[b][d][(t + 1) mod D] and writes ctl->out[b][d][f] = diag[b][d][(t + 1 - (D-1-d)) mod D]
+// (DiagonalShift.inverse: dim d lags the newest frame by D - 1 - d frames).
 __global__ void __launch_bounds__(PS_HEAD_THREADS)
 ps_head_kernel(Ctl *__restrict__ ctl, const float *__restrict__ p, const float *__restrict__ w,
                const float *__restrict__ bias, const int *__restrict__ prefix, const float *__restrict__ uniform,
                int *__restrict__ classes, int *__restrict__ cls_ring, float *__restrict__ logits, int Sk, int D, int R,
-               int K, int P, int T, int argmax) {
+               int K, int P, int T, int argmax, const float *__restrict__ temp, float *__restrict__ diag) {
   __shared__ float lg[PS_MAX_R];
   const int d = blockIdx.x, b = blockIdx.y, Cg = Sk / D, t = ctl->step;
   const float *pb = p + (size_t)b * Sk + (size_t)d * Cg;
@@ -263,11 +296,17 @@ ps_head_kernel(Ctl *__restrict__ ctl, const float *__restrict__ p, const float *
     float acc = 0.f;
     for (int j = 0; j < Cg; ++j) acc = fmaf(wr[j], pb[j], acc);
     const float l = acc + bias[d * R + r];
-    lg[r] = l;
+    lg[r] = diag ? __fdiv_rn(l, temp[b]) : l;
     if (logits) logits[(((size_t)b * (T - 1) + t) * D + d) * R + r] = l;
   }
   __syncthreads();
   if (threadIdx.x != 0) return;
+  int f = t + 1;
+  if (diag) {
+    f -= ctl->base;
+    T = ctl->T;
+    uniform = ctl->uniform;
+  }
   int k;
   if (t + 1 < P) {
     k = prefix[((size_t)b * P + t + 1) * D + d];
@@ -280,7 +319,7 @@ ps_head_kernel(Ctl *__restrict__ ctl, const float *__restrict__ p, const float *
     for (int r = 1; r < R; ++r) m = fmaxf(m, lg[r]);
     float s = 0.f;
     for (int r = 0; r < R; ++r) s += expf(lg[r] - m);
-    const float u = uniform[((size_t)b * T + t + 1) * D + d];
+    const float u = uniform[((size_t)b * T + f) * D + d];
     float cum = 0.f;
     int last = 0;
     k = -1;
@@ -292,7 +331,13 @@ ps_head_kernel(Ctl *__restrict__ ctl, const float *__restrict__ p, const float *
     }
     if (k < 0) k = last;
   }
-  classes[((size_t)b * T + t + 1) * D + d] = k;
+  if (diag) {
+    float *db = diag + ((size_t)b * D + d) * D;
+    db[(t + 1) % D] = class_to_normal(k, ctl->dither[((size_t)b * T + f) * D + d], (float)R);
+    ctl->out[((size_t)b * D + d) * T + f] = db[wrap(t + 1 - (D - 1 - d), D)];
+  } else {
+    classes[((size_t)b * T + t + 1) * D + d] = k;
+  }
   cls_ring[((size_t)b * K + (t + 1) % K) * D + d] = k;
   __threadfence();
   if (atomicAdd(&ctl->ticket, 1u) == gridDim.x * gridDim.y - 1) {
@@ -318,9 +363,7 @@ ps_latent_kernel(const int *__restrict__ cls, const float *__restrict__ dither, 
     float y;
     if (c < D) {
       const size_t e = ((size_t)b * T + t + c) * D + c;
-      const float x = __fadd_rn(__fdiv_rn((float)cls[e], rf), __fdiv_rn(dither[e], rf));
-      y = __fmul_rn(erfinvf(__fsub_rn(__fmul_rn(2.f, x), 1.f)), 1.41421356237309515f);
-      y = fminf(fmaxf(y, -4.f), 4.f);
+      y = class_to_normal(cls[e], dither[e], rf);
     } else {
       y = noise[((size_t)b * (L - D) + (c - D)) * Tq + t];
     }
@@ -342,6 +385,7 @@ struct Plan {
   float *logits;
   char *work;
   Layout L;
+  bool stream = false;     // prior_stream: temperature and diagonal-cache output in the head
 };
 
 // one step: frame ctl->step in, frame ctl->step + 1 out
@@ -372,8 +416,95 @@ void enqueue_frame(const Plan &q, cudaStream_t s) {
   ps_rows_kernel<<<ceil_div(q.Sk, PS_ROWS), PS_THREADS, rows_smem(q.Sk, 1), s>>>(pa);
   ps_head_kernel<<<dim3(q.D, q.B), PS_HEAD_THREADS, 0, s>>>(ctl, p, pp[2], pp[3], q.prefix, q.uniform, q.classes,
                                                            cls_ring, q.logits, q.Sk, q.D, q.R, q.K, q.P, q.T,
-                                                           q.argmax);
+                                                           q.argmax,
+                                                           q.stream ? reinterpret_cast<float *>(q.work + L.temp) : nullptr,
+                                                           q.stream ? reinterpret_cast<float *>(q.work + L.diag) : nullptr);
 }
+
+// prologue of a prior_stream call: temp[b] = softplus(mean_t temp_in[b][0][t]) / ln 2 (beta 1, threshold 20, the mean
+// summed in t order), and the call's frame base, length and tensors into the control block
+__global__ void ps_prologue_kernel(Ctl *__restrict__ ctl, const float *__restrict__ temp_in, float *__restrict__ temp,
+                                   const float *uniform, const float *dither, float *out, int B, int T) {
+  const int b = threadIdx.x;
+  if (b < B) {
+    float s = 0.f;
+    for (int t = 0; t < T; ++t) s += temp_in[(size_t)b * T + t];
+    const float m = __fdiv_rn(s, (float)T);
+    const float sp = m > 20.f ? m : log1pf(expf(m));
+    temp[b] = __fdiv_rn(sp, 0.693147180559945309f);
+  }
+  if (b == 0) {
+    ctl->base = ctl->step + 1;
+    ctl->T = T;
+    ctl->uniform = uniform;
+    ctl->dither = dither;
+    ctl->out = out;
+  }
+}
+
+// initial state of a prior_stream: frame 0 is QuantizedNormal.encode(0), class R / 2 in every dim
+__global__ void ps_reset_kernel(int *__restrict__ cls_ring, int B, int K, int D, int R) {
+  const int i = blockIdx.x * PS_THREADS + threadIdx.x;
+  if (i < B * D) cls_ring[(size_t)(i / D) * K * D + i % D] = R / 2;
+}
+
+// checks shared by prior_sample and prior_stream_create; sets the stages' shared-memory limit
+int check_net(const char *who, const float *const *params, int n_layers, int cycle_size, int res_size, int skp_size,
+              int K, int R, int D, int B) {
+  RAVE_CHECK_ARG(B >= 1 && B <= PS_MAX_B, "%s: B = %d, want 1 <= B <= %d", who, B, PS_MAX_B);
+  RAVE_CHECK_ARG(n_layers >= 1 && n_layers <= 64 && cycle_size >= 1 && cycle_size <= 16,
+                 "%s: n_layers %d (1..64), cycle_size %d (1..16)", who, n_layers, cycle_size);
+  RAVE_CHECK_ARG(D >= 1 && res_size >= 1 && skp_size >= 1 && res_size % D == 0 && skp_size % D == 0,
+                 "%s: D = %d must divide res_size %d and skp_size %d", who, D, res_size, skp_size);
+  RAVE_CHECK_ARG(K >= 1 && K <= PS_MAX_K, "%s: kernel_size %d, want 1..%d", who, K, PS_MAX_K);
+  RAVE_CHECK_ARG(R >= 1 && R <= PS_MAX_R, "%s: resolution %d, want 1..%d", who, R, PS_MAX_R);
+  const size_t smem = rows_smem(res_size, K);
+  RAVE_CHECK_ARG(smem <= PS_MAX_SMEM && rows_smem(skp_size, 1) <= PS_MAX_SMEM,
+                 "%s: res_size * kernel_size = %d too large", who, res_size * K);
+  for (int i = 0; i < 2 + 6 * n_layers + 4; ++i) RAVE_CHECK_ARG(params[i], "%s: parameter %d is null", who, i);
+  const size_t smem_max = smem > rows_smem(skp_size, 1) ? smem : rows_smem(skp_size, 1);
+  if (cudaFuncSetAttribute(ps_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("%s: %zu bytes of shared memory refused", who, smem_max);
+    return 2;
+  }
+  return 0;
+}
+
+int check_not_capturing(const char *who, cudaStream_t s) {
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  RAVE_CHECK_ARG(cudaStreamIsCapturing(s, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone,
+                 "%s: the stream is being captured; the call replays its own CUDA graph once per frame, "
+                 "so it cannot run inside a stream capture", who);
+  return 0;
+}
+
+// One frame's launches captured on a private stream (measured faster than enqueueing the stages frame by frame,
+// DESIGN.md §5.8b) and instantiated.
+cudaError_t capture_frame(const Plan &q, cudaGraphExec_t *exec) {
+  cudaStream_t cs = nullptr;
+  cudaGraph_t graph = nullptr;
+  *exec = nullptr;
+  cudaError_t e = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
+  if (e == cudaSuccess) e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
+  if (e == cudaSuccess) {
+    enqueue_frame(q, cs);
+    const cudaError_t el = cudaGetLastError();
+    e = cudaStreamEndCapture(cs, &graph);
+    if (e == cudaSuccess) e = el;
+  }
+  if (e == cudaSuccess) e = cudaGraphInstantiate(exec, graph, 0);
+  if (graph) cudaGraphDestroy(graph);
+  if (cs) cudaStreamDestroy(cs);
+  return e;
+}
+
+// a prior_stream: the plan of its frame graph (parameter pointers copied) and the graph
+struct PriorStream {
+  std::vector<const float *> prm;
+  Plan q;
+  cudaGraphExec_t exec;
+};
 
 }  // namespace
 }  // namespace rave
@@ -391,31 +522,12 @@ extern "C" int rave_prior_sample(const float *const *params, int n_layers, int c
                                  int argmax, int *classes, float *logits, void *work, long work_bytes, void *stream) {
   using namespace rave;
   RAVE_CHECK_ARG(params && prefix && classes && work && (argmax || uniform), "prior_sample: null pointer");
-  RAVE_CHECK_ARG(B >= 1 && B <= PS_MAX_B, "prior_sample: B = %d, want 1 <= B <= %d", B, PS_MAX_B);
-  RAVE_CHECK_ARG(n_layers >= 1 && n_layers <= 64 && cycle_size >= 1 && cycle_size <= 16,
-                 "prior_sample: n_layers %d (1..64), cycle_size %d (1..16)", n_layers, cycle_size);
-  RAVE_CHECK_ARG(D >= 1 && res_size >= 1 && skp_size >= 1 && res_size % D == 0 && skp_size % D == 0,
-                 "prior_sample: D = %d must divide res_size %d and skp_size %d", D, res_size, skp_size);
-  RAVE_CHECK_ARG(K >= 1 && K <= PS_MAX_K, "prior_sample: kernel_size %d, want 1..%d", K, PS_MAX_K);
-  RAVE_CHECK_ARG(R >= 1 && R <= PS_MAX_R, "prior_sample: resolution %d, want 1..%d", R, PS_MAX_R);
   RAVE_CHECK_ARG(P >= 1 && P <= T, "prior_sample: prefix of %d frames for %d frames, want 1 <= P <= T", P, T);
-  const size_t smem = rows_smem(res_size, K);
-  RAVE_CHECK_ARG(smem <= PS_MAX_SMEM && rows_smem(skp_size, 1) <= PS_MAX_SMEM,
-                 "prior_sample: res_size * kernel_size = %d too large", res_size * K);
-  for (int i = 0; i < 2 + 6 * n_layers + 4; ++i) RAVE_CHECK_ARG(params[i], "prior_sample: parameter %d is null", i);
+  if (const int rc = check_net("prior_sample", params, n_layers, cycle_size, res_size, skp_size, K, R, D, B)) return rc;
   const Layout L = layout(B, n_layers, cycle_size, res_size, skp_size, K, D);
   RAVE_CHECK_ARG(work_bytes >= (long)L.total, "prior_sample: workspace of %ld bytes, need %zu", work_bytes, L.total);
   const cudaStream_t s = (cudaStream_t)stream;
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  RAVE_CHECK_ARG(cudaStreamIsCapturing(s, &cap) == cudaSuccess && cap == cudaStreamCaptureStatusNone,
-                 "prior_sample: the stream is being captured; the call captures and replays its own CUDA graph, "
-                 "so it cannot run inside a stream capture");
-  const size_t smem_max = smem > rows_smem(skp_size, 1) ? smem : rows_smem(skp_size, 1);
-  if (cudaFuncSetAttribute(ps_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("prior_sample: %zu bytes of shared memory refused", smem_max);
-    return 2;
-  }
+  if (const int rc = check_not_capturing("prior_sample", s)) return rc;
 
   char *w = static_cast<char *>(work);
   cudaMemsetAsync(w, 0, L.total, s);
@@ -425,30 +537,94 @@ extern "C" int rave_prior_sample(const float *const *params, int n_layers, int c
   if (T == 1) return 0;
   const Plan q{params, n_layers, cycle_size, res_size, skp_size, K, R, D, B, P, T, argmax != 0, prefix, uniform,
                classes, logits, w, L};
-  // Capture one frame on a private stream and replay it on the caller's: measured faster than enqueueing the stages
-  // frame by frame (DESIGN.md §5.8b).
-  cudaStream_t cs = nullptr;
-  cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
-  cudaError_t e = cudaStreamCreateWithFlags(&cs, cudaStreamNonBlocking);
-  if (e == cudaSuccess) e = cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal);
-  if (e == cudaSuccess) {
-    enqueue_frame(q, cs);
-    const cudaError_t el = cudaGetLastError();
-    e = cudaStreamEndCapture(cs, &graph);
-    if (e == cudaSuccess) e = el;
-  }
-  if (e == cudaSuccess) e = cudaGraphInstantiate(&exec, graph, 0);
+  cudaError_t e = capture_frame(q, &exec);
   for (int i = 0; e == cudaSuccess && i < T - 1; ++i) e = cudaGraphLaunch(exec, s);
   if (exec) cudaGraphExecDestroy(exec);
-  if (graph) cudaGraphDestroy(graph);
-  if (cs) cudaStreamDestroy(cs);
   if (e != cudaSuccess) {
     cudaGetLastError();
     set_error("prior_sample: frame graph failed: %s", cudaGetErrorString(e));
     return 2;
   }
   count_launch(T - 1);
+  return 0;
+}
+
+extern "C" long rave_prior_stream_workspace_bytes(int B, int n_layers, int cycle_size, int res_size, int skp_size,
+                                                  int K, int D) {
+  if (B < 1 || n_layers < 1 || n_layers > 64 || cycle_size < 1 || cycle_size > 16 || res_size < 1 || skp_size < 1 ||
+      K < 1 || D < 1)
+    return -1;
+  return (long)rave::stream_layout(B, n_layers, cycle_size, res_size, skp_size, K, D).total;
+}
+
+extern "C" int rave_prior_stream_create(const float *const *params, int n_layers, int cycle_size, int res_size,
+                                        int skp_size, int K, int R, int D, int B, void *work, long work_bytes,
+                                        void **state) {
+  using namespace rave;
+  RAVE_CHECK_ARG(params && work && state, "prior_stream_create: null pointer");
+  if (const int rc = check_net("prior_stream_create", params, n_layers, cycle_size, res_size, skp_size, K, R, D, B))
+    return rc;
+  const Layout L = stream_layout(B, n_layers, cycle_size, res_size, skp_size, K, D);
+  RAVE_CHECK_ARG(work_bytes >= (long)L.total, "prior_stream_create: workspace of %ld bytes, need %zu", work_bytes,
+                 L.total);
+  auto *ps = new PriorStream;
+  ps->prm.assign(params, params + 2 + 6 * n_layers + 4);
+  ps->q = Plan{ps->prm.data(), n_layers, cycle_size, res_size, skp_size, K, R, D, B, 0, 0, 0, nullptr, nullptr,
+               nullptr, nullptr, static_cast<char *>(work), L, true};
+  const cudaError_t e = capture_frame(ps->q, &ps->exec);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    if (ps->exec) cudaGraphExecDestroy(ps->exec);
+    delete ps;
+    set_error("prior_stream_create: frame graph capture failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  *state = ps;
+  return 0;
+}
+
+extern "C" int rave_prior_stream_reset(void *state, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(state, "prior_stream_reset: null state");
+  const Plan &q = static_cast<PriorStream *>(state)->q;
+  const cudaStream_t s = (cudaStream_t)stream;
+  cudaMemsetAsync(q.work, 0, q.L.total, s);
+  ps_reset_kernel<<<blocks_of((long)q.B * q.D), PS_THREADS, 0, s>>>(reinterpret_cast<int *>(q.work + q.L.cls),
+                                                                   q.B, q.K, q.D, q.R);
+  RAVE_CHECK_LAUNCH("prior_stream_reset");
+  return 0;
+}
+
+extern "C" int rave_prior_stream(void *state, const float *temp, const float *uniform, const float *dither, float *out,
+                                 int T, void *stream) {
+  using namespace rave;
+  RAVE_CHECK_ARG(state && temp && uniform && dither && out, "prior_stream: null pointer");
+  RAVE_CHECK_ARG(T >= 1, "prior_stream: T = %d frames, want T >= 1", T);
+  const cudaStream_t s = (cudaStream_t)stream;
+  if (const int rc = check_not_capturing("prior_stream", s)) return rc;
+  const PriorStream *ps = static_cast<PriorStream *>(state);
+  const Plan &q = ps->q;
+  ps_prologue_kernel<<<1, PS_MAX_B, 0, s>>>(reinterpret_cast<Ctl *>(q.work), temp,
+                                             reinterpret_cast<float *>(q.work + q.L.temp), uniform, dither, out, q.B, T);
+  RAVE_CHECK_LAUNCH("prior_stream");
+  cudaError_t e = cudaSuccess;
+  for (int i = 0; e == cudaSuccess && i < T; ++i) e = cudaGraphLaunch(ps->exec, s);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    set_error("prior_stream: frame graph failed: %s", cudaGetErrorString(e));
+    return 2;
+  }
+  count_launch(T);
+  return 0;
+}
+
+extern "C" int rave_prior_stream_destroy(void *state) {
+  auto *ps = static_cast<rave::PriorStream *>(state);
+  if (ps) {
+    cudaGraphExecDestroy(ps->exec);
+    delete ps;
+  }
   return 0;
 }
 

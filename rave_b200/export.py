@@ -9,6 +9,10 @@
   * WasserteinEncoder: encode is the identity; decode appends the noise channels;
   * SphericalEncoder: the `latent_size - 1` hyperspherical angles in [-1, 1) of the raw encoder output; decode maps them
     back to unit vectors.
+With a trained `VariationalPrior` of the model (the export's `--prior`), `prior(temp)` generates the prior's latent
+frame by frame with its state kept from call to call (scripts/export.py TraceModel, csrc/prior_sample.cu), and
+`decode(prior(temp))` plays it.
+
 The latent arithmetic runs on csrc/export.cu.  With `target_sr` (the export's `--sr`), the model runs in a host at
 `target_sr = ratio * sr`: encode resamples its input down to the model's rate first, decode resamples the model's output
 up before the crop (rave_b200/resampler.py, csrc/resample.cu).  Neither call synchronises with the host, so
@@ -59,16 +63,30 @@ class ExportedRAVE(nn.Module):
     channel axis (the reference does this for one example; with a larger batch it slices the batch instead).  Fewer:
     the first channels are kept.  `fidelity`: explained variance that sets `latent_size` of a variational model.
     `target_sr`: the host's sample rate, a multiple of the model's `sr` (ratios 2 and 3 can be built); `sr` becomes
-    `target_sr` and `encode_ratio` counts samples at that rate.
+    `target_sr` and `encode_ratio` counts samples at that rate.  `prior`: a `VariationalPrior` trained on this model
+    (its `synth`), registered as `prior_module`; `prior(temp)` generates from it.
 
     Style transfer of a model with AdaIN layers: set `learn_target`, `learn_source`, `reset_target`, `reset_source`;
     they are applied through `RAVE.update_adain` before `encode` and before a `decode` that `forward` did not call, and
     the two resets clear after each application (scripts/export.py:213-230)."""
 
-    def __init__(self, model, channels: Optional[int] = None, fidelity: float = .95, target_sr: Optional[int] = None):
+    def __init__(self, model, channels: Optional[int] = None, fidelity: float = .95, target_sr: Optional[int] = None,
+                 prior=None):
         super().__init__()
         model.eval()
         self.model = model
+        if prior is not None:
+            from .prior import VariationalPrior
+            if not isinstance(prior, VariationalPrior):
+                raise ValueError(f"prior must be a VariationalPrior, got {prior.__class__.__name__}")
+            if prior.synth is not model:
+                raise ValueError("the prior was not trained on this model (prior.synth is not model)")
+            if prior.latent_size > model.latent_size:
+                raise ValueError(f"the prior's latent_size {prior.latent_size} exceeds the model's {model.latent_size}")
+            self.prior_module = prior.eval()
+        else:
+            self.prior_module = None
+        self._prior_state = None
         self.resampler = None
         if target_sr is not None and target_sr != model.sr:
             if target_sr % model.sr:
@@ -173,6 +191,40 @@ class ExportedRAVE(nn.Module):
         pre_process_latent for the ceil(target_channels / n_channels) B decoded rows (row b r + i is decode i of
         example b): [B r, L - latent_size, T] (variational) or [B r, noise_augmentation, T]."""
         return self._decode(z, noise, from_forward=False)
+
+    @torch.no_grad()
+    def prior(self, temp, uniform: Optional[torch.Tensor] = None, dither: Optional[torch.Tensor] = None):
+        """temp [B, 1, T] -> the prior's next T latent frames [B, D, T] float32 (D = prior.latent_size), continuing the
+        stream the last call left (scripts/export.py TraceModel.forward at a `--streaming` export).  Each row's
+        temperature for the call is softplus(mean_t temp[b, 0, t]) / ln 2 (1 for an input of 0); each step divides the
+        logits by it, draws the class by inverse CDF at `uniform` [B, T, D], decodes it with the dither `dither`
+        [B, T, D] and shifts it diagonally, so dim d lags the newest frame by D - 1 - d frames (0.0 before the first).
+        The draws default to `torch.rand` on the current CUDA generator, uniform first.  The output is in the prior's
+        latent coordinates; `decode` fills the other dimensions.  B <= 64 rows, each with its own state; a call whose B
+        or device differs from the state's raises ValueError until `reset_prior()`."""
+        if self.prior_module is None:
+            raise RuntimeError("this ExportedRAVE was built without a prior")
+        if temp.dim() != 3 or temp.shape[1] != 1:
+            raise ValueError(f"temp has shape {tuple(temp.shape)}, expected [B, 1, T]")
+        pm = self.prior_module
+        params = pm._trained_parameters()
+        B, _, T = temp.shape
+        D, dev = pm.latent_size, params[0].device
+        if self._prior_state is None:
+            if dev.type == "cuda" and torch.cuda.is_current_stream_capturing():
+                raise ops._lib.RaveB200Error("prior: the stream is being captured; the state's frame graph is "
+                                             "captured and replayed by the call, so it cannot run inside a capture")
+            self._prior_state = ops.PriorStream(params, pm.cycle_size, B, pm.quantized_normal.resolution, D)
+        elif (self._prior_state.B, self._prior_state.device) != (B, dev):
+            raise ValueError(f"the prior's state has {self._prior_state.B} rows on {self._prior_state.device}, the call "
+                             f"{B} on {dev}: call reset_prior() first")
+        uniform = torch.rand(B, T, D, device=dev) if uniform is None else self._draw(uniform, (B, T, D), dev, "uniform")
+        dither = torch.rand(B, T, D, device=dev) if dither is None else self._draw(dither, (B, T, D), dev, "dither")
+        return self._prior_state(params, temp.to(device=dev, dtype=torch.float32), uniform, dither)
+
+    def reset_prior(self):
+        """Return the prior's generation to its initial state (next call starts a new stream, at any B)."""
+        self._prior_state = None
 
     @torch.no_grad()
     def forward(self, x, eps: Optional[torch.Tensor] = None, noise: Optional[torch.Tensor] = None):

@@ -1540,6 +1540,64 @@ def prior_classes_to_latent(classes, dither, noise, latent_pca, latent_mean, R):
     return z
 
 
+class PriorStream:
+    """Generation state of the prior kept from call to call (rave_prior_stream_* of csrc/prior_sample.cu), for B rows on
+    the device of `params`, the fp32 parameter tensors in Prior._trained_parameters order.  The workspace is a tensor
+    owned here and starts in the initial state; the library keeps one captured frame graph that reads the parameters
+    where they were at capture, so a call whose parameters have moved re-captures it.  `captures` counts the captures."""
+
+    def __init__(self, params, dilation_cycle, B, R, D):
+        self.cycle, self.B, self.R, self.D = dilation_cycle, B, R, D
+        self.n_layers = (len(params) - 6) // 6
+        self.C, _, self.K = params[0].shape
+        self.Sk = params[-4].shape[0]
+        nbytes = int(_lib.load().rave_prior_stream_workspace_bytes(B, self.n_layers, self.cycle, self.C, self.Sk,
+                                                                   self.K, D))
+        if nbytes < 0:
+            raise _lib.RaveB200Error(f"prior_stream: bad shape (B {B}, {self.n_layers} layers, C {self.C}, "
+                                     f"Sk {self.Sk}, K {self.K}, D {D})")
+        self.device = params[0].device
+        self.work = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+        self.captures = 0
+        self._handle = None
+        self._capture(params)
+        call("rave_prior_stream_reset", self._handle, stream_ptr())
+
+    def _capture(self, params):
+        import ctypes
+        for p in params:
+            if p.dtype != torch.float32 or not p.is_contiguous() or p.device != self.device:
+                raise _lib.RaveB200Error(f"prior_stream: the prior's parameters must be contiguous float32 tensors on "
+                                         f"{self.device}")
+        self._destroy()
+        self.params = list(params)          # held so that the captured pointers stay valid
+        self._ptrs = [p.data_ptr() for p in params]
+        arr = (ctypes.c_void_p * len(self._ptrs))(*self._ptrs)
+        h = ctypes.c_void_p()
+        call("rave_prior_stream_create", arr, self.n_layers, self.cycle, self.C, self.Sk, self.K, self.R, self.D,
+             self.B, ptr(self.work), self.work.numel(), ctypes.byref(h))
+        self._handle = h.value
+        self.captures += 1
+
+    def _destroy(self):
+        if self._handle is not None:
+            _lib.load().rave_prior_stream_destroy(self._handle)
+            self._handle = None
+
+    def __del__(self):
+        self._destroy()
+
+    def __call__(self, params, temp, uniform, dither):
+        """The next T frames [B, D, T] float32 for temp [B, 1, T] and the draws uniform / dither [B, T, D]."""
+        if [p.data_ptr() for p in params] != self._ptrs:
+            self._capture(params)
+        B, _, T = temp.shape
+        out = torch.empty(B, self.D, T, dtype=torch.float32, device=self.device)
+        call("rave_prior_stream", self._handle, ptr(_f32c(temp)), ptr(_f32c(uniform)), ptr(_f32c(dither)), ptr(out),
+             T, stream_ptr())
+        return out
+
+
 # ----------------------------------------------------------------------------------------------
 # The exported model's compact latent (csrc/export.cu, rave_b200/export.py)
 # ----------------------------------------------------------------------------------------------
